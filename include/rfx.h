@@ -167,6 +167,11 @@ typedef struct rfx_hbao_params {
   float ao_distance, distance_power, bias, thickness;
   int32_t spp;
   int32_t blue_noise_index;
+  /* read by rfx_hbao_launch_ex only (rfx_hbao_launch reads the fields above, so callers of the shorter struct keep working): */
+  float view_matrix[16];     /* camera.matrixWorldInverse: turns the normal plane's view-space normals to world space
+                                (hbao_utils.glsl:70-79); used only with a normal plane                            */
+  float resolution[2];       /* uniform resolution = the AO target's UNROUNDED size (width * resolutionScale, ...;
+                                AOPass.js:79-83); {0, 0}: the out plane's size                                    */
 } rfx_hbao_params;
 
 /* K7  AO compose   src/ao/shader/ao_compose.frag:6-16 */
@@ -303,7 +308,8 @@ rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_t
                                          uint32_t row0, uint32_t row1);
 
 /* K3. gbuffer_or_normal: packed gBuffer (gbuffer_texture=1) or velocity-layout plane.
- * in: RGBA32F or RGBA16F; out: RGBA16F. */
+ * in: RGBA32F or RGBA16F; out: RGBA16F.  With input_linear set, in0/in1 (one size) may differ in size from out: they are
+ * sampled by uv (the AO denoiser's first pass upsamples a reduced-resolution AO target); NEAREST inputs have out's size. */
 rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p,
                                       const rfx_plane* depth, const rfx_plane* gbuffer_or_normal,
                                       const rfx_plane* in0, const rfx_plane* in1,
@@ -334,12 +340,21 @@ rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_co
                                    const rfx_plane* gi, const rfx_plane* scene,
                                    const rfx_plane* out, uint32_t row0, uint32_t row1);
 
-/* K6. out RGBA16F (rgb = world normal, a = ao); background pixels are not written. */
+/* K6. out RGBA16F (rgb = world normal, a = ao); background pixels are not written.  `out` may be smaller than `depth`
+ * (AOEffect's resolutionScale < 1: the AO target is (int)(width * scale) x (int)(height * scale), src/ao/AOEffect.js:126-146),
+ * never larger: its pixels fetch depth NEAREST by uv and rebuild the normal in depth texels.
+ * rfx_hbao_launch = rfx_hbao_launch_ex with normal = NULL and resolution {0, 0}. */
 rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
                            const rfx_plane* depth, const rfx_plane* out,
                            uint32_t row0, uint32_t row1);
+/* normal: NULL (the normal is rebuilt from 9 depth taps) or an RGBA8 plane of any size holding the VIEW-space normal packed as
+ * rgb = n * 0.5 + 0.5 (postprocessing's NormalPass target), sampled NEAREST by uv: AOEffect's useNormalPass / normalTexture
+ * (src/ao/AOEffect.js:48-55, hbao_utils.glsl:70-79). */
+rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
+                              const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
+                              uint32_t row0, uint32_t row1);
 
-/* K7. ao RGBA16F (.a), input/out RGBA16F */
+/* K7. ao RGBA16F (.a; any size: sampled LINEAR by uv, e.g. a reduced-resolution AO target), input/out RGBA16F */
 rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p,
                                  const rfx_plane* depth, const rfx_plane* ao,
                                  const rfx_plane* input, const rfx_plane* out,

@@ -345,47 +345,74 @@ export const defaultAOOptions = { resolutionScale: 1, spp: 8, distance: 2, dista
 
 export class HBAOEffect {
 	// new HBAOEffect(composer, camera, scene, options) — src/hbao/HBAOEffect.js:5-20 + src/ao/AOEffect.js:23-178
+	// resolutionScale (0, 1]: the AO pass renders to trunc(width * scale) x trunc(height * scale) with the unrounded product as `resolution`,
+	// the denoiser stays at full size (AOEffect.setSize :126-146).  normalTexture (an RGBA8 render target of view-space normals, NormalPass
+	// layout) or useNormalPass (the host's NormalPass target, scene.normalRenderTarget) replaces the depth-rebuilt normal; chosen here, like
+	// the reference (:48-55).
 	constructor(composer, camera, scene, options = defaultAOOptions) {
 		this.composer = composer; this._camera = camera; this._scene = scene
 		const opts = { ...defaultAOOptions, ...options }
+		checkAoScale(opts.resolutionScale)
 		this._options = opts
 		this.ctx = context(); this.index = new BlueNoiseIndex(options.blueNoiseStart)
 		this.velocityDepthNormalPass = opts.velocityDepthNormalPass
-		reactive(this, opts, key => { if (key === "resolutionScale") this.setSize(this.width, this.height) })
+		this.normalTarget = opts.normalTexture ?? (opts.useNormalPass ? scene?.normalRenderTarget : null)
+		if (opts.useNormalPass && !this.normalTarget) throw new Error("HBAOEffect: useNormalPass needs the host's NormalPass target as scene.normalRenderTarget")
+		this.lastSize = { width: 0, height: 0, resolutionScale: 0 }
+		reactive(this, opts, key => { if (key === "resolutionScale") { checkAoScale(opts.resolutionScale); this.setSize(this.lastSize.width, this.lastSize.height) } })
 		this.setSize(options.width ?? composer?.inputBuffer?.width, options.height ?? composer?.inputBuffer?.height)
 	}
 	setSize(width, height) {
-		if (width === undefined) return
+		if (width === undefined || height === undefined) return
+		const s = this.resolutionScale
+		if (width === this.lastSize.width && height === this.lastSize.height && s === this.lastSize.resolutionScale) return
 		this.dispose()
 		this.width = width; this.height = height
-		this.aoPlane = rfx.planeAlloc(this.ctx, FMT.RGBA16F, width, height)
+		this.aoWidth = Math.trunc(width * s); this.aoHeight = Math.trunc(height * s)
+		this.resolution = [width * s, height * s]   // AOPass.js:79-83: renderTarget.width / height as three stores them
+		this.aoPlane = rfx.planeAlloc(this.ctx, FMT.RGBA16F, this.aoWidth, this.aoHeight)
 		this.outputPlane = rfx.planeAlloc(this.ctx, FMT.RGBA16F, width, height)
 		this.outputHost = new Uint16Array(4 * width * height)
 		this.planeSource = new ReadbackPlaneSource(this.ctx, width, height)
+		if (this.normalTarget) {
+			this.normalW = this.normalTarget.width ?? width; this.normalH = this.normalTarget.height ?? height
+			this.normalPlane = rfx.planeAlloc(this.ctx, FMT.RGBA8, this.normalW, this.normalH)
+			this.normalHost = new Uint8Array(4 * this.normalW * this.normalH)
+		}
 		this.denoise = new PoissonDenoisePass(this._camera, [this.aoPlane], { ...this._options, normalPhi: 3.25, depthPhi: 2 })
 		this.denoise.setSize(width, height)
+		this.lastSize = { width, height, resolutionScale: s }
 	}
-	get texture() { return this.denoise.texture[0] }
+	// AOEffect.js:148-154: with no denoise iteration the compose reads the AO target itself
+	get texture() { return this._options.iterations > 0 ? this.denoise.texture[0] : this.aoPlane }
 	initialize() {}
 	// update(renderer, inputBuffer, deltaTime) — src/ao/AOEffect.js:126-178 + src/ao/AOPass.js:85-110
 	update(renderer, inputBuffer) {
 		const cam = cameraBlock(this._camera)
 		const pv = this._camera.projectionMatrix.clone().multiply(this._camera.matrixWorldInverse)
 		const planes = this.planeSource.read(renderer, { depth: this.composer.depthRenderTarget, velocity: this.velocityDepthNormalPass?.renderTarget, directLight: inputBuffer })
-		rfx.hbao(this.ctx, { projectionView: f32(pv), projectionInverse: cam.projectionInverse, matrixWorld: cam.matrixWorld, aoDistance: this.distance,
-			distancePower: this.distancePower, bias: this.bias, thickness: this.thickness, spp: this.spp, blueNoiseIndex: this.index.value }, planes.depth, this.aoPlane)
+		if (this.normalPlane) {
+			renderer.readRenderTargetPixels(this.normalTarget, 0, 0, this.normalW, this.normalH, this.normalHost)
+			rfx.planeUpload(this.ctx, this.normalPlane, this.normalHost)
+		}
+		rfx.hbao(this.ctx, { projectionView: f32(pv), projectionInverse: cam.projectionInverse, matrixWorld: cam.matrixWorld, viewMatrix: f32(this._camera.matrixWorldInverse),
+			resolution: this.resolution, aoDistance: this.distance, distancePower: this.distancePower, bias: this.bias, thickness: this.thickness, spp: this.spp,
+			blueNoiseIndex: this.index.value }, planes.depth, this.aoPlane, this.normalPlane ?? null)
 		this.denoise.depthPlane = planes.depth; this.denoise.gbufferPlane = planes.velocity; this.denoise.gbufferTexture = false
 		this.denoise.options.inputLinear = true
 		this.denoise.iterations = this._options.iterations
 		this.denoise.render()
-		rfx.aoCompose(this.ctx, { power: this.power, color: this.color }, planes.depth, this.denoise.texture[0], planes.directLight, this.outputPlane)   // ao_compose.frag:6-16
+		rfx.aoCompose(this.ctx, { power: this.power, color: this.color }, planes.depth, this.texture, planes.directLight, this.outputPlane)   // ao_compose.frag:6-16
 		rfx.planeDownload(this.ctx, this.outputPlane, this.outputHost)
 	}
 	get outputTexture() { return this.outputHost }
 	dispose() {
-		for (const k of ["aoPlane", "outputPlane"]) if (this[k]) { rfx.planeFree(this.ctx, this[k]); this[k] = null }
+		for (const k of ["aoPlane", "outputPlane", "normalPlane"]) if (this[k]) { rfx.planeFree(this.ctx, this[k]); this[k] = null }
 		this.planeSource?.dispose(); this.denoise?.dispose()
 	}
+}
+function checkAoScale(s) {
+	if (!(typeof s === "number" && s > 0 && s <= 1)) throw new RangeError(`HBAOEffect: resolutionScale must lie in (0, 1], got ${s}`)
 }
 HBAOEffect.DefaultOptions = defaultAOOptions
 

@@ -289,15 +289,17 @@ napi_value GiCompose(napi_env env, napi_callback_info info) {  // giCompose(ctx,
                                  unwrap<rfx_plane>(env, argv[6]), unwrap<rfx_plane>(env, argv[7]), 0, 0), "rfx_gi_compose_launch");
   return undefined(env);
 }
-napi_value Hbao(napi_env env, napi_callback_info info) {  // hbao(ctx, params, depth, out)
-  ARGS(4); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+napi_value Hbao(napi_env env, napi_callback_info info) {  // hbao(ctx, params, depth, out[, normal]); params.viewMatrix (with a normal plane), params.resolution
+  ARGS(5); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
   Obj b{env, argv[1]};
   rfx_hbao_params p{};
   if (!b.f32("projectionView", p.projection_view, 16) || !b.f32("projectionInverse", p.projection_inverse, 16) || !b.f32("matrixWorld", p.camera_matrix_world, 16)) {
     napi_throw_type_error(env, nullptr, "hbao: projectionView / projectionInverse / matrixWorld"); return nullptr; }
   p.ao_distance = (float)b.num("aoDistance", 2); p.distance_power = (float)b.num("distancePower", 1); p.bias = (float)b.num("bias", 40); p.thickness = (float)b.num("thickness", 0.075);
   p.spp = (int32_t)b.num("spp", 8); p.blue_noise_index = (int32_t)b.num("blueNoiseIndex", 1);
-  CHECK(c, rfx_hbao_launch(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), 0, 0), "rfx_hbao_launch");
+  b.floats("viewMatrix", p.view_matrix, 16); b.floats("resolution", p.resolution, 2);  // absent: unused / {0, 0} = the out plane's size
+  CHECK(c, rfx_hbao_launch_ex(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[4]), unwrap<rfx_plane>(env, argv[3]), 0, 0),
+        "rfx_hbao_launch_ex");
   return undefined(env);
 }
 napi_value AoCompose(napi_env env, napi_callback_info info) {  // aoCompose(ctx, {power, color}, depth, ao, input, out)

@@ -166,8 +166,8 @@ RFX_D float flum(v3 c2) { return ex2a(fma_(0.125f, lg2a(dot(mk3(0.2125f, 0.7154f
 
 template <bool LINEAR>
 RFX_D void fetch2(const PoissonArgs& a, v2 uv, bool two, v3& c0, v3& c1, float* alpha0 = nullptr, float* alpha1 = nullptr) {
-  if (LINEAR) {  // RGBA16F + LinearFilter: one bilinear setup shared by both planes
-    const Bilin b = bilin_setup(uv, a.W, a.H);
+  if (LINEAR) {  // RGBA16F + LinearFilter: one bilinear setup shared by both planes, in texels of the input (it may be smaller than the output)
+    const Bilin b = bilin_setup(uv, a.in0.w, a.in0.h);
     {
       const v4 t00 = ld_h4(a.in0, b.x0, b.y0), t10 = ld_h4(a.in0, b.x1, b.y0), t01 = ld_h4(a.in0, b.x0, b.y1), t11 = ld_h4(a.in0, b.x1, b.y1);
       c0 = mk3(bilin_blend(b, t00.x, t10.x, t01.x, t11.x), bilin_blend(b, t00.y, t10.y, t01.y, t11.y), bilin_blend(b, t00.z, t10.z, t01.z, t11.z));

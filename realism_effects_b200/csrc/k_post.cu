@@ -15,21 +15,30 @@ RFX_D v3 hbao_world_pos(const HbaoArgs& a, float depth, v2 coord) {  // hbao_uti
   return xyz(ws) / ws.w;
 }
 
+// GENERAL = false: the target has the depth plane's size, `resolution` is that size and the normal is rebuilt from depth, so the
+// pixel itself addresses the depth texel and the blue noise.  GENERAL = true: the target may be smaller than the depth plane
+// (AOEffect.setSize scales the AO pass by resolutionScale, src/ao/AOEffect.js:126-146) and `resolution` may be fractional; the
+// depth is fetched NEAREST by uv, the blue-noise pixel is ivec2(vUv * resolution) and the normal may come from a normal texture.
+template <bool GENERAL>
 __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.W || y >= a.row1) return;
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
-  const float depth = ld_r32f(a.depth, x, y);
+  const float depth = GENERAL ? tex_r32f_nearest(a.depth, vUv) : ld_r32f(a.depth, x, y);
   if (depth == 1.0f) return;  // discard: target keeps its texel
   const v4 cp = mul(a.camera_matrix_world, mk4(0.0f, 0.0f, 0.0f, 1.0f));
   const v3 cameraPosition = xyz(cp);
   const v3 worldPos = hbao_world_pos(a, depth, vUv);
-  // computeWorldNormal  hbao_utils.glsl:46-68 (texelFetch clamps at the border)
   v3 worldNormal;
-  {
-    const float sx = (float)a.W, sy = (float)a.H;
+  if (GENERAL && a.normal.p) {  // useNormalTexture  hbao_utils.glsl:70-79: RGBA8 NEAREST, unpackRGBToNormal, (vec4(n, 1.) * viewMatrix).xyz
+    const uchar4 t = __ldg((const uchar4*)(a.normal.p + pv_off(a.normal, nearest_i(vUv.x, a.normal.w), nearest_i(vUv.y, a.normal.h), 4)));
+    const v3 n = mk3(2.0f * ((float)t.x / 255.0f) - 1.0f, 2.0f * ((float)t.y / 255.0f) - 1.0f, 2.0f * ((float)t.z / 255.0f) - 1.0f);
+    worldNormal = normalize(xyz(mul(mk4(n, 1.0f), a.view_matrix)));
+  } else {  // computeWorldNormal  hbao_utils.glsl:46-68: in depth texels (textureSize(depthTexture)); texelFetch clamps at the border
+    const int DW = a.depth.w, DH = a.depth.h;
+    const float sx = (float)DW, sy = (float)DH;
     const int ix = (int)(vUv.x * sx), iy = (int)(vUv.y * sy);
-    auto D = [&](int dx, int dy) { return ld_r32f(a.depth, clampi(ix + dx, a.W), clampi(iy + dy, a.H)); };
+    auto D = [&](int dx, int dy) { return ld_r32f(a.depth, clampi(ix + dx, DW), clampi(iy + dy, DH)); };
     const float c0 = D(0, 0), l2 = D(-2, 0), l1 = D(-1, 0), r1 = D(1, 0), r2 = D(2, 0), b2 = D(0, -2), b1 = D(0, -1), t1 = D(0, 1), t2 = D(0, 2);
     const float dl = fabsf((2.0f * l1 - l2) - c0), dr = fabsf((2.0f * r1 - r2) - c0);
     const float db = fabsf((2.0f * b1 - b2) - c0), dt = fabsf((2.0f * t1 - t2) - c0);
@@ -41,7 +50,8 @@ __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoA
   // getOcclusion: blueNoise() is re-evaluated with the same index for every sample (A9), so the
   // `spp` samples are identical; the loop is kept (it is what the shader executes) but the sample
   // itself is computed once.
-  const uchar4 bn = __ldg(a.blue.tex + ((y + a.blue.shift.sy) % a.blue.size) * a.blue.size + ((x + a.blue.shift.sx) % a.blue.size));
+  const int bx = GENERAL ? (int)(vUv.x * a.res_x) : x, by = GENERAL ? (int)(vUv.y * a.res_y) : y;  // ivec2(vUv * resolution)
+  const uchar4 bn = __ldg(a.blue.tex + ((by + a.blue.shift.sy) % a.blue.size) * a.blue.size + ((bx + a.blue.shift.sx) % a.blue.size));
   const float2 sc = __ldg(a.rot_table + bn.y);
   const float ux = (float)bn.x / 255.0f, bz = (float)bn.z / 255.0f;
   v3 sampleWorldDir;
@@ -77,7 +87,8 @@ __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoA
 }
 cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
-  hbao_kernel<<<grid, 256, 0, s>>>(a);
+  if (a.general) hbao_kernel<true><<<grid, 256, 0, s>>>(a);
+  else hbao_kernel<false><<<grid, 256, 0, s>>>(a);
   return cudaGetLastError();
 }
 

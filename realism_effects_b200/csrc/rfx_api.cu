@@ -568,8 +568,10 @@ rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_pois
   }
   if (p->input_linear && !a.in_half) return fail(ctx, RFX_ERR_UNSUPPORTED, "poisson: LINEAR inputs must be RGBA16F");
   a.W = (int)out0->width; a.H = (int)out0->height;
-  if (a.depth.w != a.W || a.depth.h != a.H || a.gb.w != a.W || a.gb.h != a.H || a.in0.w != a.W || a.in0.h != a.H)
+  if (a.depth.w != a.W || a.depth.h != a.H || a.gb.w != a.W || a.gb.h != a.H || a.in1.w != a.in0.w || a.in1.h != a.in0.h)
     return fail(ctx, RFX_ERR_SIZE_MISMATCH, "poisson: plane sizes differ");
+  // LINEAR inputs are sampled by uv and may have any size (the AO denoiser's first pass reads a reduced-resolution AO target)
+  if (!p->input_linear && (a.in0.w != a.W || a.in0.h != a.H)) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "poisson: NEAREST inputs must have the output's size");
   if (out0->ptr == in0->ptr || (out1 && in1 && out1->ptr == in1->ptr)) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: in-place filtering is not allowed");
   rows(row0, row1, out0->height, a.row0, a.row1);
   set_segs(ctx, a.row0, a.row1, a.segs);
@@ -657,17 +659,26 @@ rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_co
   return RFX_OK;
 }
 
-rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
+                              uint32_t row0, uint32_t row1) {
   if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: null argument");
   HbaoArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !ov(out, RFX_FMT_RGBA16F, a.out)) return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao: depth R32F, out RGBA16F required");
+  if (normal && !pv(normal, RFX_FMT_RGBA8, a.normal)) return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao: the normal plane must be RGBA8");
   a.W = (int)out->width; a.H = (int)out->height;
-  if (a.depth.w != a.W || a.depth.h != a.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "hbao: plane sizes differ");
+  if (a.W > a.depth.w || a.H > a.depth.h)
+    return fail(ctx, RFX_ERR_SIZE_MISMATCH, "hbao: the output may be smaller than the depth plane (resolutionScale <= 1), not larger");
   if (p->spp < 0) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: spp < 0");
+  const bool res_default = p->resolution[0] == 0.0f && p->resolution[1] == 0.0f;
+  if (!res_default && !(p->resolution[0] > 0.0f && p->resolution[1] > 0.0f)) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: resolution must be positive or {0, 0}");
+  a.res_x = res_default ? (float)a.W : p->resolution[0];
+  a.res_y = res_default ? (float)a.H : p->resolution[1];
+  a.general = a.W != a.depth.w || a.H != a.depth.h || a.normal.p || a.res_x != (float)a.W || a.res_y != (float)a.H;
   rows(row0, row1, out->height, a.row0, a.row1);
   memcpy(a.projection_view.m, p->projection_view, 64);
   memcpy(a.projection_inverse.m, p->projection_inverse, 64);
   memcpy(a.camera_matrix_world.m, p->camera_matrix_world, 64);
+  memcpy(a.view_matrix.m, p->view_matrix, 64);
   a.ao_distance = p->ao_distance; a.distance_power = p->distance_power; a.bias = p->bias; a.thickness = p->thickness; a.spp = p->spp;
   rfx_status st = blue_for(ctx, p->blue_noise_index, a.blue);
   if (st != RFX_OK) return st;
@@ -677,6 +688,13 @@ rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
   return RFX_OK;
 }
 
+rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  if (!ctx || !p) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: null argument");
+  rfx_hbao_params q{};  // the fields before view_matrix only: callers built against the shorter struct pass no more than those
+  memcpy(&q, p, offsetof(rfx_hbao_params, view_matrix));
+  return rfx_hbao_launch_ex(ctx, stream, &q, depth, nullptr, out, row0, row1);
+}
+
 rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p, const rfx_plane* depth, const rfx_plane* ao,
                                  const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1) {
   if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_compose: null argument");
@@ -684,7 +702,8 @@ rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compos
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(ao, RFX_FMT_RGBA16F, a.ao) || !pv(input, RFX_FMT_RGBA16F, a.input) || !ov(out, RFX_FMT_RGBA16F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "ao_compose: depth R32F, ao/input/out RGBA16F required");
   a.W = (int)out->width; a.H = (int)out->height;
-  if (a.depth.w != a.W || a.depth.h != a.H || a.ao.w != a.W || a.input.w != a.W) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ao_compose: plane sizes differ");
+  // `ao` is sampled LINEAR by uv: any size (a reduced-resolution AO target when the denoiser runs no iteration, AOEffect.js:148-154)
+  if (a.depth.w != a.W || a.depth.h != a.H || a.input.w != a.W || a.input.h != a.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ao_compose: depth / input / out sizes differ");
   rows(row0, row1, out->height, a.row0, a.row1);
   a.power = p->power;
   memcpy(a.color, p->color, 12);

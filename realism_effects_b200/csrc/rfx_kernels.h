@@ -161,9 +161,13 @@ cudaError_t launch_viewz(const SsgiArgs& a, OutV vz, cudaStream_t s);
 // ---- K6 / K7 / K8 / K9 -----------------------------------------------------------------------
 struct HbaoArgs {
   PV depth;
+  PV normal;  // RGBA8 view-space normal (NormalPass layout) or p == nullptr: rebuilt from depth
   OutV out;
   int W, H, row0, row1;
   M4 projection_view, projection_inverse, camera_matrix_world;
+  M4 view_matrix;       // normal texture only
+  float res_x, res_y;   // uniform `resolution` (the target's unrounded size)
+  int general;          // scaled target, a `resolution` other than W x H or a normal texture: hbao_kernel<true>
   float ao_distance, distance_power, bias, thickness;
   int spp;
   BlueD blue;

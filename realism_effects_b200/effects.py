@@ -443,7 +443,12 @@ class PoissonDenoisePass:
 class HBAOEffect(_Reactive):
     """new HBAOEffect(composer, camera, scene, options)  (src/hbao/HBAOEffect.js:5-20, src/ao/AOEffect.js:23-178).
     The reference class does not compile at its pinned commit (SURVEY.md D3); this is hbao.frag + the 1-plane
-    velocity-layout Poisson denoise + ao_compose.frag, the wiring the shaders are written for."""
+    velocity-layout Poisson denoise + ao_compose.frag, the wiring the shaders are written for.
+
+    resolutionScale (0, 1]: the AO pass renders to (int)(width * scale) x (int)(height * scale); the denoiser and the compose stay at
+    full size and upsample it LINEAR (AOEffect.setSize :126-146).  normalTexture (an RGBA8 view-space normal plane) or useNormalPass
+    (the host's NormalPass output, `scene.normal`) replaces the normal K6 rebuilds from depth; like the reference this is chosen at
+    construction (:48-55)."""
 
     DefaultOptions = defaultAOOptions
 
@@ -453,17 +458,48 @@ class HBAOEffect(_Reactive):
         self.blueNoiseIndex = BlueNoiseIndex((options or {}).get("blueNoiseStart", 1234567))
         o = {**defaultAOOptions, **(options or {})}
         o.pop("blueNoiseStart", None)
+        _check_ao_scale(o["resolutionScale"])
+        self._normal = o["normalTexture"]
+        if self._normal is None and o["useNormalPass"]:
+            self._normal = getattr(scene, "normal", None)
+            if self._normal is None:
+                raise abi.RfxError("HBAOEffect: useNormalPass needs the host's NormalPass output as scene.normal (RGBA8 view-space normals)")
+        if self._normal is not None and self._normal.format != abi.FMT_RGBA8:
+            raise abi.RfxError("HBAOEffect: the normal texture must be an RGBA8 plane (NormalPass layout)")
         self.aoTarget = self.ctx.alloc(abi.FMT_RGBA16F, composer.width, composer.height)
         self.PoissonDenoisePass = PoissonDenoisePass(camera, [self.aoTarget], dict(iterations=o["iterations"], radius=o["radius"], phi=o["phi"],
                                                                                     lumaPhi=o["lumaPhi"], depthPhi=o["depthPhi"],
                                                                                     normalPhi=o["normalPhi"], inputType="diffuse"))
         self._options = o
+        self._resolution = (0.0, 0.0)  # {0, 0}: the AO target's own size
+        self._lastSize = (composer.width, composer.height, 1)
+        self.setSize(composer.width, composer.height)
+
+    def __setattr__(self, k, v):
+        if k == "resolutionScale":
+            _check_ao_scale(v)
+        super().__setattr__(k, v)
+
+    def setSize(self, width, height):
+        """AOEffect.setSize: a no-op when the size and the scale are unchanged; the AO target gets (int)(width * scale) x
+        (int)(height * scale) and the unrounded product as its `resolution` (AOPass.js:79-83), the Poisson targets the full size"""
+        s = self._options["resolutionScale"]
+        if (width, height, s) == self._lastSize:
+            return
+        self.aoTarget.free()
+        self.aoTarget = self.ctx.alloc(abi.FMT_RGBA16F, int(width * s), int(height * s))
+        self._resolution = (width * s, height * s)
+        self.PoissonDenoisePass.textures = [self.aoTarget]
+        self.PoissonDenoisePass.setSize(width, height)
+        self._lastSize = (width, height, s)
 
     def _option_changed(self, k):
         if k in ("iterations", "radius", "phi"):
             setattr(self.PoissonDenoisePass, k, self._options[k])
         elif k in ("lumaPhi", "depthPhi", "normalPhi"):
             setattr(self.PoissonDenoisePass, k, max(self._options[k], 0.0001))  # AOEffect.js:107-111
+        elif k == "resolutionScale":
+            self.setSize(*self._lastSize[:2])
 
     @property
     def texture(self):
@@ -477,9 +513,11 @@ class HBAOEffect(_Reactive):
         abi.set_f16(p.projection_view, np.ascontiguousarray((P @ V).T.reshape(16)).astype(np.float32))  # AOPass.js:93-96
         abi.set_f16(p.projection_inverse, cam_u["projection_inverse"])
         abi.set_f16(p.camera_matrix_world, cam_u["camera_matrix_world"])
+        abi.set_f16(p.view_matrix, cam_u["view_matrix"])
+        p.resolution[:] = [float(self._resolution[0]), float(self._resolution[1])]
         p.ao_distance, p.distance_power, p.bias, p.thickness = o["distance"], o["distancePower"], o["bias"], o["thickness"]
         p.spp, p.blue_noise_index = int(o["spp"]), self.blueNoiseIndex.value
-        self.ctx.hbao(p, self._scene.depth, self.aoTarget)
+        self.ctx.hbao(p, self._scene.depth, self.aoTarget, normal=self._normal)
         self.PoissonDenoisePass.setGBufferPass(self._scene.velocity, self._scene.depth, is_gbuffer=False)
         self.PoissonDenoisePass.render(renderer)
         if inputBuffer is not None and getattr(self.composer, "outputBuffer", None) is not None:
@@ -491,6 +529,11 @@ class HBAOEffect(_Reactive):
     def dispose(self):
         self.PoissonDenoisePass.dispose()
         self.aoTarget.free()
+
+
+def _check_ao_scale(s):
+    if not (isinstance(s, (int, float)) and 0.0 < s <= 1.0):
+        raise abi.RfxError(f"HBAOEffect: resolutionScale must lie in (0, 1], got {s!r}")
 
 
 # ---------------------------------------------------------------------------------------------------

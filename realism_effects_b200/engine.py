@@ -191,8 +191,10 @@ class Context:
         self._chk(self.lib.rfx_ssgi_compose_launch(self.h, stream, C.byref(params) if params is not None else None, _r(depth), _r(gi), _r(scene), _r(out),
                                                    rows[0], rows[1]))
 
-    def hbao(self, p, depth, out, rows=(0, 0), stream=None):
-        self._chk(self.lib.rfx_hbao_launch(self.h, stream, C.byref(p), _r(depth), _r(out), rows[0], rows[1]))
+    def hbao(self, p, depth, out, rows=(0, 0), stream=None, normal=None):
+        """out may be smaller than depth (AO resolutionScale; p.resolution = its unrounded size, {0, 0} = out's size);
+        normal: RGBA8 view-space normal plane (NormalPass layout, p.view_matrix turns it to world space) or None"""
+        self._chk(self.lib.rfx_hbao_launch_ex(self.h, stream, C.byref(p), _r(depth), _r(normal), _r(out), rows[0], rows[1]))
 
     def ao_compose(self, p, depth, ao, inp, out, rows=(0, 0), stream=None):
         self._chk(self.lib.rfx_ao_compose_launch(self.h, stream, C.byref(p), _r(depth), _r(ao), _r(inp), _r(out), rows[0], rows[1]))
