@@ -435,7 +435,7 @@ rfx_status rfx_ssgi_chain_reset(rfx_ssgi_chain* chain);
 rfx_status rfx_ssgi_chain_set_options(rfx_ssgi_chain* chain, const rfx_ssgi_chain_options* opt);
 rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame);
 /* Row-block sharded frame (SURVEY.md §8e): ranges[2k], ranges[2k+1] = output rows [a,b) of launch k in chain order
- * (K1, K2, K3 pass 0..2*denoiseIterations-1, K4).  The caller (realism_effects_b200/parallel.py) sizes
+ * (K1, K2, K3 pass 0..2*denoiseIterations-1, K4, and the TRAA tail as one more launch when it is on).  The caller (realism_effects_b200/parallel.py) sizes
  * the ranges so that every pass finds valid halo rows produced locally by the previous pass, then all-gathers the
  * produced-then-gathered planes (composed, dnB[0..1]) across ranks.  Results are bit-identical to rfx_ssgi_chain_render. */
 rfx_status rfx_ssgi_chain_render_ranges(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame, const uint32_t* ranges,
@@ -452,7 +452,30 @@ rfx_status rfx_ssgi_chain_render_blocks(rfx_ssgi_chain* chain, void* stream, con
  * in order 0, 1, 2 with the same frame and ranges.  ranges == NULL: whole planes (n_launches / n_blocks ignored). */
 rfx_status rfx_ssgi_chain_render_part(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame, const uint32_t* ranges,
                                       uint32_t n_launches, uint32_t n_blocks, uint32_t part);
-/* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1] */
+/* TRAA frame tail: the second EffectPass of the reference demo's SSGI + TRAA frame (example/main.js:525-532) rendered by the chain
+ * after K4 on every frame:  K5 ssgi_compose (of `composed`, depth and frame->direct_light, the composer input buffer SSGIEffect.update
+ * binds) rounded to RGBA16F -> K2 in its TRAA form (temporal_reproject.frag with textureCount 1, inputType "diffuse", RGBA16F history
+ * sampled LINEAR; src/traa/TRAAEffect.js:21-31) -> K9 traa_compose.  The TRAA pass uses the frame's un-jittered camera and the chain's
+ * previous-frame matrices; jittering the rasteriser (TAAUtils.js) stays the host's job.  The fast chain runs the three passes as ONE
+ * kernel (the K5 plane never reaches memory); every other chain runs rfx_ssgi_compose_launch -> rfx_temporal_reproject_launch ->
+ * rfx_traa_compose_launch.  Both write the same bytes. */
+typedef struct rfx_traa_tail_options {
+  rfx_ssgi_compose_params compose;    /* K5: fog / isDebug (ssgi_compose.frag:20-44)                                           */
+  float max_blend;                    /* TRAAEffect forces 0.9                                                                   */
+  float neighborhood_clamp_intensity; /* 1                                                                                   */
+  float confidence_power;             /* 4                                                                                   */
+  int32_t log_transform;              /* 1                                                                                   */
+  int32_t full_accumulate;            /* option fullAccumulate (0); AND-ed with !frame->camera_moved                          */
+  int32_t _pad;
+} rfx_traa_tail_options;
+/* Allocates the tail's planes (TRAA accumulated RGBA16F x 2 by frame parity, K9 output RGBA16F) and renders the tail from the next
+ * frame on.  On a chain whose tail is on it replaces the options and resets the TRAA history (keepData 0 on the next frame:
+ * TemporalReprojectPass.reset()).  opt == NULL turns the tail off and frees its planes.  With the tail on, a frame without
+ * direct_light is RFX_ERR_INVALID_ARG; rfx_ssgi_chain_reset resets the TRAA history too.  A chain attached to a group
+ * (rfx_group_attach_chain*) cannot change its tail: RFX_ERR_UNSUPPORTED. */
+rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* chain, const rfx_traa_tail_options* opt);
+/* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the K9 output (RGBA16F), 7 the TRAA
+ * accumulated plane of the latest frame (RGBA16F; next frame's history).  6 / 7 with the tail off: RFX_ERR_NOT_READY. */
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane* out);
 /* host-buffer frame: uploads the four input planes from (pinned) host memory, renders,
  * downloads `composed` into out_host.  This is the call `bench.py`'s e2e leg times. */
@@ -521,7 +544,12 @@ rfx_status rfx_group_allgather_rows(rfx_group* group, void* stream, const rfx_pl
 /* collective: one frame; this rank renders its band from full-frame input planes and joins the frame's collective on `stream` */
 rfx_status rfx_ssgi_chain_render_sharded(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame);
 /* pure host arithmetic, exported for hosts that drive the per-launch ranges themselves (and for the CPU tests):
- * rows [ranges[2k], ranges[2k+1]) of launch k (K1, K2, K3 pass 0.., K4) for the band [own0, own1); n_launches = 3 + n_poisson_passes */
+ * rows [ranges[2k], ranges[2k+1]) of launch k (K1, K2, K3 pass 0.., K4) for the band [own0, own1); n_launches = 3 + n_poisson_passes.
+ * n_launches = 4 + n_poisson_passes: the same with the TRAA tail as the last launch; it runs on the band and K4 on the band widened
+ * by RFX_TRAA_TAIL_ROWS (every earlier launch widens with it). */
+#define RFX_TRAA_TAIL_ROWS 4  /* 2: the 5x5 clamp window; 1: its LINEAR fetches at texel centres touch row y +- 1; 1: K9's LINEAR fetch
+                                 of the accumulated plane at the pixel centre (same reason).  The TRAA form takes no derivative,
+                                 so no quad row is added. */
 rfx_status rfx_shard_ranges(uint32_t width, uint32_t height, uint32_t own0, uint32_t own1, int32_t n_poisson_passes, float radius,
                             int32_t ssgi_mode, uint32_t* ranges, uint32_t n_launches);
 rfx_status rfx_shard_rebalance(const uint32_t* bounds, const uint32_t* measured_bounds, const float* costs, int32_t n, uint32_t* out);

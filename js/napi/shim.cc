@@ -230,6 +230,28 @@ napi_value ChainWaitHost(napi_env env, napi_callback_info info) {  // chainWaitH
 }
 napi_value ChainReset(napi_env env, napi_callback_info info) { ARGS(1); rfx_ssgi_chain_reset(unwrap<rfx_ssgi_chain>(env, argv[0])); return undefined(env); }
 napi_value ChainDestroy(napi_env env, napi_callback_info info) { ARGS(1); rfx_ssgi_chain_destroy(unwrap<rfx_ssgi_chain>(env, argv[0])); return undefined(env); }
+// chainEnableTraa(ctx, chain, {maxBlend, neighborhoodClampIntensity, confidencePower, logTransform, fullAccumulate,
+//                              fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug} | null)
+// null turns the TRAA tail off; the defaults are the values TRAAEffect forces
+napi_value ChainEnableTraa(napi_env env, napi_callback_info info) {
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  napi_valuetype t = napi_undefined;
+  napi_typeof(env, argv[2], &t);
+  if (t != napi_object) { CHECK(ctx, rfx_ssgi_chain_enable_traa(unwrap<rfx_ssgi_chain>(env, argv[1]), nullptr), "rfx_ssgi_chain_enable_traa"); return undefined(env); }
+  Obj b{env, argv[2]};
+  rfx_traa_tail_options o{};
+  o.max_blend = (float)b.num("maxBlend", 0.9); o.neighborhood_clamp_intensity = (float)b.num("neighborhoodClampIntensity", 1);
+  o.confidence_power = (float)b.num("confidencePower", 4); o.log_transform = (int32_t)b.num("logTransform", 1); o.full_accumulate = (int32_t)b.num("fullAccumulate", 0);
+  rfx_ssgi_compose_params& p = o.compose;
+  p.camera_near = (float)b.num("near", 0.1); p.camera_far = (float)b.num("far", 1000); p.perspective = (int32_t)b.num("perspective", 1); p.is_debug = (int32_t)b.num("isDebug", 0);
+  if (b.has("fog")) {
+    Obj f{env, b.get("fog")};
+    p.use_fog = 1; p.fog_exp2 = (int32_t)f.num("isFogExp2", 0); f.floats("color", p.fog_color, 3);
+    p.fog_near = (float)f.num("near", 1); p.fog_far = (float)f.num("far", 1000); p.fog_density = (float)f.num("density", 0.00025);
+  }
+  CHECK(ctx, rfx_ssgi_chain_enable_traa(unwrap<rfx_ssgi_chain>(env, argv[1]), &o), "rfx_ssgi_chain_enable_traa");
+  return undefined(env);
+}
 
 // ---- per-pass launches (one per reference fullscreen draw; whole planes) ------------------------------------------------------------
 napi_value SsgiCompose(napi_env env, napi_callback_info info) {  // ssgiCompose(ctx, depth, gi, scene, out[, {fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug}])
@@ -415,7 +437,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("envBuild", EnvBuild), FN("envSet", EnvSet), FN("envClear", EnvClear), FN("planeAlloc", PlaneAlloc), FN("planeFree", PlaneFree),
       FN("planeUpload", PlaneUpload), FN("planeDownload", PlaneDownload), FN("chainCreate", ChainCreate), FN("chainSetOptions", ChainSetOptions),
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
-      FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
+      FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
       FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur),
       FN("traaCompose", TraaCompose), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),

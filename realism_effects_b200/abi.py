@@ -19,6 +19,7 @@ FMT_BYTES = {FMT_R32F: 4, FMT_RGBA32F: 16, FMT_RGBA16F: 8, FMT_RGBA8: 4}
 SSGI_IMPORTANCE_SAMPLING, SSGI_MISSED_RAYS, SSGI_USE_DIRECT_LIGHT, SSGI_USE_ENVMAP = 1, 2, 4, 8
 MODE_SSGI, MODE_SSR = 0, 1
 GROUP_ID_BYTES = 128
+ERR_UNSUPPORTED = 6
 ERR_NCCL = 7
 INPUT_DIFFUSE_SPECULAR, INPUT_DIFFUSE, INPUT_SPECULAR = 0, 1, 2
 DENOISE_FULL, DENOISE_FULL_TEMPORAL, DENOISE_TEMPORAL = 0, 1, 2  # option denoiseMode (src/denoise/Denoiser.js:7)
@@ -71,6 +72,22 @@ class ComposeParams(C.Structure):
 class SsgiComposeParams(C.Structure):
     _fields_ = [("use_fog", C.c_int32), ("fog_exp2", C.c_int32), ("fog_color", F3), ("fog_near", C.c_float), ("fog_far", C.c_float),
                 ("fog_density", C.c_float), ("camera_near", C.c_float), ("camera_far", C.c_float), ("perspective", C.c_int32), ("is_debug", C.c_int32)]
+
+
+class TraaTailOptions(C.Structure):
+    _fields_ = [("compose", SsgiComposeParams), ("max_blend", C.c_float), ("neighborhood_clamp_intensity", C.c_float), ("confidence_power", C.c_float),
+                ("log_transform", C.c_int32), ("full_accumulate", C.c_int32), ("_pad", C.c_int32)]
+
+
+def make_traa_tail_options(compose: "SsgiComposeParams | None" = None, full_accumulate: bool = False) -> TraaTailOptions:
+    """The chain's TRAA tail with the values TRAAEffect forces (src/traa/TRAAEffect.js:21-31: maxBlend 0.9, neighborhoodClampIntensity 1,
+    confidencePower 4, logTransform true); `compose`: the K5 fog / isDebug uniforms (None: no fog, no debug)."""
+    o = TraaTailOptions()
+    if compose is not None:
+        o.compose = compose
+    o.max_blend, o.neighborhood_clamp_intensity, o.confidence_power, o.log_transform = 0.9, 1.0, 4.0, 1
+    o.full_accumulate = int(bool(full_accumulate))
+    return o
 
 
 class HbaoParams(C.Structure):
@@ -215,6 +232,7 @@ def _sig(lib):
     lib.rfx_ssgi_chain_set_options.argtypes = [vp, _P(ChainOptions)]
     lib.rfx_ssgi_chain_render.argtypes = [vp, vp, _P(SsgiFrame)]
     lib.rfx_ssgi_chain_output.argtypes = [vp, C.c_int32, PP]
+    lib.rfx_ssgi_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
     lib.rfx_ssgi_chain_render_ranges.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32]
     lib.rfx_ssgi_chain_render_blocks.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
     lib.rfx_ssgi_chain_render_part.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32, C.c_uint32, C.c_uint32]
@@ -255,7 +273,7 @@ EXPORTS = [
     "rfx_plane_download", "rfx_host_alloc", "rfx_host_free", "rfx_format_bytes", "rfx_ssgi_trace_launch",
     "rfx_temporal_reproject_launch", "rfx_poisson_denoise_launch", "rfx_gi_compose_launch", "rfx_ssgi_compose_launch", "rfx_hbao_launch", "rfx_hbao_launch_ex",
     "rfx_ao_compose_launch", "rfx_motion_blur_launch", "rfx_traa_compose_launch", "rfx_gbuffer_ingest_launch", "rfx_effects_launch", "rfx_taa_launch", "rfx_ssgi_chain_create", "rfx_ssgi_chain_destroy",
-    "rfx_ssgi_chain_reset", "rfx_ssgi_chain_render", "rfx_ssgi_chain_output", "rfx_ssgi_chain_render_host",
+    "rfx_ssgi_chain_reset", "rfx_ssgi_chain_render", "rfx_ssgi_chain_output", "rfx_ssgi_chain_enable_traa", "rfx_ssgi_chain_render_host",
     "rfx_ssgi_chain_submit_host", "rfx_ssgi_chain_wait_host", "rfx_ssgi_chain_render_part",
     "rfx_ssgi_chain_set_profiling", "rfx_ssgi_chain_get_profile", "rfx_ssgi_chain_set_options", "rfx_ssgi_chain_render_ranges", "rfx_ssgi_chain_render_blocks",
     "rfx_plane_download_rows", "rfx_group_get_unique_id", "rfx_group_create", "rfx_group_create_inprocess", "rfx_group_attach_chains_inprocess", "rfx_group_destroy", "rfx_group_rank", "rfx_group_world", "rfx_group_uses_peer_reads",

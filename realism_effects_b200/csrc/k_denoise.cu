@@ -390,25 +390,7 @@ cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s) {
 __global__ void __launch_bounds__(256) ssgi_compose_kernel(const __grid_constant__ SsgiComposeArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.W || y >= a.row1) return;
-  if (a.is_debug) {  // :21-24
-    const float4 t = ld_f4(a.gi, x, y);
-    st_h4(a.out.p, a.out.pitch, x, y, mk4(t.x, t.y, t.z, t.w));
-    return;
-  }
-  const float depth = ld_r32f(a.depth, x, y);
-  v3 c;
-  if (depth == 1.0f) {
-    c = xyz(tex_h4_linear(a.scene, pixel_uv(x, y, a.W, a.H)));
-  } else {
-    c = xyz(f4v(ld_f4(a.gi, x, y)));
-    if (a.use_fog) {  // :34-41 + three.js <fog_fragment>
-      const float gz = a.perspective ? perspectiveDepthToViewZ(depth, a.camera_near, a.camera_far) : orthographicDepthToViewZ(depth, a.camera_near, a.camera_far);
-      const float vFogDepth = -(gz * 0.4f);
-      const float fogFactor = a.fog_exp2 ? 1.0f - expf(-a.fog_density * a.fog_density * vFogDepth * vFogDepth) : smoothstepf(a.fog_near, a.fog_far, vFogDepth);
-      c = mix(c, mk3(a.fog_color[0], a.fog_color[1], a.fog_color[2]), fogFactor);
-    }
-  }
-  st_h4(a.out.p, a.out.pitch, x, y, mk4(c, 1.0f));
+  st_h4(a.out.p, a.out.pitch, x, y, ssgi_compose_px(a, x, y));
 }
 cudaError_t launch_ssgi_compose(const SsgiComposeArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);

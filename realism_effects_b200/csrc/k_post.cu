@@ -163,8 +163,7 @@ cudaError_t launch_motion_blur(const MotionBlurArgs& a, cudaStream_t s) {
 __global__ void __launch_bounds__(256) traa_compose_kernel(const __grid_constant__ TraaComposeArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.W || y >= a.row1) return;
-  const v4 t = tex_h4_linear(a.acc, pixel_uv(x, y, a.W, a.H));
-  st_h4(a.out.p, a.out.pitch, x, y, mk4(t.x, t.y, t.z, 1.0f));
+  st_h4(a.out.p, a.out.pitch, x, y, traa_compose_px(PlaneH4{a.acc}, x, y, a.W, a.H));
 }
 cudaError_t launch_traa_compose(const TraaComposeArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);

@@ -89,10 +89,15 @@ RFX_D v4 fetch_hist(const TemporalArgs& a, const PV& t, v2 uv) {
   if (a.hist_f32) return HLIN ? tex_f4_linear(t, uv) : f4v(tex_f4_nearest(t, uv));  // block-uniform: the FloatType FramebufferTexture history
   return HLIN ? tex_h4_linear(t, uv) : tex_h4_nearest(t, uv);
 }
+template <bool HLIN>
+RFX_D v4 fetch_hist(const TemporalArgs&, const PeerPV& t, v2 uv) {  // the fused TRAA tail: RGBA16F LINEAR, rows on their owners
+  static_assert(HLIN, "the TRAA history is sampled LINEAR");
+  return peer_h4_linear(t, uv);
+}
 
 // BiCubicCatmullRom5Tap  reproject.frag:212-255
-template <bool HLIN>
-RFX_D v4 catmull5(const TemporalArgs& a, const PV& tex, v2 P) {
+template <bool HLIN, class Hist>
+RFX_D v4 catmull5(const TemporalArgs& a, const Hist& tex, v2 P) {
   const v2 inv = mk2(a.inv_w, a.inv_h);
   const v2 UV = P / inv;
   const v2 tc = mk2(floorf(UV.x - 0.5f) + 0.5f, floorf(UV.y - 0.5f) + 0.5f);
@@ -117,35 +122,39 @@ RFX_D v4 catmull5(const TemporalArgs& a, const PV& tex, v2 P) {
   return r;
 }
 
-template <int TC, int ITYPE, bool LOG, bool HLIN, bool FAST>
-#ifndef RFX_K2_MIN_BLOCKS
-#define RFX_K2_MIN_BLOCKS 4  // tools/sweep_occupancy.sh sweeps it
-#endif
-__global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(const __grid_constant__ TemporalArgs a) {
-  int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
-  const bool active = x < a.W && y < a.H && in_rows;
-  const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
-  TState s;
+// getVelocityNormalDepth  reproject.frag:97-105 (the quad derivatives of depth / normal are taken by the caller)
+RFX_D void temporal_state(const TemporalArgs& a, int x, int y, int xc, int yc, TState& s) {
   s.vUv = pixel_uv(x, y, a.W, a.H);
   s.roughness = 1.0f; s.moveFactor = 0.0f; s.rayLength = 0.0f;
-
-  // getVelocityNormalDepth  reproject.frag:97-105
   const float4 vt = ld_f4(a.velocity, xc, yc);
   s.velocity = mk2(vt.x, vt.y);
   s.worldNormal = unpackNormal(vt.z);
   s.depth = vt.w;
-  const float fwd = fwidth_f(s.depth);
-  s.curvature = length(fwidth_3(s.worldNormal));  // getCurvature :265-269
-  if (!active) return;
+}
 
+// output of plane i at (x, y) into out0 / out1
+struct PlaneStore {
+  const TemporalArgs& a;
+  int x, y;
+  RFX_D void operator()(int i, v4 v) const {
+    const OutV& o = i == 0 ? a.out0 : a.out1;
+    if (a.out_half) st_h4(o.p, o.pitch, x, y, v);
+    else st_f4(o.p, o.pitch, x, y, make_float4(v.x, v.y, v.z, v.w));
+  }
+};
+
+// K2 of one pixel once its quad derivatives are known (fwd = fwidth(depth), s.curvature; the TRAA form, ITYPE DIFFUSE, reads
+// neither).  `in` samples the RGBA16F input, h0 / h1 are the history planes, store(i, v) receives plane i.  temporal_kernel and
+// the fused TRAA tail (ctraa_kernel) both run this code, so their arithmetic cannot differ.
+template <int TC, int ITYPE, bool LOG, bool HLIN, bool FAST, class In, class Hist, class Store>
+RFX_D void temporal_px(const TemporalArgs& a, const In& in, const Hist& h0, const Hist& h1, TState& s, float fwd, int x, int y, const Store& store) {
   // getTexels + preprocessInput  temporal_reproject.frag:124-145
   v4 inp[2];
   bool sampled[2] = {false, false};
   if (ITYPE == RFX_INPUT_DIFFUSE_SPECULAR) {
     unpackTwoVec4(a.in_scaled ? tex_f4_nearest(a.input, s.vUv) : ld_f4(a.input, x, y), inp[0], inp[1]);
   } else if (a.input_half) {
-    inp[0] = tex_h4_linear(a.input, s.vUv);  // composer buffer: LINEAR, fetched at the pixel centre
+    inp[0] = in.linear(s.vUv);  // composer buffer: LINEAR, fetched at the pixel centre
   } else {
     inp[0] = f4v(a.in_scaled ? tex_f4_nearest(a.input, s.vUv) : ld_f4(a.input, x, y));
   }
@@ -235,7 +244,7 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(c
       for (int dx = -radius[0]; dx <= radius[0]; dx++)
         for (int dy = -radius[0]; dy <= radius[0]; dy++) {
           const v2 nuv = mk2(s.vUv.x + (float)dx * a.inv_w, s.vUv.y + (float)dy * a.inv_h);
-          const v4 nt = a.input_half ? tex_h4_linear(a.input, nuv) : f4v(tex_f4_nearest(a.input, nuv));
+          const v4 nt = a.input_half ? in.linear(nuv) : f4v(tex_f4_nearest(a.input, nuv));
           if (nt.x >= 0.0f) { mn[0] = vmin(xyz(nt), mn[0]); mx[0] = vmax(xyz(nt), mx[0]); }
         }
     }
@@ -245,7 +254,7 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(c
   for (int i = 0; i < TC; i++) {
     const bool spec = rs[i] != 0;
     const v3 uvc = spec ? ruvS : ruvD;
-    const PV& hist = i == 0 ? a.hist0 : a.hist1;
+    const Hist& hist = i == 0 ? h0 : h1;
     // reproject()  temporal_reproject.frag:83-122
     const v4 acc = catmull5<HLIN>(a, hist, mk2(uvc.x, uvc.y));
     v3 accRgb = transformColor<LOG, FAST>(xyz(acc));
@@ -280,10 +289,24 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(c
     float oa = 1.0f / (1.0f - tmix) - 1.0f;
     oa = fminf(65536.0f, oa);
     const v3 orgb = undoColorTransform<LOG, FAST>(mix(inRgb, accRgb, tmix));
-    const OutV& o = i == 0 ? a.out0 : a.out1;
-    if (a.out_half) st_h4(o.p, o.pitch, x, y, mk4(orgb, oa));
-    else st_f4(o.p, o.pitch, x, y, make_float4(orgb.x, orgb.y, orgb.z, oa));
+    store(i, mk4(orgb, oa));
   }
+}
+
+template <int TC, int ITYPE, bool LOG, bool HLIN, bool FAST>
+#ifndef RFX_K2_MIN_BLOCKS
+#define RFX_K2_MIN_BLOCKS 4  // tools/sweep_occupancy.sh sweeps it
+#endif
+__global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(const __grid_constant__ TemporalArgs a) {
+  int x, y;
+  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool active = x < a.W && y < a.H && in_rows;
+  TState s;
+  temporal_state(a, x, y, min(x, a.W - 1), min(y, a.H - 1), s);
+  const float fwd = fwidth_f(s.depth);
+  s.curvature = length(fwidth_3(s.worldNormal));  // getCurvature :265-269
+  if (!active) return;
+  temporal_px<TC, ITYPE, LOG, HLIN, FAST>(a, PlaneH4{a.input}, a.hist0, a.hist1, s, fwd, x, y, PlaneStore{a, x, y});
 }
 
 template <int TC, int IT, bool FAST>
@@ -305,6 +328,96 @@ cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s) {
   else if (a.input_type == RFX_INPUT_SPECULAR && a.texture_count == 1) RFX_LT(1, RFX_INPUT_SPECULAR);
   else return cudaErrorNotSupported;
 #undef RFX_LT
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// TRAA frame tail of the fast chain: K5 ssgi_compose -> K2 (TRAA form) -> K9 traa_compose in one launch per frame.
+// K9 fetches the accumulated plane LINEAR at the pixel centre, which touches texels x +- 1 / y +- 1 wherever
+// ((x + .5) / W) * W - .5 is not exactly x, so a block runs K2 on its 16x16 tile plus a ring of one texel (18 x 18).  K2 fetches
+// K5 LINEAR at vUv + (dx, dy) / size with |dx|, |dy| <= 2, i.e. texels up to 3 away, so K5 is staged for the tile plus 4 texels on
+// each side (24 x 24), rounded to RGBA16F as ssgi_compose_kernel stores it.  K2 and K9 read those fp16 texels from shared memory
+// with tex_h4_linear's arithmetic, and K2 / K5 / K9 are the per-pass kernels' own device functions: the bytes are those of the
+// three per-pass launches, and the K5 plane never reaches memory.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int kTraaTileW = 64;  // a block covers 64 x 16 output pixels: the ring and the K5 halo are recomputed on 16 % / 69 % extra texels
+constexpr int kTraaRing = 1, kTraaK5Halo = 3 + kTraaRing;
+constexpr int kTraaAccW = kTraaTileW + 2 * kTraaRing, kTraaAccH = kTileH + 2 * kTraaRing;
+constexpr int kTraaK5W = kTraaTileW + 2 * kTraaK5Halo, kTraaK5H = kTileH + 2 * kTraaK5Halo;
+
+struct TileH4 {  // RGBA16F texels of a W x H plane held in shared memory: texel (x, y) at s[(y - y0) * w + (x - x0)]
+  const uint2* s;
+  int x0, y0, w, W, H;
+  RFX_D v4 tex(int x, int y) const { return half4_to_v4(s[(y - y0) * w + (x - x0)]); }
+  RFX_D v4 linear(v2 uv) const {
+    const Bilin b = bilin_setup(uv, W, H);
+    return bilin_blend4(b, tex(b.x0, b.y0), tex(b.x1, b.y0), tex(b.x0, b.y1), tex(b.x1, b.y1));
+  }
+};
+RFX_D uint2 pack_h4(v4 v) {  // st_h4's rounding
+  uint2 u;
+  u.x = packHalf2x16(v.x, v.y);
+  u.y = packHalf2x16(v.z, v.w);
+  return u;
+}
+struct TraaStore {  // K2's output: into the shared tile for K9, and into the accumulated plane for the block's own output pixels
+  uint2* slot;
+  const OutV& acc;
+  int x, y;
+  bool own;
+  RFX_D void operator()(int, v4 v) const {
+    const uint2 u = pack_h4(v);
+    *slot = u;
+    if (own) *((uint2*)(acc.p + ((unsigned)y * (unsigned)acc.pitch + (unsigned)x * 8u))) = u;
+  }
+};
+
+#ifndef RFX_TRAA_MIN_BLOCKS
+#define RFX_TRAA_MIN_BLOCKS 3
+#endif
+template <bool LOG, bool FAST>
+__global__ void __launch_bounds__(kThreads, RFX_TRAA_MIN_BLOCKS) ctraa_kernel(const __grid_constant__ CTraaArgs a) {
+  __shared__ uint2 k5s[kTraaK5W * kTraaK5H];
+  __shared__ uint2 accs[kTraaAccW * kTraaAccH];
+  const TemporalArgs& t = a.t;
+  const int W = t.W, H = t.H;
+  int k = 0;  // the segment of this block's tile row, laid out as seg_pixel does
+  while (k + 1 < t.segs.n && (int)blockIdx.y >= t.segs.tile0[k + 1]) k++;
+  const int x0 = blockIdx.x * kTraaTileW, y0 = (t.segs.r0[k] & ~1) + ((int)blockIdx.y - t.segs.tile0[k]) * kTileH;
+  const int r0 = t.segs.r0[k], r1 = t.segs.r1[k];
+  for (int i = threadIdx.x; i < kTraaK5W * kTraaK5H; i += kThreads)  // slots outside the image hold a clamped duplicate, never read
+    k5s[i] = pack_h4(ssgi_compose_px(a.k5, clampi(x0 - kTraaK5Halo + i % kTraaK5W, W), clampi(y0 - kTraaK5Halo + i / kTraaK5W, H)));
+  __syncthreads();
+  const TileH4 k5{k5s, x0 - kTraaK5Halo, y0 - kTraaK5Halo, kTraaK5W, W, H};
+  for (int i = threadIdx.x; i < kTraaAccW * kTraaAccH; i += kThreads) {
+    const int x = x0 - kTraaRing + i % kTraaAccW, y = y0 - kTraaRing + i / kTraaAccW;
+    if (x < 0 || x >= W || y < 0 || y >= H) continue;
+    const bool own = x >= x0 && x < x0 + kTraaTileW && y >= y0 && y < y0 + kTileH && y >= r0 && y < r1;
+    TState s;
+    temporal_state(t, x, y, x, y, s);
+    s.curvature = 0.0f;  // the TRAA form takes no derivative (fwidth feeds only the discard / hit-point tests of the other forms)
+    temporal_px<1, RFX_INPUT_DIFFUSE, LOG, true, FAST>(t, k5, a.hist, a.hist, s, 0.0f, x, y, TraaStore{&accs[i], a.acc, x, y, own});
+  }
+  __syncthreads();
+  const TileH4 acc{accs, x0 - kTraaRing, y0 - kTraaRing, kTraaAccW, W, H};
+  for (int i = threadIdx.x; i < kTraaTileW * kTileH; i += kThreads) {
+    const int x = x0 + i % kTraaTileW, y = y0 + i / kTraaTileW;
+    if (x < W && y < H && y >= r0 && y < r1) st_h4(a.out.p, a.out.pitch, x, y, traa_compose_px(acc, x, y, W, H));
+  }
+}
+
+cudaError_t launch_ctraa(const CTraaArgs& a, cudaStream_t s) {
+  const TemporalArgs& t = a.t;
+  if (t.texture_count != 1 || t.input_type != RFX_INPUT_DIFFUSE || !t.input_half || !t.out_half || !t.history_linear || t.hist_f32 || t.in_scaled)
+    return cudaErrorNotSupported;
+  dim3 grid((t.W + kTraaTileW - 1) / kTraaTileW, t.segs.tiles);
+  if (t.fast) {
+    if (t.log_transform) ctraa_kernel<true, true><<<grid, kThreads, 0, s>>>(a);
+    else ctraa_kernel<false, true><<<grid, kThreads, 0, s>>>(a);
+  } else {
+    if (t.log_transform) ctraa_kernel<true, false><<<grid, kThreads, 0, s>>>(a);
+    else ctraa_kernel<false, false><<<grid, kThreads, 0, s>>>(a);
+  }
   return cudaGetLastError();
 }
 

@@ -413,6 +413,22 @@ static rfx_status ensure_step_table(rfx_ctx* ctx, int steps) {
   ctx->step_table_steps = steps;
   return RFX_OK;
 }
+// K2's uniforms for an a.W x a.H target (rfx_temporal_reproject_launch and the fused TRAA tail of the chain)
+static void temporal_uniforms(const rfx_ctx* ctx, const rfx_temporal_params* p, TemporalArgs& a) {
+  cam_to_dev(p->cam, a.cam);
+  memcpy(a.prev_view.m, p->prev_view_matrix, 64);
+  memcpy(a.prev_world.m, p->prev_camera_matrix_world, 64);
+  memcpy(a.prev_proj.m, p->prev_projection, 64);
+  memcpy(a.prev_proj_inv.m, p->prev_projection_inverse, 64);
+  matmul(p->prev_projection, p->prev_view_matrix, a.prev_proj_view.m);
+  memcpy(a.camera_pos, p->camera_pos, 12);
+  a.max_blend = p->max_blend; a.clamp_intensity = p->neighborhood_clamp_intensity; a.keep_data = p->keep_data; a.confidence_power = p->confidence_power;
+  a.inv_w = (float)(1.0 / (double)a.W);  // TemporalReprojectPass.js:135: JS doubles, uploaded as float32
+  a.inv_h = (float)(1.0 / (double)a.H);
+  a.full_accumulate = p->full_accumulate; a.texture_count = p->texture_count; a.input_type = p->input_type; a.log_transform = p->log_transform;
+  a.rs0 = p->reproject_specular[0]; a.rs1 = p->reproject_specular[1]; a.history_linear = p->history_linear;
+  a.fast = ctx->fast_math;
+}
 #define LAUNCHED(expr)                                                                                   \
   do {                                                                                                   \
     cudaError_t e_ = (expr);                                                                             \
@@ -534,19 +550,7 @@ rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_t
   if (a.in_scaled && a.input_half) return fail(ctx, RFX_ERR_UNSUPPORTED, "temporal: a scaled input is the RGBA32F SSGI target");
   rows(row0, row1, out0->height, a.row0, a.row1);
   set_segs(ctx, a.row0, a.row1, a.segs);
-  cam_to_dev(p->cam, a.cam);
-  memcpy(a.prev_view.m, p->prev_view_matrix, 64);
-  memcpy(a.prev_world.m, p->prev_camera_matrix_world, 64);
-  memcpy(a.prev_proj.m, p->prev_projection, 64);
-  memcpy(a.prev_proj_inv.m, p->prev_projection_inverse, 64);
-  matmul(p->prev_projection, p->prev_view_matrix, a.prev_proj_view.m);
-  memcpy(a.camera_pos, p->camera_pos, 12);
-  a.max_blend = p->max_blend; a.clamp_intensity = p->neighborhood_clamp_intensity; a.keep_data = p->keep_data; a.confidence_power = p->confidence_power;
-  a.inv_w = (float)(1.0 / (double)a.W);  // TemporalReprojectPass.js:135: JS doubles, uploaded as float32
-  a.inv_h = (float)(1.0 / (double)a.H);
-  a.full_accumulate = p->full_accumulate; a.texture_count = p->texture_count; a.input_type = p->input_type; a.log_transform = p->log_transform;
-  a.rs0 = p->reproject_specular[0]; a.rs1 = p->reproject_specular[1]; a.history_linear = p->history_linear;
-  a.fast = ctx->fast_math;
+  temporal_uniforms(ctx, p, a);
   LAUNCHED(launch_temporal(a, pick(ctx, stream)));
   return RFX_OK;
 }
@@ -847,6 +851,15 @@ struct rfx_ssgi_chain {
   float keep_data = 0.0f;  // SSGIEffect's constructor resets the denoiser (makeOptionsReactive -> reset())
   // blue-noise counters: one closure per material (BlueNoiseUtils.js:17-33)
   int32_t bn_trace = 0, bn_poisson = 0;
+  // TRAA frame tail (rfx_ssgi_chain_enable_traa): one more launch after K4
+  bool traa_on = false;
+  rfx_traa_tail_options traa{};
+  rfx_plane traa_acc[2]{}, traa_out{};  // accumulated plane by tail parity (acc[prev] is the history), K9 output
+  rfx_plane traa_k5{};                  // K5 plane of the per-pass tail (chains other than the fast one)
+  uint64_t traa_frames = 0;             // tails rendered; acc[traa_frames & 1] is written next
+  float traa_keep = 0.0f;               // keepData of the TRAA pass
+  rfx_temporal_params traa_tp{};        // the frame's camera and the previous-frame matrices its K2 used
+  PeerPV peer_traa[2]{};
   // optional per-pass event timing
   bool profiling = false;
   struct Span { cudaEvent_t a, b; int slot; };
@@ -922,7 +935,7 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->composed,
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
-  for (rfx_plane* p : {&ch->composed2[0], &ch->composed2[1]}) if (p->ptr) rfx_plane_free(ctx, p);
+  for (rfx_plane* p : {&ch->composed2[0], &ch->composed2[1], &ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
   for (IPlane* p : {&ch->nrdz, &ch->tr32, &ch->dnA16[0], &ch->dnA16[1], &ch->dnB16[0], &ch->dnB16[1]}) if (p->p) cudaFree(p->p);
   for (int i = 0; i < 2; i++) for (cudaEvent_t e : {ch->ev_up[i], ch->ev_rendered[i], ch->ev_dn[i]}) if (e) cudaEventDestroy(e);
   if (ch->s_up) cudaStreamDestroy(ch->s_up);
@@ -969,13 +982,45 @@ rfx_status rfx_ssgi_chain_set_options(rfx_ssgi_chain* ch, const rfx_ssgi_chain_o
 rfx_status rfx_ssgi_chain_reset(rfx_ssgi_chain* ch) {
   if (!ch) return RFX_ERR_INVALID_ARG;
   ch->keep_data = 0.0f;  // TemporalReprojectPass.reset()  :158-160
+  ch->traa_keep = 0.0f;  // the TRAA pass's too (TRAAEffect.reset)
+  return RFX_OK;
+}
+
+rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_options* opt) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (ch->group) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
+  if (!opt) {
+    CU(cudaStreamSynchronize(ctx->stream));
+    for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
+    ch->traa_on = false;
+    return RFX_OK;
+  }
+  if (!ch->traa_out.ptr) {
+    rfx_status st = RFX_OK;
+    for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out})
+      if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
+    if (st == RFX_OK && !ch->fastpath) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
+    if (st != RFX_OK) {
+      for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
+      return st;
+    }
+  }
+  ch->traa = *opt;
+  ch->traa_on = true;
+  ch->traa_keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
   return RFX_OK;
 }
 
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
-  if (which < 0 || which > 5) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..5");
+  if (which < 0 || which > 7) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..7");
+  if (which >= 6) {
+    if (!ch->traa_on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
+    *out = which == 6 ? ch->traa_out : ch->traa_acc[(ch->traa_frames + 1) & 1];
+    return RFX_OK;
+  }
   if (ch->fastpath) {
     const int last = (int)((ch->frame_idx + 1) & 1);  // parity of the most recently completed frame
     if (which == 0) { *out = ch->composed2[last]; return RFX_OK; }
@@ -1046,6 +1091,70 @@ static void peer_single(PeerPV& pp, PV local) {
   pp.own0 = 0; pp.own1 = local.h;
 }
 
+// K2's camera state of this frame, kept for the TRAA tail: the current (un-jittered) camera and the previous-frame matrices before
+// K2 replaces them (the TRAA TemporalReprojectPass tracks the same camera, so its previous frame is the chain's)
+static void keep_traa_camera(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
+  rfx_temporal_params& tp = ch->traa_tp;
+  tp.cam = f->cam;
+  memcpy(tp.prev_view_matrix, ch->prev_view, 64); memcpy(tp.prev_camera_matrix_world, ch->prev_world, 64);
+  memcpy(tp.prev_projection, ch->prev_proj, 64); memcpy(tp.prev_projection_inverse, ch->prev_proj_inv, 64);
+  memcpy(tp.camera_pos, f->camera_pos, 12); memcpy(tp.prev_camera_pos, ch->prev_pos, 12);
+}
+
+// The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
+// rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
+// K2 on them +- 1).
+static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane* composed, const uint32_t* ranges,
+                                    uint32_t n_blocks, uint32_t n_launches, uint32_t k) {
+  rfx_ctx* ctx = ch->ctx;
+  const int W = (int)ch->opt.width, H = (int)ch->opt.height;
+  const int cur = (int)(ch->traa_frames & 1), prev = cur ^ 1;
+  rfx_temporal_params tp = ch->traa_tp;  // TRAAEffect's forced options over the TemporalReprojectPass defaults (TRAAEffect.js:21-31)
+  tp.max_blend = ch->traa.max_blend; tp.neighborhood_clamp_intensity = ch->traa.neighborhood_clamp_intensity;
+  tp.confidence_power = ch->traa.confidence_power; tp.log_transform = ch->traa.log_transform ? 1 : 0;
+  tp.keep_data = ch->traa_keep;
+  tp.full_accumulate = ch->traa.full_accumulate && !f->camera_moved ? 1 : 0;
+  tp.texture_count = 1; tp.input_type = RFX_INPUT_DIFFUSE; tp.history_linear = 1;
+  tp.reproject_specular[0] = tp.reproject_specular[1] = 0;
+  if (ch->fastpath) {
+    CTraaArgs a{};
+    TemporalArgs& t = a.t;
+    if (!pv(f->velocity, RFX_FMT_RGBA32F, t.velocity)) return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: velocity must be RGBA32F");
+    t.W = W; t.H = H;
+    t.segs = segs_for(ranges, n_blocks, n_launches, k, H);
+    temporal_uniforms(ctx, &tp, t);
+    t.input_half = 1; t.out_half = 1;
+    SsgiComposeArgs& c = a.k5;
+    if (!pv(f->depth, RFX_FMT_R32F, c.depth) || !pv(composed, RFX_FMT_RGBA32F, c.gi) || !pv(f->direct_light, RFX_FMT_RGBA16F, c.scene))
+      return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: the TRAA tail needs an RGBA16F direct light plane");
+    if (c.scene.w != W || c.scene.h != H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "chain: the direct light plane must match the chain size");
+    c.W = W; c.H = H; c.row0 = 0; c.row1 = H;
+    const rfx_ssgi_compose_params& q = ch->traa.compose;
+    c.use_fog = q.use_fog; c.fog_exp2 = q.fog_exp2; c.perspective = q.perspective; c.is_debug = q.is_debug;
+    memcpy(c.fog_color, q.fog_color, 12);
+    c.fog_near = q.fog_near; c.fog_far = q.fog_far; c.fog_density = q.fog_density; c.camera_near = q.camera_near; c.camera_far = q.camera_far;
+    if (ch->group) a.hist = ch->peer_traa[prev]; else peer_single(a.hist, rpv(ch->traa_acc[prev]));
+    a.acc = OutV{(unsigned char*)ch->traa_acc[cur].ptr, (long long)ch->traa_acc[cur].pitch};
+    a.out = OutV{(unsigned char*)ch->traa_out.ptr, (long long)ch->traa_out.pitch};
+    LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
+  } else {
+    const int halo = RFX_TRAA_TAIL_ROWS;
+    for (uint32_t b = 0; b < (ranges ? n_blocks : 1u); b++) {
+      const int r0 = ranges ? (int)ranges[(b * n_launches + k) * 2] : 0, r1 = ranges ? (int)ranges[(b * n_launches + k) * 2 + 1] : H;
+      rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
+                                              (uint32_t)std::max(0, r0 - halo), (uint32_t)std::min(H, r1 + halo));
+      if (st == RFX_OK)
+        st = rfx_temporal_reproject_launch(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
+                                           (uint32_t)std::max(0, r0 - 1), (uint32_t)std::min(H, r1 + 1));
+      if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc[cur], &ch->traa_out, (uint32_t)r0, (uint32_t)r1);
+      if (st != RFX_OK) return st;
+    }
+  }
+  ch->traa_keep = 1.0f;
+  ch->traa_frames++;
+  return RFX_OK;
+}
+
 // 2-D TMA descriptor over a plane of 16-byte texels, addressed as rows of 4-byte elements (box dims are limited to 256 elements)
 static bool encode_texel_map(CUtensorMap* map, const void* base, int W, int H, size_t pitch, int box_w, int box_h) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1071,7 +1180,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
   const int W = (int)o.width, H = (int)o.height;
-  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations;
+  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations + (ch->traa_on ? 1u : 0u);
   if (!ranges) n_blocks = 1;
   auto on = [&](uint32_t k) { return k >= k_begin && k < k_end; };
   const cudaStream_t cs = stream ? (cudaStream_t)stream : ctx->stream;
@@ -1121,6 +1230,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
       memcpy(ch->prev_pos, f->camera_pos, 12);
       ch->have_prev = true;
     }
+    keep_traa_camera(ch, f);
     memcpy(a.prev_world.m, ch->prev_world, 64); memcpy(a.prev_proj_inv.m, ch->prev_proj_inv, 64);
     matmul(ch->prev_proj, ch->prev_view, a.prev_proj_view.m);
     memcpy(a.camera_pos, f->camera_pos, 12);
@@ -1215,7 +1325,9 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     SpanGuard g(ch, cs, 4);
     LAUNCHED(launch_ccompose(a, cs));
   }
-  if (on(k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
+  // ---- TRAA tail (reads this frame's `composed`, so it runs before the planes change parity)
+  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed2[cur], ranges, n_blocks, n_launches, k_compose + 1)) != RFX_OK) return st;
+  if (on(ch->traa_on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
   return RFX_OK;
 }
 
@@ -1226,6 +1338,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
 // different all-gather; per-frame state advances with the launch that consumes it.
 static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_blocks,
                                     uint32_t k_begin, uint32_t k_end, int k1_phase = 0) {
+  if (ch->traa_on && !f->direct_light) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail composes over the direct light plane (the composer input buffer): it may not be NULL");
   if (ch->fastpath) return chain_render_fast(ch, stream, f, ranges, n_blocks, k_begin, k_end, k1_phase);
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
@@ -1233,7 +1346,8 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   const bool dm_full = o.denoise_mode == RFX_DENOISE_FULL;
   if (!dm_full && ranges) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for denoise_mode full only");
   if (ranges && ch->ssgi_out.height != o.height) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for resolution_scale 1 only");
-  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations;  // K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too)
+  // K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too), then the TRAA tail when it is on
+  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations + (ch->traa_on ? 1u : 0u);
   if (!ranges) n_blocks = 1;
   // what SSGIPass samples as accumulatedTexture = denoiser.texture (Denoiser.js:67-78): the compose target, or the temporal pass's first texture
   rfx_plane* accumulated = o.denoise_mode == RFX_DENOISE_TEMPORAL ? &ch->tr[0] : &ch->composed;
@@ -1274,6 +1388,7 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
       memcpy(ch->prev_pos, f->camera_pos, 12);
       ch->have_prev = true;
     }
+    keep_traa_camera(ch, f);
     memcpy(tp.prev_view_matrix, ch->prev_view, 64); memcpy(tp.prev_camera_matrix_world, ch->prev_world, 64);
     memcpy(tp.prev_projection, ch->prev_proj, 64); memcpy(tp.prev_projection_inverse, ch->prev_proj_inv, 64);
     memcpy(tp.camera_pos, f->camera_pos, 12); memcpy(tp.prev_camera_pos, ch->prev_pos, 12);
@@ -1339,6 +1454,9 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     }
     if (st != RFX_OK) return st;
   }
+  k++;
+  // ---- TRAA tail over the effect's output (`composed`, or the temporal texture in denoiseMode "temporal")
+  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, accumulated, ranges, n_blocks, n_launches, k);
   return RFX_OK;
 }
 
@@ -1347,7 +1465,7 @@ rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* ch, void* stream, const rfx_ssg
   return chain_render_impl(ch, stream, f, nullptr, 1, 0, 0xffffffffu);
 }
 static rfx_status check_ranges(rfx_ssgi_chain* ch, const uint32_t* ranges, uint32_t n_launches, uint32_t n_blocks) {
-  const uint32_t expect = 3u + 2u * (uint32_t)ch->opt.denoise_iterations;
+  const uint32_t expect = 3u + 2u * (uint32_t)ch->opt.denoise_iterations + (ch->traa_on ? 1u : 0u);
   if (n_launches != expect || n_blocks == 0 || n_blocks > RFX_MAX_SEGS) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain ranges: expected %u launches per block, got %u (blocks %u)", expect, n_launches, n_blocks);
   for (uint32_t i = 0; i < n_launches * n_blocks; i++)
     if (ranges[2 * i] >= ranges[2 * i + 1] || ranges[2 * i + 1] > ch->opt.height) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain ranges: bad range %u", i);

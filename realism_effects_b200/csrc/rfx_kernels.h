@@ -38,6 +38,14 @@ RFX_D const unsigned char* peer_row_base(const PeerPV& p, int y) {
   for (int i = 1; i < RFX_MAX_PEERS; i++) k += (i < p.n && y >= p.bound[i]) ? 1 : 0;
   return p.base[k];
 }
+// LINEAR fetch of an RGBA16F plane whose rows live on their owners: tex_h4_linear's arithmetic, each row from peer_row_base
+RFX_D v4 peer_h4_linear(const PeerPV& p, v2 uv) {
+  const Bilin b = bilin_setup(uv, p.local.w, p.local.h);
+  const unsigned char* r0 = peer_row_base(p, b.y0) + (unsigned)b.y0 * (unsigned)p.local.pitch;
+  const unsigned char* r1 = peer_row_base(p, b.y1) + (unsigned)b.y1 * (unsigned)p.local.pitch;
+  auto ld = [](const unsigned char* r, int x) { return half4_to_v4(__ldg((const uint2*)(r + (unsigned)x * 8u))); };
+  return bilin_blend4(b, ld(r0, b.x0), ld(r0, b.x1), ld(r1, b.x0), ld(r1, b.x1));
+}
 
 struct CamD {  // device copy of rfx_camera
   M4 projection, projection_inverse, camera_matrix_world, view_matrix;
@@ -103,6 +111,27 @@ struct SsgiComposeArgs {
   float fog_color[3], fog_near, fog_far, fog_density, camera_near, camera_far;
 };
 cudaError_t launch_ssgi_compose(const SsgiComposeArgs& a, cudaStream_t s);
+// K5 for pixel (x, y): the texel ssgi_compose_kernel stores (RGBA16F).  Shared with the fused TRAA tail (k_temporal.cu).
+RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
+  if (a.is_debug) {  // ssgi_compose.frag:21-24
+    const float4 t = ld_f4(a.gi, x, y);
+    return mk4(t.x, t.y, t.z, t.w);
+  }
+  const float depth = ld_r32f(a.depth, x, y);
+  v3 c;
+  if (depth == 1.0f) {
+    c = xyz(tex_h4_linear(a.scene, pixel_uv(x, y, a.W, a.H)));
+  } else {
+    c = xyz(f4v(ld_f4(a.gi, x, y)));
+    if (a.use_fog) {  // :34-41 + three.js <fog_fragment>
+      const float gz = a.perspective ? perspectiveDepthToViewZ(depth, a.camera_near, a.camera_far) : orthographicDepthToViewZ(depth, a.camera_near, a.camera_far);
+      const float vFogDepth = -(gz * 0.4f);
+      const float fogFactor = a.fog_exp2 ? 1.0f - expf(-a.fog_density * a.fog_density * vFogDepth * vFogDepth) : smoothstepf(a.fog_near, a.fog_far, vFogDepth);
+      c = mix(c, mk3(a.fog_color[0], a.fog_color[1], a.fog_color[2]), fogFactor);
+    }
+  }
+  return mk4(c, 1.0f);
+}
 
 // ---- K2 ----------------------------------------------------------------------------------
 struct TemporalArgs {
@@ -123,6 +152,18 @@ struct TemporalArgs {
   int fast;  // SFU variants of log/exp/pow
 };
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
+
+// TRAA frame tail of the fast chain (k_temporal.cu: ctraa_kernel): K5 -> K2 (TRAA form) -> K9 in one launch over the rows of `t.segs`.
+// `t` carries the TRAA K2 uniforms exactly as rfx_temporal_reproject_launch fills them (input_half = out_half = history_linear = 1,
+// texture_count 1, input_type DIFFUSE); `k5.gi` is `composed`, `k5.scene` the direct light; history rows live on their owners.
+struct CTraaArgs {
+  TemporalArgs t;
+  SsgiComposeArgs k5;
+  PeerPV hist;  // TRAA accumulated plane of the previous frame
+  OutV acc;     // TRAA accumulated plane of this frame
+  OutV out;     // K9 output
+};
+cudaError_t launch_ctraa(const CTraaArgs& a, cudaStream_t s);
 
 // ---- K1 ----------------------------------------------------------------------------------
 struct SsgiArgs {
@@ -199,6 +240,17 @@ struct TraaComposeArgs {
   int W, H, row0, row1;
 };
 cudaError_t launch_traa_compose(const TraaComposeArgs& a, cudaStream_t s);
+// LINEAR sampler of an RGBA16F plane in device memory; the fused TRAA tail has one with the same interface over shared memory
+struct PlaneH4 {
+  const PV& t;
+  RFX_D v4 linear(v2 uv) const { return tex_h4_linear(t, uv); }
+};
+// K9 for pixel (x, y) of the W x H target (traa_compose.frag:3-6): the accumulated plane fetched LINEAR at the pixel centre, a = 1
+template <class S>
+RFX_D v4 traa_compose_px(const S& acc, int x, int y, int W, int H) {
+  const v4 t = acc.linear(pixel_uv(x, y, W, H));
+  return mk4(t.x, t.y, t.z, 1.0f);
+}
 
 // merged cosmetic effects + TAAPass (k_fx.cu)
 struct EffectsArgs {

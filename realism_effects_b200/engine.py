@@ -228,6 +228,7 @@ class SsgiChain:
     def __init__(self, ctx: Context, opt: abi.ChainOptions):
         self.ctx = ctx
         self.opt = opt
+        self.traa = None
         h = C.c_void_p()
         ctx._chk(ctx.lib.rfx_ssgi_chain_create(ctx.h, C.byref(opt), C.byref(h)))
         self.h = h
@@ -243,6 +244,17 @@ class SsgiChain:
     def set_options(self, opt: abi.ChainOptions):
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_set_options(self.h, C.byref(opt)))
         self.opt = opt
+
+    def enable_traa(self, options: "abi.TraaTailOptions | None" = None, enable: bool = True):
+        """TRAA frame tail (K5 -> TRAA -> K9 after K4, include/rfx.h: rfx_ssgi_chain_enable_traa): outputs 6 (the K9 frame) and 7 (the
+        TRAA accumulated plane).  options: abi.make_traa_tail_options(...) (default: TRAAEffect's values, no fog); enable=False turns it off.
+        Enabling again replaces the options and resets the TRAA history."""
+        if not enable:
+            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_enable_traa(self.h, None))
+            self.traa = None
+            return
+        self.traa = options if options is not None else abi.make_traa_tail_options()
+        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_enable_traa(self.h, C.byref(self.traa)))
 
     @staticmethod
     def _frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved) -> abi.SsgiFrame:
@@ -283,6 +295,7 @@ class SsgiChain:
             self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_part(self.h, stream, C.byref(f), flat, nl, nb, part))
 
     def output(self, which: int = 0) -> Plane:
+        """0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA accumulated plane"""
         p = Plane()
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_output(self.h, which, C.byref(p)))
         return p

@@ -46,9 +46,14 @@ class ShardPlan:
     mirror: bool = False  # True: odd super-blocks are assigned in REVERSE rank order (boustrophedon), see block_of()
     bounds: tuple | None = None  # explicit band borders (world + 1 ascending rows, 0 .. height): one contiguous band per rank
     width: int | None = None     # frame width: portrait frames (H > W) stretch the Poisson taps' row reach by H / W
+    traa: bool = False           # the TRAA tail runs as one more launch after K4 (rfx_ssgi_chain_enable_traa)
 
     K2_NEIGHBOURHOOD_ROWS = 2  # 5x5 clamp window (reproject.frag:57-59)
     K4_INPUT_ROWS = 1          # literal bilinear fetch of the LINEAR Poisson targets at the pixel centre
+    # `composed` rows the TRAA tail reads around its band (include/rfx.h RFX_TRAA_TAIL_ROWS): 2 for the TRAA clamp window, 1 because
+    # those taps are LINEAR fetches at texel centres (the reason of K4_INPUT_ROWS), 1 for K9's LINEAR fetch of the accumulated plane at
+    # the pixel centre; the TRAA form takes no derivative, so no quad row
+    TRAA_TAIL_ROWS = 4
 
     def block_of(self, rank: int, j: int):
         """rows of the block `rank` owns inside super-block j.  With `mirror`, odd super-blocks run in reverse rank order, so a
@@ -99,16 +104,17 @@ class ShardPlan:
 
     def ranges_for(self, own) -> list:
         n = self.n_poisson_passes
+        k4 = self._expand(own, self.TRAA_TAIL_ROWS) if self.traa else own
         k3 = [None] * n
-        nxt = own
+        nxt = k4
         if n:
-            k3[n - 1] = self._expand(own, self.K4_INPUT_ROWS)
+            k3[n - 1] = self._expand(k4, self.K4_INPUT_ROWS)
             for j in range(n - 2, -1, -1):
                 k3[j] = self._expand(k3[j + 1], self.poisson_halo)
             nxt = self._expand(k3[0], self.poisson_halo)
         k2 = nxt
         k1 = self._expand(k2, self.K2_NEIGHBOURHOOD_ROWS)
-        return [k1, k2, *k3, own]  # K4 runs in both modes (SSR composes with inputType specular)
+        return [k1, k2, *k3, k4] + ([own] if self.traa else [])  # K4 runs in both modes (SSR composes with inputType specular)
 
     @property
     def ranges(self) -> list:
@@ -122,7 +128,7 @@ class ShardPlan:
 
     @property
     def n_launches(self) -> int:
-        return 3 + self.n_poisson_passes
+        return 3 + self.n_poisson_passes + (1 if self.traa else 0)
 
     def super_block(self, j: int):
         """rows of super-block j: N consecutive blocks, one per rank, in rank order (an in-place all-gather unit)"""
@@ -206,7 +212,8 @@ class ShardedSsgiChain:
     INPUTS = (("depth", 4, True), ("gbuffer", 16, False), ("velocity", 16, True), ("direct", 8, False))  # name, bytes/px, sampled anywhere
 
     def __init__(self, ctx, chain_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
-                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None):
+                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None):
+        """traa: abi.TraaTailOptions (abi.make_traa_tail_options()) to render the TRAA tail too (the same on every rank), or None"""
         import ctypes as C
 
         from . import abi, engine
@@ -226,6 +233,8 @@ class ShardedSsgiChain:
             unique_id = box[0]
         self.rank, self.world = rank, world
         self.chain = engine.SsgiChain(ctx, chain_options)
+        if traa is not None:  # before the attach: the group maps the tail's history plane then
+            self.chain.enable_traa(traa)
         g = C.c_void_p()
         ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, rank, world, C.byref(g)))
         self.g = g
@@ -323,7 +332,10 @@ class ShardedSsgiChain:
     def submit_host(self, cam, host: dict, camera_pos, camera_moved: bool, out_host):
         """One frame from host planes (dict name -> CPU tensor of the FULL frame, pinned for asynchronous copies) to this rank's
         rows of `composed`, written to the start of out_host (CPU float32 tensor of at least MAX_SHARE x the mean band height).
-        Returns the band (row0, row1) the rows belong to, after enqueueing."""
+        Returns the band (row0, row1) the rows belong to, after enqueueing.  Not with the TRAA tail: the rows uploaded here
+        (local_input_rows) are sized for the chain without it."""
+        if self.chain.traa is not None:
+            raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path does not render the TRAA tail")
         if self._host is None:
             self._host_init()
         h = self._host
@@ -398,7 +410,8 @@ class InProcessGroup:
     renders the bands one after the other on one GPU — the N-band logic (halo recomputation, owner lookup of history rows, carried texels,
     moving borders) without N GPUs; with one context per device it is a single-process multi-GPU host."""
 
-    def __init__(self, ctxs, chain_options, world: int):
+    def __init__(self, ctxs, chain_options, world: int, traa=None):
+        """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None"""
         import ctypes as C
 
         from . import abi, engine
@@ -408,6 +421,9 @@ class InProcessGroup:
         assert len(self.ctxs) == world
         self.lib = self.ctxs[0].lib
         self.chains = [engine.SsgiChain(c, chain_options) for c in self.ctxs]
+        if traa is not None:
+            for ch in self.chains:
+                ch.enable_traa(traa)
         self.groups = []
         for r, c in enumerate(self.ctxs):
             g = C.c_void_p()
