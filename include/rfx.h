@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define RFX_VERSION 2
+#define RFX_VERSION 3
 
 typedef enum rfx_status {
   RFX_OK = 0,
@@ -434,24 +434,6 @@ rfx_status rfx_ssgi_chain_reset(rfx_ssgi_chain* chain);
  * width/height (use a new chain to resize) and resets the temporal history like the reference's setters do. */
 rfx_status rfx_ssgi_chain_set_options(rfx_ssgi_chain* chain, const rfx_ssgi_chain_options* opt);
 rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame);
-/* Row-block sharded frame (SURVEY.md §8e): ranges[2k], ranges[2k+1] = output rows [a,b) of launch k in chain order
- * (K1, K2, K3 pass 0..2*denoiseIterations-1, K4, and the TRAA tail as one more launch when it is on).  The caller (realism_effects_b200/parallel.py) sizes
- * the ranges so that every pass finds valid halo rows produced locally by the previous pass, then all-gathers the
- * produced-then-gathered planes (composed, dnB[0..1]) across ranks.  Results are bit-identical to rfx_ssgi_chain_render. */
-rfx_status rfx_ssgi_chain_render_ranges(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame, const uint32_t* ranges,
-                                        uint32_t n_launches);
-/* General form: this rank owns `n_blocks` row blocks (block-cyclic assignment balances sky / floor content across ranks);
- * ranges[(blk*n_launches + k)*2 + {0,1}] = rows of launch k for block blk.  Only launches k in [k_begin, k_end) are issued,
- * which lets the caller split a frame into phases — K1 (needs last frame's `composed` gathered) | K2..K4 (need `dnB`
- * gathered) — so the dnB all-gather overlaps K1.  Per-frame state advances with the launch that consumes it. */
-rfx_status rfx_ssgi_chain_render_blocks(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame, const uint32_t* ranges,
-                                        uint32_t n_launches, uint32_t n_blocks, uint32_t k_begin, uint32_t k_end);
-/* One frame in three parts (for row-sharded callers that overlap the plane exchange with the ray march): part 0 = K1 ray march
- * only (reads depth / gbuffer; writes a context scratch record per ray), part 1 = K1 shading from those records (the only
- * reader of last frame's `composed`), part 2 = K2..K4.  Parts 0 and 1 together produce the bytes of the fused K1; issue them
- * in order 0, 1, 2 with the same frame and ranges.  ranges == NULL: whole planes (n_launches / n_blocks ignored). */
-rfx_status rfx_ssgi_chain_render_part(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame, const uint32_t* ranges,
-                                      uint32_t n_launches, uint32_t n_blocks, uint32_t part);
 /* TRAA frame tail: the second EffectPass of the reference demo's SSGI + TRAA frame (example/main.js:525-532) rendered by the chain
  * after K4 on every frame:  K5 ssgi_compose (of `composed`, depth and frame->direct_light, the composer input buffer SSGIEffect.update
  * binds) rounded to RGBA16F -> K2 in its TRAA form (temporal_reproject.frag with textureCount 1, inputType "diffuse", RGBA16F history
@@ -543,7 +525,7 @@ rfx_status rfx_group_get_last_bounds(const rfx_group* group, uint32_t* bounds); 
 rfx_status rfx_group_allgather_rows(rfx_group* group, void* stream, const rfx_plane* plane, const uint32_t* bounds);
 /* collective: one frame; this rank renders its band from full-frame input planes and joins the frame's collective on `stream` */
 rfx_status rfx_ssgi_chain_render_sharded(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame);
-/* pure host arithmetic, exported for hosts that drive the per-launch ranges themselves (and for the CPU tests):
+/* pure host arithmetic, exported for hosts that plan their bands with it (and for the CPU tests): the ranges render_sharded uses,
  * rows [ranges[2k], ranges[2k+1]) of launch k (K1, K2, K3 pass 0.., K4) for the band [own0, own1); n_launches = 3 + n_poisson_passes.
  * n_launches = 4 + n_poisson_passes: the same with the TRAA tail as the last launch; it runs on the band and K4 on the band widened
  * by RFX_TRAA_TAIL_ROWS (every earlier launch widens with it). */

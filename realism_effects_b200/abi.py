@@ -233,9 +233,6 @@ def _sig(lib):
     lib.rfx_ssgi_chain_render.argtypes = [vp, vp, _P(SsgiFrame)]
     lib.rfx_ssgi_chain_output.argtypes = [vp, C.c_int32, PP]
     lib.rfx_ssgi_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
-    lib.rfx_ssgi_chain_render_ranges.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32]
-    lib.rfx_ssgi_chain_render_blocks.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
-    lib.rfx_ssgi_chain_render_part.argtypes = [vp, vp, _P(SsgiFrame), _P(C.c_uint32), C.c_uint32, C.c_uint32, C.c_uint32]
     lib.rfx_ssgi_chain_render_host.argtypes = [vp, _P(SsgiHostFrame)]
     lib.rfx_ssgi_chain_submit_host.argtypes = [vp, _P(SsgiHostFrame)]
     lib.rfx_ssgi_chain_wait_host.argtypes = [vp, C.c_int32]
@@ -274,8 +271,8 @@ EXPORTS = [
     "rfx_temporal_reproject_launch", "rfx_poisson_denoise_launch", "rfx_gi_compose_launch", "rfx_ssgi_compose_launch", "rfx_hbao_launch", "rfx_hbao_launch_ex",
     "rfx_ao_compose_launch", "rfx_motion_blur_launch", "rfx_traa_compose_launch", "rfx_gbuffer_ingest_launch", "rfx_effects_launch", "rfx_taa_launch", "rfx_ssgi_chain_create", "rfx_ssgi_chain_destroy",
     "rfx_ssgi_chain_reset", "rfx_ssgi_chain_render", "rfx_ssgi_chain_output", "rfx_ssgi_chain_enable_traa", "rfx_ssgi_chain_render_host",
-    "rfx_ssgi_chain_submit_host", "rfx_ssgi_chain_wait_host", "rfx_ssgi_chain_render_part",
-    "rfx_ssgi_chain_set_profiling", "rfx_ssgi_chain_get_profile", "rfx_ssgi_chain_set_options", "rfx_ssgi_chain_render_ranges", "rfx_ssgi_chain_render_blocks",
+    "rfx_ssgi_chain_submit_host", "rfx_ssgi_chain_wait_host",
+    "rfx_ssgi_chain_set_profiling", "rfx_ssgi_chain_get_profile", "rfx_ssgi_chain_set_options",
     "rfx_plane_download_rows", "rfx_group_get_unique_id", "rfx_group_create", "rfx_group_create_inprocess", "rfx_group_attach_chains_inprocess", "rfx_group_destroy", "rfx_group_rank", "rfx_group_world", "rfx_group_uses_peer_reads",
     "rfx_group_attach_chain", "rfx_group_get_bounds", "rfx_group_set_bounds", "rfx_group_set_rebalance", "rfx_group_last_costs",
     "rfx_group_begin_frame", "rfx_group_get_last_bounds", "rfx_group_allgather_rows", "rfx_ssgi_chain_render_sharded", "rfx_shard_ranges",

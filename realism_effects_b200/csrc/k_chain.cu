@@ -30,14 +30,9 @@ __global__ void __launch_bounds__(256) cdecode_kernel(const CDecodeArgs a, int r
   const float k = mod_gl(g.z, 257.0f);  // float2color(...).r * 256 : the 9-bit roughness code (gbuffer_packing.glsl:24-34)
   st_f4(a.nrdz.p, a.nrdz.pitch, x, y, nrdz_pack(n, fminf(fmaxf(k, 0.0f), 256.0f), ld_r32f(a.depth, x, y)));
 }
-cudaError_t launch_cdecode(const CDecodeArgs& a, const RowSegs& segs, int halo, cudaStream_t s) {
-  for (int k = 0; k < segs.n; k++) {
-    int r0 = max(0, segs.r0[k] - halo), r1 = min(a.H, segs.r1[k] + halo);
-    if (k > 0) r0 = max(r0, min(a.H, segs.r1[k - 1] + halo));
-    if (r0 >= r1) continue;
-    dim3 grid((a.W + 31) / 32, (r1 - r0 + 7) / 8);
-    cdecode_kernel<<<grid, 256, 0, s>>>(a, r0, r1);
-  }
+cudaError_t launch_cdecode(const CDecodeArgs& a, int row0, int row1, int halo, cudaStream_t s) {
+  const int r0 = max(0, row0 - halo), r1 = min(a.H, row1 + halo);
+  if (r0 < r1) cdecode_kernel<<<dim3((a.W + 31) / 32, (r1 - r0 + 7) / 8), 256, 0, s>>>(a, r0, r1);
   return cudaGetLastError();
 }
 
@@ -194,7 +189,7 @@ RFX_D void c_temporal_planes(const CTemporalArgs& a, const CTState& s, v3 ruvD, 
 template <bool PEER>
 __global__ void __launch_bounds__(kThreads, 4) ctemporal_kernel(const __grid_constant__ CTemporalArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
   CTState s;
@@ -279,7 +274,7 @@ __global__ void __launch_bounds__(kThreads, 4) ctemporal_kernel(const __grid_con
 }
 
 cudaError_t launch_ctemporal(const CTemporalArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   if (a.hist.n > 1) ctemporal_kernel<true><<<grid, kThreads, 0, s>>>(a);
   else ctemporal_kernel<false><<<grid, kThreads, 0, s>>>(a);
   return cudaGetLastError();
@@ -288,72 +283,19 @@ cudaError_t launch_ctemporal(const CTemporalArgs& a, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------------------------------
 // K4 as a device function: constructGlobalIllumination (denoiser_compose_functions.glsl:53-107)
 // ------------------------------------------------------------------------------------------------------------------
-// Arithmetic precision is a template parameter because it was MEASURED to matter (tools/sweep_k1.sh: first 4K frame on H100):
-// the two fp16 inputs already sit up to one fp16 ulp (9.8e-4) from the oracle's, so composed pixels crowd the 1e-3 line.
-//   CM = 0  the exact K4's IEEE division / sqrt (k_denoise.cu: gi_compose_kernel): 1.8e-4 of the pixels outside 1e-3 — the default;
-//   CM = 1  SFU rcp / rsqrt / sqrt / ex2 (2^-22): 4.2e-4;
-//   CM = 2  SFU seed + one Newton step (<= 1 ulp): 4.2e-4 — no better than 1, so the residue is not the reciprocals' precision.
-// The pixel-centre fetch is the centre texel and pow(x, 5) is multiplies in every mode, as in the round-1 fast K4.
-template <int CM> RFX_D float cm_rsqrt(float x) {
-  if (CM == 0) return 1.0f / sqrtf(x);
-  const float y = fx_rsqrt(x);
-  if (CM == 1) return y;
-  return y * fma_(-0.5f * x * y, y, 1.5f);  // y (1.5 - 0.5 x y^2)
-}
-template <int CM> RFX_D float cm_rcp(float x) {
-  if (CM == 0) return 1.0f / x;
-  const float r = fx_rcp(x);
-  if (CM == 1) return r;
-  return r * fma_(-x, r, 2.0f);
-}
-template <int CM> RFX_D float cm_sqrt(float x) {
-  if (CM == 0) return sqrtf(x);
-  if (CM == 1) return fx_sqrt(x);
-  return x > 0.0f ? x * cm_rsqrt<2>(x) : 0.0f;
-}
-template <int CM> RFX_D v3 cm_normalize(v3 a) { return a * cm_rsqrt<CM>(dot(a, a)); }
-template <int CM> RFX_D v3 cm_unpack_normal(float packed) {
-  v2 f = unpackHalf2x16(__float_as_uint(packed));
-  f = f * 2.0f - 1.0f;
-  v3 n = mk3(f.x, f.y, 1.0f - fabsf(f.x) - fabsf(f.y));
-  const float t = fmaxf(-n.z, 0.0f);
-  n.x += n.x >= 0.0f ? -t : t;
-  n.y += n.y >= 0.0f ? -t : t;
-  return cm_normalize<CM>(n);
-}
-template <int CM> RFX_D v3 cm_byte3(uint32_t v) {  // floatToVec4(...).rgb
-  if (CM == 0) return mk3(fmaxf((float)(v & 0xFFu) / 255.0f - RFX_NON_ZERO_OFFSET, 0.0f), fmaxf((float)((v >> 8) & 0xFFu) / 255.0f - RFX_NON_ZERO_OFFSET, 0.0f),
-                          fmaxf((float)((v >> 16) & 0xFFu) / 255.0f - RFX_NON_ZERO_OFFSET, 0.0f));
-  const float k = 1.0f / 255.0f;
-  return mk3(fmaxf((float)(v & 0xFFu) * k - RFX_NON_ZERO_OFFSET, 0.0f), fmaxf((float)((v >> 8) & 0xFFu) * k - RFX_NON_ZERO_OFFSET, 0.0f),
-             fmaxf((float)((v >> 16) & 0xFFu) * k - RFX_NON_ZERO_OFFSET, 0.0f));
-}
-template <int CM>
-RFX_D v3 cm_sample_ggx_vndf(v3 V, float ax, float ay, float r1, float cphi, float sphi) {
-  const v3 Vh = cm_normalize<CM>(mk3(ax * V.x, ay * V.y, V.z));
-  const float lensq = Vh.x * Vh.x + Vh.y * Vh.y;
-  const v3 T1 = lensq > 0.0f ? mk3(-Vh.y, Vh.x, 0.0f) * cm_rsqrt<CM>(lensq) : mk3(1.0f, 0.0f, 0.0f);
-  const v3 T2 = cross(Vh, T1);
-  const float r = cm_sqrt<CM>(r1);
-  const float t1 = r * cphi;
-  float t2 = r * sphi;
-  const float sv = 0.5f * (1.0f + Vh.z);
-  t2 = (1.0f - sv) * cm_sqrt<CM>(1.0f - t1 * t1) + sv * t2;
-  const v3 Nh = t1 * T1 + t2 * T2 + cm_sqrt<CM>(fmaxf(0.0f, 1.0f - t1 * t1 - t2 * t2)) * Vh;
-  return cm_normalize<CM>(mk3(ax * Nh.x, ay * Nh.y, fmaxf(0.0f, Nh.z)));
-}
-template <int CM>
-RFX_D float4 c_compose_t(const CamD& cam, int x, int y, int W, int H, float4 g, float rough0, float depth, v3 dgi, v3 sgi) {
+// The arithmetic is the exact K4's IEEE division / sqrt (k_denoise.cu: gi_compose_kernel): the two fp16 inputs already sit up to
+// one fp16 ulp (9.8e-4) from the oracle's, so composed pixels crowd the 1e-3 line, and SFU reciprocals were measured to more than
+// double the pixels outside it (DESIGN.md §2).  The pixel-centre fetch is the centre texel and pow(x, 5) is multiplies.
+RFX_D float4 c_compose(const CamD& cam, int x, int y, int W, int H, float4 g, float rough0, float depth, v3 dgi, v3 sgi) {
   const v2 vUv = pixel_uv(x, y, W, H);
-  const v3 diffuse = cm_byte3<CM>(__float_as_uint(g.x));
-  const v3 wn = cm_unpack_normal<CM>(g.y);  // the exact packed normal (the nrdz copy carries the roughness code in its low mantissa bits)
+  const v3 diffuse = xyz(floatToVec4(g.x));
+  const v3 wn = unpackNormal(g.y);  // the exact packed normal (the nrdz copy carries the roughness code in its low mantissa bits)
   const float metalness = gb_metalness(g.z);
-  const uint32_t ev = __float_as_uint(g.w);
-  const float ew = CM == 0 ? fmaxf((float)(ev >> 24) / 255.0f - RFX_NON_ZERO_OFFSET, 0.0f) : fmaxf((float)(ev >> 24) * (1.0f / 255.0f) - RFX_NON_ZERO_OFFSET, 0.0f);
-  const float fexp = ew * 255.0f - 128.0f;
-  const v3 emissive = cm_byte3<CM>(ev) * (CM == 0 ? exp2f(fexp) : fx_ex2(fexp));  // decodeRGBE8
+  const v4 e = floatToVec4(g.w);
+  const float fexp = e.w * 255.0f - 128.0f;
+  const v3 emissive = xyz(e) * exp2f(fexp);  // decodeRGBE8
   const v3 viewNormal = mul_dir_left(wn, cam.camera_matrix_world);
-  const float gz = cam.perspective ? (cam.near_plane * cam.far_plane) * cm_rcp<CM>((cam.far_plane - cam.near_plane) * depth - cam.far_plane)
+  const float gz = cam.perspective ? (cam.near_plane * cam.far_plane) * (1.0f / ((cam.far_plane - cam.near_plane) * depth - cam.far_plane))
                                    : orthographicDepthToViewZ(depth, cam.near_plane, cam.far_plane);
   const float viewZ = -gz;
   const float clipW = cam.projection.m[2 * 4 + 3] * viewZ + cam.projection.m[3 * 4 + 3];
@@ -361,26 +303,22 @@ RFX_D float4 c_compose_t(const CamD& cam, int x, int y, int W, int H, float4 g, 
   clip = mk4(clip.x * clipW, clip.y * clipW, clip.z * clipW, clip.w * clipW);
   v3 viewPos = xyz(mul(cam.projection_inverse, clip));
   viewPos.z = -viewZ;
-  const v3 viewDir = cm_normalize<CM>(viewPos);
+  const v3 viewDir = normalize(viewPos);
   const float roughness = rough0 * rough0;
   const v3 N = mul_dir_left(viewNormal, cam.view_matrix);
   v3 T, B;
   const v3 v = -viewDir;
   v3 V = mul_dir_left(v, cam.view_matrix);
-  {  // Onb
-    const v3 up = fabsf(N.z) < 0.9999999f ? mk3(0, 0, 1) : mk3(1, 0, 0);
-    T = cm_normalize<CM>(cross(up, N));
-    B = cross(N, T);
-  }
+  Onb(N, T, B);
   V = ToLocal(T, B, N, V);
-  v3 Hh = cm_sample_ggx_vndf<CM>(V, roughness, roughness, 0.25f, -4.37113883e-08f, 1.0f);  // r2 = 0.25: (cos, sin) of fp32(pi/2)
+  v3 Hh = SampleGGXVNDF_cs(V, roughness, roughness, 0.25f, -4.37113883e-08f, 1.0f);  // r2 = 0.25: (cos, sin) of fp32(pi/2)
   if (Hh.z < 0.0f) Hh = -Hh;
-  v3 l = cm_normalize<CM>(reflect(-V, Hh));
+  v3 l = normalize(reflect(-V, Hh));
   l = ToWorld(T, B, N, l);
   l = xyz(mul(mk4(l, 1.0f), cam.camera_matrix_world));
-  l = cm_normalize<CM>(l);
+  l = normalize(l);
   if (dot(viewNormal, l) < 0.0f) l = -l;
-  const v3 h = cm_normalize<CM>(v + l);
+  const v3 h = normalize(v + l);
   const float VoH = fmaxf(1e-6f, dot(v, h));
   const v3 f0 = mix(mk3(0.04f), diffuse, metalness);
   const float omv = 1.0f - VoH, omv2 = omv * omv;
@@ -388,21 +326,11 @@ RFX_D float4 c_compose_t(const CamD& cam, int x, int y, int W, int H, float4 g, 
   const v3 gi = diffuse * (1.0f - metalness) * (mk3(1.0f) - F) * dgi + sgi * F + emissive;
   return make_float4(gi.x, gi.y, gi.z, 1.0f);
 }
-RFX_D float4 c_compose(int mode, const CamD& cam, int x, int y, int W, int H, float4 g, float rough0, float depth, v3 dgi, v3 sgi) {
-  if (mode == 0) return c_compose_t<0>(cam, x, y, W, H, g, rough0, depth, dgi, sgi);
-  if (mode == 1) return c_compose_t<1>(cam, x, y, W, H, g, rough0, depth, dgi, sgi);
-  return c_compose_t<2>(cam, x, y, W, H, g, rough0, depth, dgi, sgi);
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // K3  Poisson pass on the interleaved planes.  FIRST: `in` = tr (fp32, NEAREST); else `in` = dn (fp16, LINEAR).
 // Arithmetic = poisson_fast_kernel (k_denoise.cu): colours in log2 units, merged exponents.
 // ------------------------------------------------------------------------------------------------------------------
-RFX_D bool in_segs(const RowSegs& s, int y) {
-  bool r = false;
-  for (int k = 0; k < s.n; k++) r = r || (y >= s.r0[k] && y < s.r1[k]);
-  return r;
-}
 RFX_D v3 cp_log1p(v3 c) { return mk3(fx_lg2(c.x + 1.0f), fx_lg2(c.y + 1.0f), fx_lg2(c.z + 1.0f)); }
 #define CP_LUM_C (-0.06609580f) /* 0.125 * log2(ln 2) */
 RFX_D float cp_lum(v3 c2) { return fx_ex2(fma_(0.125f, fx_lg2(dot(mk3(0.2125f, 0.7154f, 0.0721f), c2)), CP_LUM_C)); }
@@ -515,10 +443,10 @@ RFX_D void cpoisson_body(const CPoissonArgs& a, int x, int y, float4 nc, float f
   q.x = pack_h2(f2lo(orr), f2lo(og)); q.y = pack_h2(f2lo(ob), f2lo(alpha)); q.z = pack_h2(f2hi(orr), f2hi(og)); q.w = pack_h2(f2hi(ob), f2hi(alpha));
   *((uint4*)(a.out.p + ((unsigned)y * (unsigned)a.out.pitch + (unsigned)x * 16u))) = q;
   if (COMPOSE) {
-    if (in_segs(a.csegs, y)) {  // K4 reads the fp16 texel just stored (DenoiserComposePass.js:66-67)
+    if (y >= a.crow0 && y < a.crow1) {  // K4 reads the fp16 texel just stored (DenoiserComposePass.js:66-67)
       const float4 g = ld_f4(a.gb, x, y);
       st_f4(a.composed.p, a.composed.pitch, x, y,
-            c_compose(a.compose_mode, a.cam, x, y, a.W, a.H, g, roughness, depth, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
+            c_compose(a.cam, x, y, a.W, a.H, g, roughness, depth, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
     }
   }
 }
@@ -526,7 +454,7 @@ RFX_D void cpoisson_body(const CPoissonArgs& a, int x, int y, float4 nc, float f
 template <bool FIRST, bool COMPOSE>
 __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_constant__ CPoissonArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
   const float4 nc = ld_f4(a.nrdz, xc, yc);
@@ -539,7 +467,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_cons
       const unsigned off = (unsigned)y * (unsigned)a.carry.local.pitch + (unsigned)x * 16u;
       *((uint4*)(a.out.p + ((unsigned)y * (unsigned)a.out.pitch + (unsigned)x * 16u))) = *((const uint4*)(peer_row_base(a.carry, y) + off));
     }
-    if (COMPOSE && a.composed_carry.local.p && in_segs(a.csegs, y)) {
+    if (COMPOSE && a.composed_carry.local.p && y >= a.crow0 && y < a.crow1) {
       const unsigned off = (unsigned)y * (unsigned)a.composed_carry.local.pitch + (unsigned)x * 16u;
       st_f4(a.composed.p, a.composed.pitch, x, y, *((const float4*)(peer_row_base(a.composed_carry, y) + off)));
     }
@@ -555,7 +483,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_cons
 }
 
 cudaError_t launch_cpoisson(const CPoissonArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   if (a.first) { if (a.compose) cpoisson_kernel<true, true><<<grid, kThreads, 0, s>>>(a); else cpoisson_kernel<true, false><<<grid, kThreads, 0, s>>>(a); }
   else { if (a.compose) cpoisson_kernel<false, true><<<grid, kThreads, 0, s>>>(a); else cpoisson_kernel<false, false><<<grid, kThreads, 0, s>>>(a); }
   return cudaGetLastError();
@@ -589,7 +517,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_
   __shared__ unsigned long long bar;
   const CPoissonArgs& a = t.a;
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   int lx, ly;
   lane_to_pixel(threadIdx.x & 31, lx, ly);
@@ -625,7 +553,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_
       const unsigned off = (unsigned)y * (unsigned)a.carry.local.pitch + (unsigned)x * 16u;
       *((uint4*)(a.out.p + ((unsigned)y * (unsigned)a.out.pitch + (unsigned)x * 16u))) = *((const uint4*)(peer_row_base(a.carry, y) + off));
     }
-    if (COMPOSE && a.composed_carry.local.p && in_segs(a.csegs, y)) {
+    if (COMPOSE && a.composed_carry.local.p && y >= a.crow0 && y < a.crow1) {
       const unsigned off = (unsigned)y * (unsigned)a.composed_carry.local.pitch + (unsigned)x * 16u;
       st_f4(a.composed.p, a.composed.pitch, x, y, *((const float4*)(peer_row_base(a.composed_carry, y) + off)));
     }
@@ -636,7 +564,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_
 }
 
 cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s) {
-  dim3 grid((t.a.W + kTileW - 1) / kTileW, t.a.segs.tiles);
+  dim3 grid((t.a.W + kTileW - 1) / kTileW, row_tiles(t.a.row0, t.a.row1));
   const size_t tile_bytes = (size_t)t.box_w * t.box_h * 16, smem = ((tile_bytes + 127) & ~(size_t)127) + tile_bytes;
   static bool attr_set = false;
   if (!attr_set) {
@@ -652,7 +580,7 @@ cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s) {
 // stand-alone K4 (denoiseIterations == 0: no Poisson pass to ride on)
 __global__ void __launch_bounds__(kThreads) ccompose_kernel(const __grid_constant__ CComposeArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
   const float4 nc = ld_f4(a.nrdz, xc, yc);
@@ -668,10 +596,10 @@ __global__ void __launch_bounds__(kThreads) ccompose_kernel(const __grid_constan
   const uint4 q = __ldg((const uint4*)(a.dn.p + ((unsigned)y * (unsigned)a.dn.pitch + (unsigned)x * 16u)));
   const float4 g = ld_f4(a.gb, x, y);
   st_f4(a.composed.p, a.composed.pitch, x, y,
-        c_compose(a.compose_mode, a.cam, x, y, a.W, a.H, g, nrdz_roughness(nc), nc.w, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
+        c_compose(a.cam, x, y, a.W, a.H, g, nrdz_roughness(nc), nc.w, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
 }
 cudaError_t launch_ccompose(const CComposeArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   ccompose_kernel<<<grid, kThreads, 0, s>>>(a);
   return cudaGetLastError();
 }

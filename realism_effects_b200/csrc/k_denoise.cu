@@ -21,7 +21,7 @@ RFX_D v4 fetch_in(const PV& t, v2 uv) {
 template <int TC, bool GB, bool LINEAR, bool HALF>
 __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant__ PoissonArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   // helper pixels beyond the edge evaluate at the clamped texel (clamp-to-edge sampling)
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
@@ -127,17 +127,12 @@ __global__ void __launch_bounds__(256) gbuffer_decode_kernel(PV gb, OutV nrd, in
   const float r = gbuffer_texture ? gb_roughness(g.z) : g.w;
   st_f4(nrd.p, nrd.pitch, x, y, make_float4(n.x, n.y, n.z, r));
 }
-// Decodes the rows the Poisson taps of `segs` can reach: every output segment widened by `halo` rows (ceil(radius) + 1: tap offsets
-// are at most `radius` pixels, + 1 for the quad-derivative helper row).  A rank that owns a few row blocks of a tall frame decodes
-// those bands only, not the whole plane.
-cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_texture, const RowSegs& segs, int halo, cudaStream_t s) {
-  for (int k = 0; k < segs.n; k++) {
-    int r0 = max(0, segs.r0[k] - halo), r1 = min(H, segs.r1[k] + halo);
-    if (k > 0) r0 = max(r0, min(H, segs.r1[k - 1] + halo));  // segments are ascending: skip rows the previous band already covered
-    if (r0 >= r1) continue;
-    dim3 grid((W + 31) / 32, (r1 - r0 + 7) / 8);
-    gbuffer_decode_kernel<<<grid, 256, 0, s>>>(gb, nrd, W, r0, r1, gbuffer_texture);
-  }
+// Decodes the rows the Poisson taps of output rows [row0, row1) can reach: the range widened by `halo` rows (ceil(radius) + 1: tap
+// offsets are at most `radius` pixels, + 1 for the quad-derivative helper row).  A rank that owns a band of a tall frame decodes
+// that band only, not the whole plane.
+cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_texture, int row0, int row1, int halo, cudaStream_t s) {
+  const int r0 = max(0, row0 - halo), r1 = min(H, row1 + halo);
+  if (r0 < r1) gbuffer_decode_kernel<<<dim3((W + 31) / 32, (r1 - r0 + 7) / 8), 256, 0, s>>>(gb, nrd, W, r0, r1, gbuffer_texture);
   return cudaGetLastError();
 }
 
@@ -198,7 +193,7 @@ template <int TC, bool LINEAR, bool GB>
 #endif
 __global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kernel(const __grid_constant__ PoissonArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
@@ -286,7 +281,7 @@ __global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kern
 }
 
 cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   if (a.input_linear && !a.in_half) return cudaErrorInvalidValue;
   if (!a.input_linear && a.in_half) return cudaErrorNotSupported;
 #define RFX_PF(TC, LIN) do { if (a.gbuffer_texture) poisson_fast_kernel<TC, LIN, true><<<grid, kThreads, 0, s>>>(a); else poisson_fast_kernel<TC, LIN, false><<<grid, kThreads, 0, s>>>(a); } while (0)
@@ -297,7 +292,7 @@ cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s) {
 }
 
 cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
 #define RFX_LP(TC, GB, LIN, HALF) poisson_kernel<TC, GB, LIN, HALF><<<grid, kThreads, 0, s>>>(a)
   const bool lin = a.input_linear, half = a.in_half, gb = a.gbuffer_texture;
   if (lin && !half) return cudaErrorInvalidValue;
@@ -314,7 +309,7 @@ cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s) {
 
 __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_constant__ ComposeArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const int xc = min(x, a.W - 1), yc = min(y, a.H - 1);
   const float depth = ld_r32f(a.depth, xc, yc);
@@ -382,7 +377,7 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
 }
 
 cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   gi_compose_kernel<<<grid, kThreads, 0, s>>>(a);
   return cudaGetLastError();
 }

@@ -12,25 +12,11 @@
 //   * when the projection matrix has the perspective sparsity pattern (detected on the host) the
 //     fma chain of `projectionMatrix * vec4(p, 1)` drops its exact-zero terms: x' = fma(P00,x,P20*z),
 //     y' = fma(P11,y,P21*z), w' = -z — bit-identical to the full chain;
-//   * the ray positions do not depend on the fetched depths, so the taps of a batch of RFX_MARCH_BATCH steps can be
-//     issued together and tested in order (tunable; see the sweep note at the macro).
+//   * the fast variant (ssgi_fast_kernel) projects and fetches RFX_K1_BATCH march steps together and tests them in order.
 // All blue-noise driven transcendentals (sin/cos of 2*pi*k/255, the march step profile
 // 1-exp(-0.25 (i+b-0.5)^2)) come from small host-built tables indexed by the 8-bit noise value.
 // FAST = true additionally moves the remaining continuous transcendentals to the SFU pipe.
 #include "rfx_kernels.h"
-
-// Taps issued per march batch.  Batching trades wasted speculative taps after the first hit (plus registers) against
-// memory-level parallelism; at 4 resident blocks per SM the other warps already hide the L2 latency, so the default is a plain
-// dependent loop.
-#ifndef RFX_MARCH_BATCH
-#define RFX_MARCH_BATCH 1
-#endif
-// 1: the march as the shader's plain loop + fma(x, 0.5, 0.5) for the screen uv (bit-identical by construction, ~100 fewer
-// instructions per pixel).  Written at the end of round 1 with no GPU time left to re-run parity, so it ships disabled;
-// tools/next_round_sweeps.sh measures it.
-#ifndef RFX_K1_SIMPLE_MARCH
-#define RFX_K1_SIMPLE_MARCH 0
-#endif
 
 namespace rfx {
 
@@ -66,12 +52,11 @@ RFX_D float ssgi_view_z(const SsgiArgs& a, float depth) {
 
 // prepass: viewZ plane = getViewZ(depth), same arithmetic as the shader => bit-identical taps
 __global__ void __launch_bounds__(256) viewz_kernel(PV depth, OutV vz, int W, int H, float near_mul_far, float far_minus_near, float near_minus_far,
-                                                    float near_plane, float far_plane, int perspective, int tiles_x) {
+                                                    float near_plane, float far_plane, int perspective) {
   const int x = (blockIdx.x * 256 + threadIdx.x) * 4, y = blockIdx.y;
   if (x >= W) return;
   const float* src = (const float*)(depth.p + (long long)y * depth.pitch) + x;
-  // tiles_x > 0: 8x4-texel tiles, 32 floats each (x is a multiple of 4, so the four texels stay inside one tile row)
-  float* dst = tiles_x > 0 ? (float*)vz.p + ((size_t)((y >> 2) * tiles_x + (x >> 3)) * 32 + ((y & 3) << 3) + (x & 7)) : (float*)(vz.p + (long long)y * vz.pitch) + x;
+  float* dst = (float*)(vz.p + (long long)y * vz.pitch) + x;
   float d[4];
   if (x + 3 < W) { const float4 t = __ldg((const float4*)src); d[0] = t.x; d[1] = t.y; d[2] = t.z; d[3] = t.w; }
   else { for (int i = 0; i < 4; i++) d[i] = x + i < W ? __ldg(src + i) : 0.0f; }
@@ -85,7 +70,7 @@ cudaError_t launch_viewz(const SsgiArgs& a, OutV vz, cudaStream_t s) {
   const int W = a.depth.w, H = a.depth.h;  // the depth plane's own size (larger than the render target when resolutionScale < 1)
   dim3 grid((W / 4 + 255) / 256 + 1, H);
   viewz_kernel<<<grid, 256, 0, s>>>(a.depth, vz, W, H, a.near_mul_far, a.far_minus_near, a.near_minus_far, a.cam.near_plane, a.cam.far_plane,
-                                    a.cam.perspective, a.vz_tiled ? a.vz_tiles_x : 0);
+                                    a.cam.perspective);
   return cudaGetLastError();
 }
 
@@ -104,19 +89,11 @@ RFX_D v2 view_to_screen(const SsgiArgs& a, v3 p) {
     cw = fma_(M[3], p.x, fma_(M[7], p.y, fma_(M[11], p.z, M[15])));
   }
   const float r = rcp_<AP>(cw);
-#if RFX_K1_SIMPLE_MARCH
-  // x * 0.5 is exact, so fma(x, 0.5, 0.5) rounds exactly like the shader's (x * 0.5) + 0.5: one instruction instead of two
-  return mk2(fma_(cx * r, 0.5f, 0.5f), fma_(cy * r, 0.5f, 0.5f));
-#else
   return mk2((cx * r) * 0.5f + 0.5f, (cy * r) * 0.5f + 0.5f);
-#endif
 }
 
-// 1: polynomial atan2 / acos (Abramowitz-Stegun 4.4.49 / 4.4.46 evaluated in fp32: 3e-7 / 1.3e-5 rad, i.e. < 0.003 texel of a
-// 512-row env map) for the fast variant's env lookup, ~45 instructions per fetch fewer than libm.  Unmeasured in round 1, so off.
-#ifndef RFX_K1_FAST_TRIG
-#define RFX_K1_FAST_TRIG 0  /* round-1 kernels; the round-2 fast kernel always uses the polynomials (env_uv_fast) */
-#endif
+// Polynomial atan2 / acos (Abramowitz-Stegun 4.4.49 / 4.4.46 evaluated in fp32: 3e-7 / 1.3e-5 rad, i.e. < 0.003 texel of a
+// 512-row env map) for the fast kernel's env lookup, ~45 instructions per fetch fewer than libm.
 RFX_D float acos_poly(float x) {
   const float ax = fabsf(x);
   float p = -0.0012624911f;
@@ -144,7 +121,7 @@ RFX_D float atan2_poly(float y, float x) {
 
 template <bool AP, bool POLY = false>
 RFX_D v2 equirectDirectionToUv(v3 d) {  // ssgi_utils.frag:64-74
-  v2 uv = (AP && (POLY || RFX_K1_FAST_TRIG)) ? mk2(atan2_poly(d.z, d.x), acos_poly(d.y)) : mk2(atan2f(d.z, d.x), acosf(d.y));
+  v2 uv = POLY ? mk2(atan2_poly(d.z, d.x), acos_poly(d.y)) : mk2(atan2f(d.z, d.x), acosf(d.y));
   uv = mk2(div_<AP>(uv.x, 2.0f * PI_F), div_<AP>(uv.y, PI_F));
   uv.x += 0.5f;
   uv.y = 1.0f - uv.y;
@@ -263,41 +240,12 @@ RFX_D v2 rayMarch(const SsgiArgs& a, v3& dir, v3& hitPos, int noiseB, bool& hit)
   v2 uv = mk2(0.0f, 0.0f);
   hit = false;
   const float* cs_row = a.step_table + noiseB;  // cs(i, b) at [(i-1)*256 + b]
-#if RFX_K1_SIMPLE_MARCH && RFX_MARCH_BATCH == 1
-  for (int i = 1; i < a.steps; i++, cs_row += 256) {  // the shader's loop as it stands: no batch scaffolding
+  for (int i = 1; i < a.steps && !hit; i++, cs_row += 256) {
     hitPos = hitPos + dir * __ldg(cs_row);
     uv = view_to_screen<SPARSE, AP>(a, hitPos);
     const float diff = tex_r32f_nearest(a.viewz, uv) - hitPos.z;
-    if (diff >= 0.0f && diff < a.thickness) { hit = true; break; }
+    hit = diff >= 0.0f && diff < a.thickness;
   }
-#else
-  int i = 1;
-  while (i < a.steps && !hit) {
-    v3 pos[RFX_MARCH_BATCH];
-    v2 uvs[RFX_MARCH_BATCH];
-    float vzs[RFX_MARCH_BATCH];
-    v3 p = hitPos;
-#pragma unroll
-    for (int k = 0; k < RFX_MARCH_BATCH; k++) {  // issue the whole batch of taps before testing any
-      const int ii = min(i + k, a.steps - 1);
-      const float cs = __ldg(cs_row + (ii - 1) * 256);
-      p = p + dir * cs;
-      pos[k] = p;
-      uvs[k] = view_to_screen<SPARSE, AP>(a, p);
-      vzs[k] = tex_r32f_nearest(a.viewz, uvs[k]);
-    }
-#pragma unroll
-    for (int k = 0; k < RFX_MARCH_BATCH; k++) {
-      if (!hit && i + k < a.steps) {
-        const float diff = vzs[k] - pos[k].z;
-        hitPos = pos[k];
-        uv = uvs[k];
-        if (diff >= 0.0f && diff < a.thickness) hit = true;
-      }
-    }
-    i += RFX_MARCH_BATCH;
-  }
-#endif
   if (!hit) {
     hitPos = mk3(10.0e9f);
     return uv;
@@ -320,16 +268,10 @@ struct PixelMat {
   float roughness, metalness;
 };
 
-// Split-phase K1 (row-sharded multi-GPU frames): PHASE 1 marches the rays - it needs the depth plane only - and stores one
-// float4 per ray; PHASE 2 repeats the (deterministic) per-pixel prologue, takes the march result from the record instead of
-// marching and does everything that samples last frame's `composed`.  The exchange of `composed` between the GPUs runs under
-// PHASE 1 of the next frame.  PHASE 0 is the fused kernel.  Record: hit -> (hitPos.xyz, 1); miss -> (10e9, uv.x, uv.y, 0).
-RFX_D float4 march_record(bool hit, v3 hitPos, v2 uv) { return hit ? make_float4(hitPos.x, hitPos.y, hitPos.z, 1.0f) : make_float4(10.0e9f, uv.x, uv.y, 0.0f); }
-
 // doSample  ssgi.frag:362-439
-template <bool SPARSE, bool FAST, int PHASE>
+template <bool SPARSE, bool FAST>
 RFX_D v3 doSample(const SsgiArgs& a, const PixelMat& m, v3 viewPos, v3 viewNormal, float roughnessSq, bool isDiffuseSample, bool isEnvSample,
-                  float NoV, float NoL, float NoH, float LoH, int noiseB, v3& l, v3& hitPos, float& brdf, float& pdf, const float4* rec) {
+                  float NoV, float NoL, float NoH, float LoH, int noiseB, v3& l, v3& hitPos, float& brdf, float& pdf) {
   const float cosTheta = fmaxf(0.0f, dot(viewNormal, l));
   if (isDiffuseSample) {
     brdf = evalDisneyDiffuse<FAST>(NoL, NoV, LoH, roughnessSq, m.metalness);
@@ -342,22 +284,7 @@ RFX_D v3 doSample(const SsgiArgs& a, const PixelMat& m, v3 viewPos, v3 viewNorma
   pdf = fmaxf(SSGI_EPSILON, pdf);
   hitPos = viewPos;
   bool hit;
-  v2 coords;
-  if (PHASE == 2) {  // the march ran in the PHASE 1 launch; replay its effect on hitPos, the hit uv and the in-place scaled direction
-    const float4 r = *rec;
-    hit = r.w != 0.0f;
-    l = l * (a.ray_distance / (float)a.steps);
-    if (hit) {
-      hitPos = mk3(r.x, r.y, r.z);
-      coords = view_to_screen<SPARSE, FAST>(a, hitPos);  // what rayMarch returns for a hit, with or without refinement
-      if (a.refine_steps > 0) { l = l * 0.5f; for (int k = 0; k < a.refine_steps; k++) l = l * 0.5f; }
-    } else {
-      hitPos = mk3(10.0e9f);
-      coords = mk2(r.y, r.z);
-    }
-  } else {
-    coords = rayMarch<SPARSE, FAST>(a, l, hitPos, noiseB, hit);
-  }
+  const v2 coords = rayMarch<SPARSE, FAST>(a, l, hitPos, noiseB, hit);
   const bool allowMissedRays = (a.flags & RFX_SSGI_MISSED_RAYS) != 0;
   if (!hit && !allowMissedRays) return getEnvColor<FAST>(a, l, roughnessSq, isDiffuseSample, isEnvSample);
   v2 vel = mk2(0.0f, 0.0f);
@@ -389,16 +316,13 @@ RFX_D v3 doSample(const SsgiArgs& a, const PixelMat& m, v3 viewPos, v3 viewNorma
   return SSGI;
 }
 
-template <int MODE, bool IS, bool SPARSE, bool FAST, int PHASE>
+template <int MODE, bool IS, bool SPARSE, bool FAST>
 #ifndef RFX_K1_MIN_BLOCKS
 #define RFX_K1_MIN_BLOCKS 4  // 64 registers/thread, 4 blocks (32 warps) per SM.  tools/sweep_k1.sh on H100 at 4K: 3 and 4 give the same K1 time, 5 is ~10 % slower
 #endif
-#ifndef RFX_K1_MARCH_MIN_BLOCKS
-#define RFX_K1_MARCH_MIN_BLOCKS 8  // march-only phase of row-sharded groups: L2-latency bound, so occupancy wins over the spills of its prologue
-#endif
-__global__ void __launch_bounds__(kThreads, PHASE == 1 ? RFX_K1_MARCH_MIN_BLOCKS : RFX_K1_MIN_BLOCKS) ssgi_kernel(const __grid_constant__ SsgiArgs a) {
+__global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_kernel(const __grid_constant__ SsgiArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const uchar4 bn = __ldg(a.blue.tex + ((y + a.blue.shift.sy) % a.blue.size) * a.blue.size + ((x + a.blue.shift.sx) % a.blue.size));
   const v4 random = mk4((float)bn.x / 255.0f, (float)bn.y / 255.0f, (float)bn.z / 255.0f, (float)bn.w / 255.0f);
@@ -423,7 +347,6 @@ __global__ void __launch_bounds__(kThreads, PHASE == 1 ? RFX_K1_MARCH_MIN_BLOCKS
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
   const float unpackedDepth = a.scaled ? tex_r32f_nearest(a.depth, vUv) : ld_r32f(a.depth, x, y);  // scaled: NEAREST by uv in the full-size plane
   if (unpackedDepth == 1.0f) {  // background :109-113
-    if (PHASE == 1) return;
     v4 dl = mk4(0.0f, 0.0f, 0.0f, 1.0f);
     if (a.direct.p) dl = tex_h4_linear(a.direct, vUv);
     st_f4(a.out.p, a.out.pitch, x, y, packTwoVec4(dl, dl));
@@ -506,29 +429,13 @@ __global__ void __launch_bounds__(kThreads, PHASE == 1 ? RFX_K1_MARCH_MIN_BLOCKS
   const v3 diffuseRay = emsIsEnvSample ? envMisDir : cosineSampleHemisphere_cs<FAST>(viewNormal, random.x, sc.x, sc.y);
   const v3 specularRay = emsIsEnvSample ? envMisDir : l;
 
-  float4* rec = PHASE != 0 ? (float4*)(a.rec + (long long)y * a.rec_pitch) + 2 * x : nullptr;
-  if (PHASE == 1) {  // march only
-    float4 r0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    if (MODE == RFX_MODE_SSGI && isDiffuseSample) {
-      v3 d = diffuseRay, hp = viewPos;
-      bool hit;
-      const v2 uv = rayMarch<SPARSE, FAST>(a, d, hp, bn.z, hit);
-      r0 = march_record(hit, hp, uv);
-    }
-    v3 d = specularRay, hp = viewPos;
-    bool hit;
-    const v2 uv = rayMarch<SPARSE, FAST>(a, d, hp, bn.z, hit);
-    rec[0] = r0;
-    rec[1] = march_record(hit, hp, uv);
-    return;
-  }
   v3 diffuseGI = mk3(0.0f), specularGI = mk3(0.0f), hitPos = mk3(0.0f);
   float brdf, pdf;
   bool haveDiffuse = false;
   if (MODE == RFX_MODE_SSGI && isDiffuseSample) {  // :222-242
     l = diffuseRay;
     calculateAngles<FAST>(l, v, n, NoL, NoH, LoH, VoH);
-    v3 gi = doSample<SPARSE, FAST, PHASE>(a, m, viewPos, viewNormal, roughnessSq, true, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf, rec);
+    v3 gi = doSample<SPARSE, FAST>(a, m, viewPos, viewNormal, roughnessSq, true, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf);
     gi = gi * brdf;
     if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<FAST>(aa, aa + bb); } else gi = vdiv_<FAST>(gi, pdf);
     gi = vdiv_<FAST>(gi, emsPdf);
@@ -538,8 +445,7 @@ __global__ void __launch_bounds__(kThreads, PHASE == 1 ? RFX_K1_MARCH_MIN_BLOCKS
   l = specularRay;  // :246-265
   calculateAngles<FAST>(l, v, n, NoL, NoH, LoH, VoH);
   {
-    v3 gi = doSample<SPARSE, FAST, PHASE>(a, m, viewPos, viewNormal, roughnessSq, isDiffuseSample, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf,
-                                          rec + 1);
+    v3 gi = doSample<SPARSE, FAST>(a, m, viewPos, viewNormal, roughnessSq, isDiffuseSample, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf);
     gi = gi * brdf;
     if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<FAST>(aa, aa + bb); } else gi = vdiv_<FAST>(gi, pdf);
     gi = vdiv_<FAST>(gi, emsPdf);
@@ -569,7 +475,7 @@ __global__ void __launch_bounds__(kThreads, PHASE == 1 ? RFX_K1_MARCH_MIN_BLOCKS
 }
 
 // ==========================================================================================================================
-// K1, fast variant (fast_math on, fused phase): same shader, restructured for what bounds it (issue
+// K1, fast variant (fast_math on, full-size target): same shader, restructured for what bounds it (issue
 // 68 %, 22.5 of 32 lanes active, 58 instructions per march tap).  Tried and dropped: compacting the
 // diffuse rays of a block through shared memory so that full warps trace them — lane use stayed at 22 / 32 (the waste is rays
 // leaving the loop at different steps, not the lottery) while the two block barriers cost 0.1 ms.
@@ -590,7 +496,6 @@ RFX_D float tap_viewz(const SsgiArgs& a, v3 p) {
     t = mkf2(uv.x * (float)a.W, uv.y * (float)a.H);
   }
   const int ix = clamp_idx(__float2int_rd(f2lo(t)), a.W - 1), iy = clamp_idx(__float2int_rd(f2hi(t)), a.H - 1);
-  if (a.vz_tiled) return __ldg((const float*)a.viewz.p + (((iy >> 2) * a.vz_tiles_x + (ix >> 3)) * 32 + ((iy & 3) << 3) + (ix & 7)));
   return __ldg((const float*)a.viewz.p + (iy * a.vz_pitchw + ix));
 }
 RFX_D v3 fma3(v3 d, float s, v3 p) {
@@ -600,9 +505,13 @@ RFX_D v3 fma3(v3 d, float s, v3 p) {
 // RayMarch + BinarySearch  ssgi.frag:441-503.  The ray positions do not depend on the fetched depths, so BATCH steps are projected
 // and fetched together and tested in order: the march is a chain of dependent L2-latency gathers (L1 hit ~50 %), and at ~25
 // instructions per tap the other resident warps no longer hide that latency on their own (at most BATCH - 1 wasted taps per hit).
-// BATCH is picked at run time (SsgiArgs::march_batch; RFX_K1_BATCH in the environment) from {1, 2, 4}.
-template <bool SPARSE, int BATCH>
+#ifndef RFX_K1_BATCH
+#define RFX_K1_BATCH 4  // tools/sweep_k1.sh on H100 at 4K: 2 and 4 are within the run-to-run spread, 1 is slower
+#endif
+static_assert(RFX_K1_BATCH >= 1 && RFX_K1_BATCH <= 4, "the host step table (ensure_step_table) carries 3 spare rows for the speculative reads");
+template <bool SPARSE>
 RFX_D v2 march_fast(const SsgiArgs& a, v3& dir, v3& hitPos, int noiseB, bool& hit) {
+  constexpr int BATCH = RFX_K1_BATCH;
   dir = dir * (a.ray_distance / (float)a.steps);
   hit = false;
   const float* cs_row = a.step_table + noiseB;  // row i-1 holds cs(i, b); the table carries BATCH spare rows for the speculative reads
@@ -644,7 +553,7 @@ RFX_D v2 march_fast(const SsgiArgs& a, v3& dir, v3& hitPos, int noiseB, bool& hi
 }
 
 // doSample  ssgi.frag:362-439 (SFU arithmetic; `desat` = (1 - roughnessSq) * saturation(diffuse) * 0.4)
-template <bool SPARSE, bool PEER, int BATCH>
+template <bool SPARSE, bool PEER>
 RFX_D v3 sample_fast(const SsgiArgs& a, v3 viewPos, v3 viewNormal, float roughnessSq, float metalness, float desat, bool isDiffuseSample, bool isEnvSample, float NoV,
                      float NoL, float NoH, float LoH, int noiseB, v3 l, v3& hitPos, float& brdf, float& pdf) {
   const float cosTheta = fmaxf(0.0f, dot(viewNormal, l));
@@ -659,7 +568,7 @@ RFX_D v3 sample_fast(const SsgiArgs& a, v3 viewPos, v3 viewNormal, float roughne
   pdf = fmaxf(SSGI_EPSILON, pdf);
   hitPos = viewPos;
   bool hit;
-  const v2 coords = march_fast<SPARSE, BATCH>(a, l, hitPos, noiseB, hit);
+  const v2 coords = march_fast<SPARSE>(a, l, hitPos, noiseB, hit);
   const bool allowMissedRays = (a.flags & RFX_SSGI_MISSED_RAYS) != 0;
   if (!hit && !allowMissedRays) return getEnvColor<true, true>(a, l, roughnessSq, isDiffuseSample, isEnvSample);
   v2 vel = mk2(0.0f, 0.0f);
@@ -691,10 +600,10 @@ RFX_D v3 sample_fast(const SsgiArgs& a, v3 viewPos, v3 viewNormal, float roughne
   return SSGI;
 }
 
-template <int MODE, bool IS, bool SPARSE, bool PEER, int BATCH>
+template <int MODE, bool IS, bool SPARSE, bool PEER>
 __global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_fast_kernel(const __grid_constant__ SsgiArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   const uchar4 bn = __ldg(a.blue.tex + blue_index(a.blue, x, y));
   const v4 random = mk4((float)bn.x / 255.0f, (float)bn.y / 255.0f, (float)bn.z / 255.0f, (float)bn.w / 255.0f);
@@ -796,14 +705,14 @@ __global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_fast_kernel(
   if (MODE == RFX_MODE_SSGI && isDiffuseSample) {  // :222-242
     const v3 dray = emsIsEnvSample ? envMisDir : cosineSampleHemisphere_cs<true>(viewNormal, random.x, sc.x, sc.y);
     calculateAngles<true>(dray, v, n, NoL, NoH, LoH, VoH);
-    v3 gi = sample_fast<SPARSE, PEER, BATCH>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, true, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, dray, hitPos, brdf, pdf);
+    v3 gi = sample_fast<SPARSE, PEER>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, true, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, dray, hitPos, brdf, pdf);
     gi = gi * brdf;
     if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, pdf);
     diffuseGI = gi * inv_ems;
   }
   calculateAngles<true>(l, v, n, NoL, NoH, LoH, VoH);  // the specular ray :246-265
   {
-    v3 gi = sample_fast<SPARSE, PEER, BATCH>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, isDiffuseSample, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf);
+    v3 gi = sample_fast<SPARSE, PEER>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, isDiffuseSample, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf);
     gi = gi * brdf;
     if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, pdf);
     specularGI = gi * inv_ems;
@@ -832,28 +741,22 @@ __global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_fast_kernel(
 
 template <int MODE, bool IS>
 static void launch_ssgi_t(const SsgiArgs& a, dim3 grid, cudaStream_t s) {
-#define RFX_K1_LAUNCH(SP, F, PH) ssgi_kernel<MODE, IS, SP, F, PH><<<grid, kThreads, 0, s>>>(a)
-  if (a.phase == 0 && a.fast && !a.legacy_fast) {
+  if (a.fast && !a.scaled) {  // the fused fast kernel addresses texels by pixel index: a scaled target takes the general kernel
+#define RFX_K1F(SP, PE) ssgi_fast_kernel<MODE, IS, SP, PE><<<grid, kThreads, 0, s>>>(a)
     const bool peer = a.acc_peer.n > 1;
-#define RFX_K1F(SP, PE, BA) ssgi_fast_kernel<MODE, IS, SP, PE, BA><<<grid, kThreads, 0, s>>>(a)
-#define RFX_K1F_B(SP, PE) do { if (a.march_batch >= 4) RFX_K1F(SP, PE, 4); else if (a.march_batch <= 1) RFX_K1F(SP, PE, 1); else RFX_K1F(SP, PE, 2); } while (0)
-    if (a.proj_sparse) { if (peer) RFX_K1F_B(true, true); else RFX_K1F_B(true, false); }
-    else { if (peer) RFX_K1F_B(false, true); else RFX_K1F_B(false, false); }
-#undef RFX_K1F_B
+    if (a.proj_sparse) { if (peer) RFX_K1F(true, true); else RFX_K1F(true, false); }
+    else { if (peer) RFX_K1F(false, true); else RFX_K1F(false, false); }
 #undef RFX_K1F
-  } else if (a.phase == 0) {
-    if (a.proj_sparse) { if (a.fast) RFX_K1_LAUNCH(true, true, 0); else RFX_K1_LAUNCH(true, false, 0); }
-    else { if (a.fast) RFX_K1_LAUNCH(false, true, 0); else RFX_K1_LAUNCH(false, false, 0); }
-  } else if (a.phase == 1) {  // split phases exist for the fast variant only (rfx_api.cu falls back to the fused kernel otherwise)
-    if (a.proj_sparse) RFX_K1_LAUNCH(true, true, 1); else RFX_K1_LAUNCH(false, true, 1);
   } else {
-    if (a.proj_sparse) RFX_K1_LAUNCH(true, true, 2); else RFX_K1_LAUNCH(false, true, 2);
+#define RFX_K1(SP, F) ssgi_kernel<MODE, IS, SP, F><<<grid, kThreads, 0, s>>>(a)
+    if (a.proj_sparse) { if (a.fast) RFX_K1(true, true); else RFX_K1(true, false); }
+    else { if (a.fast) RFX_K1(false, true); else RFX_K1(false, false); }
+#undef RFX_K1
   }
-#undef RFX_K1_LAUNCH
 }
 
 cudaError_t launch_ssgi(const SsgiArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   const bool is = (a.flags & RFX_SSGI_IMPORTANCE_SAMPLING) != 0;
   if (a.mode == RFX_MODE_SSGI) {
     if (is) launch_ssgi_t<RFX_MODE_SSGI, true>(a, grid, s); else launch_ssgi_t<RFX_MODE_SSGI, false>(a, grid, s);

@@ -299,7 +299,7 @@ template <int TC, int ITYPE, bool LOG, bool HLIN, bool FAST>
 #endif
 __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(const __grid_constant__ TemporalArgs a) {
   int x, y;
-  const bool in_rows = seg_pixel(a.segs, x, y);
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
   TState s;
   temporal_state(a, x, y, min(x, a.W - 1), min(y, a.H - 1), s);
@@ -321,7 +321,7 @@ static void launch_temporal_t(const TemporalArgs& a, dim3 grid, cudaStream_t s) 
 }
 
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + kTileW - 1) / kTileW, a.segs.tiles);
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
 #define RFX_LT(TC, IT) do { if (a.fast) launch_temporal_t<TC, IT, true>(a, grid, s); else launch_temporal_t<TC, IT, false>(a, grid, s); } while (0)
   if (a.input_type == RFX_INPUT_DIFFUSE_SPECULAR && a.texture_count == 2) RFX_LT(2, RFX_INPUT_DIFFUSE_SPECULAR);
   else if (a.input_type == RFX_INPUT_DIFFUSE && a.texture_count == 1) RFX_LT(1, RFX_INPUT_DIFFUSE);
@@ -381,10 +381,8 @@ __global__ void __launch_bounds__(kThreads, RFX_TRAA_MIN_BLOCKS) ctraa_kernel(co
   __shared__ uint2 accs[kTraaAccW * kTraaAccH];
   const TemporalArgs& t = a.t;
   const int W = t.W, H = t.H;
-  int k = 0;  // the segment of this block's tile row, laid out as seg_pixel does
-  while (k + 1 < t.segs.n && (int)blockIdx.y >= t.segs.tile0[k + 1]) k++;
-  const int x0 = blockIdx.x * kTraaTileW, y0 = (t.segs.r0[k] & ~1) + ((int)blockIdx.y - t.segs.tile0[k]) * kTileH;
-  const int r0 = t.segs.r0[k], r1 = t.segs.r1[k];
+  const int x0 = blockIdx.x * kTraaTileW, y0 = (t.row0 & ~1) + (int)blockIdx.y * kTileH;  // tile rows laid out as range_pixel does
+  const int r0 = t.row0, r1 = t.row1;
   for (int i = threadIdx.x; i < kTraaK5W * kTraaK5H; i += kThreads)  // slots outside the image hold a clamped duplicate, never read
     k5s[i] = pack_h4(ssgi_compose_px(a.k5, clampi(x0 - kTraaK5Halo + i % kTraaK5W, W), clampi(y0 - kTraaK5Halo + i / kTraaK5W, H)));
   __syncthreads();
@@ -410,7 +408,7 @@ cudaError_t launch_ctraa(const CTraaArgs& a, cudaStream_t s) {
   const TemporalArgs& t = a.t;
   if (t.texture_count != 1 || t.input_type != RFX_INPUT_DIFFUSE || !t.input_half || !t.out_half || !t.history_linear || t.hist_f32 || t.in_scaled)
     return cudaErrorNotSupported;
-  dim3 grid((t.W + kTraaTileW - 1) / kTraaTileW, t.segs.tiles);
+  dim3 grid((t.W + kTraaTileW - 1) / kTraaTileW, row_tiles(t.row0, t.row1));
   if (t.fast) {
     if (t.log_transform) ctraa_kernel<true, true><<<grid, kThreads, 0, s>>>(a);
     else ctraa_kernel<false, true><<<grid, kThreads, 0, s>>>(a);

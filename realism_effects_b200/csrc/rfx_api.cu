@@ -39,25 +39,12 @@ struct rfx_ctx {
   void* nrd = nullptr;
   int nrd_w = 0, nrd_h = 0;
   size_t nrd_pitch = 0;
-  bool nrd_reuse = false;  // set by the native chain: the scratch already holds this frame's decode
   // scratch: view-space z plane for the SSGI march
   void* viewz = nullptr;
   int viewz_w = 0, viewz_h = 0;
   size_t viewz_pitch = 0;
-  bool viewz_reuse = false;  // set by the native chain for the 2nd.. row block of a frame
-  int k1_phase = 0;          // set by the native chain: 0 fused K1, 1 ray march only, 2 shading from the march records
-  void* k1rec = nullptr;     // march records, 2 x float4 per pixel
-  size_t k1rec_pitch = 0;
-  int k1rec_w = 0, k1rec_h = 0;
-  const RowSegs* segs_override = nullptr;  // set by the native chain: all owned row blocks in ONE launch
-  // defaults measured on H100 at 4K with tools/sweep_k1.sh
+  // default measured on H100 at 4K with tools/sweep_k1.sh
   int k3_tma = 1;     // RFX_K3_TMA=0 disables the TMA-staged tap tiles of the Poisson passes >= 1 (same bytes out; ~6 % slower per pass)
-  int k1_batch = 4;   // RFX_K1_BATCH: march steps fetched together (1, 2, 4; 2 and 4 are within the run-to-run spread, 1 is slower)
-  int compose_mode = 0;  // RFX_COMPOSE_MODE: arithmetic of the fused K4: 0 IEEE (default: 1.8e-4 of the first 4K frame's pixels outside 1e-3), 1 SFU, 2 SFU + Newton (both 4.2e-4)
-  int debug_no_a_carry = 0;  // RFX_DEBUG_NO_A_CARRY=1: groups leave discarded texels of the A target as they are (the pre-fix behaviour; shows what tests/test_gpu_chain.py's in-process group test catches)
-  int k1_vz_tiled = 0;  // RFX_K1_VZ_TILED=1: 8x4-tiled viewZ scratch for the fast K1 (experiment)
-  int legacy_k1 = 0;  // RFX_LEGACY_K1=1 in the environment: the round-1 fast K1 kernel (A/B timing)
-  const PeerPV* peer_accumulated = nullptr;  // set by the native chain in a row-sharded group: K1's `accumulated` rows live on their owners
 };
 
 static rfx_status fail(rfx_ctx* c, rfx_status st, const char* fmt, ...) {
@@ -91,12 +78,7 @@ rfx_status rfx_ctx_create(int device, rfx_ctx** out) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || device < 0 || device >= n) return RFX_ERR_CUDA;
   rfx_ctx* ctx = new rfx_ctx();
   ctx->device = device;
-  if (const char* e = getenv("RFX_LEGACY_K1")) ctx->legacy_k1 = atoi(e);
   if (const char* e = getenv("RFX_K3_TMA")) ctx->k3_tma = atoi(e);
-  if (const char* e = getenv("RFX_K1_BATCH")) ctx->k1_batch = atoi(e);
-  if (const char* e = getenv("RFX_K1_VZ_TILED")) ctx->k1_vz_tiled = atoi(e);
-  if (const char* e = getenv("RFX_DEBUG_NO_A_CARRY")) ctx->debug_no_a_carry = atoi(e);
-  if (const char* e = getenv("RFX_COMPOSE_MODE")) ctx->compose_mode = atoi(e);
   if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) {
     delete ctx;
     return RFX_ERR_CUDA;
@@ -136,7 +118,6 @@ void rfx_ctx_destroy(rfx_ctx* ctx) {
   cudaFree(ctx->step_table);
   cudaFree(ctx->nrd);
   cudaFree(ctx->viewz);
-  cudaFree(ctx->k1rec);
   cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
@@ -373,11 +354,6 @@ static void rows(uint32_t row0, uint32_t row1, uint32_t H, int& r0, int& r1) {
   if (row0 == 0 && row1 == 0) { r0 = 0; r1 = (int)H; }
   else { r0 = (int)row0; r1 = (int)(row1 > H ? H : row1); }
 }
-// the row segments of a launch: [r0,r1) of the call, or the multi-block table the native chain installed for this launch
-static void set_segs(rfx_ctx* ctx, int r0, int r1, RowSegs& s) {
-  if (ctx->segs_override) s = *ctx->segs_override;
-  else s = make_segs(&r0, &r1, 1);
-}
 // mat4 * mat4 with the oracle's lowering: s = ((a0*b0 + a1*b1) + a2*b2) + a3*b3, no contraction
 static void matmul(const float* A, const float* B, float* R) {
   for (int c = 0; c < 4; c++)
@@ -438,10 +414,13 @@ static void temporal_uniforms(const rfx_ctx* ctx, const rfx_temporal_params* p, 
 
 extern "C" {
 
-rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_params* p, const rfx_plane* depth, const rfx_plane* gbuffer,
-                                 const rfx_plane* velocity, const rfx_plane* direct_light, const rfx_plane* accumulated, const rfx_plane* out,
-                                 uint32_t row0, uint32_t row1) {
-  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ssgi_trace: null argument");
+// The four per-pass entry points the native chain drives are split in two: the extern "C" wrapper checks its pointers and resolves
+// the row arguments (row0 == row1 == 0: every row); the static implementation validates the planes and launches over output rows
+// [r0, r1), with what only the chain knows passed explicitly.
+
+// K1.  acc_peer: K1's `accumulated` in a row-sharded group, whose rows live on their owners (nullptr: the local plane)
+static rfx_status ssgi_trace(rfx_ctx* ctx, void* stream, const rfx_ssgi_params* p, const rfx_plane* depth, const rfx_plane* gbuffer, const rfx_plane* velocity,
+                             const rfx_plane* direct_light, const rfx_plane* accumulated, const rfx_plane* out, int r0, int r1, const PeerPV* acc_peer) {
   SsgiArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gbuffer, RFX_FMT_RGBA32F, a.gb) || !ov(out, RFX_FMT_RGBA32F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "ssgi_trace: depth must be R32F, gbuffer/out RGBA32F");
@@ -456,8 +435,7 @@ rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_para
   if (a.W > TW || a.H > TH) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ssgi_trace: the output may be smaller than the input planes (resolutionScale <= 1), not larger");
   a.scaled = a.W != TW || a.H != TH;
   if (p->steps < 1 || p->refine_steps < 0 || (p->mode != RFX_MODE_SSGI && p->mode != RFX_MODE_SSR)) return fail(ctx, RFX_ERR_INVALID_ARG, "ssgi_trace: bad steps/mode");
-  rows(row0, row1, out->height, a.row0, a.row1);
-  set_segs(ctx, a.row0, a.row1, a.segs);
+  a.row0 = r0; a.row1 = r1;
   cam_to_dev(p->cam, a.cam);
   a.ray_distance = p->ray_distance; a.thickness = p->thickness; a.env_blur = p->env_blur; a.max_env_mip = p->max_env_map_mip_level;
   a.near_minus_far = p->cam.near_plane - p->cam.far_plane;  // SSGIPass.js:85-87
@@ -488,7 +466,7 @@ rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_para
     cudaFree(ctx->viewz);
     ctx->viewz = nullptr;
     ctx->viewz_pitch = ((size_t)TW * 4 + 255) & ~(size_t)255;
-    CU(cudaMalloc(&ctx->viewz, std::max(ctx->viewz_pitch * TH, (size_t)((TW + 7) / 8) * ((TH + 3) / 4) * 128)));  // row-major or 8x4 tiles
+    CU(cudaMalloc(&ctx->viewz, ctx->viewz_pitch * TH));
     ctx->viewz_w = TW; ctx->viewz_h = TH;
   }
   {  // fast fused kernel: projection rows in texel units (0.5 W P00, 0.5 W P20, 0.5 H P11, 0.5 H P21), word pitch of the viewZ plane
@@ -496,39 +474,25 @@ rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_para
     const float hw = 0.5f * (float)a.W, hh = 0.5f * (float)a.H;
     a.ps_x0 = hw * M[0]; a.ps_x2 = hw * M[8]; a.ps_y1 = hh * M[5]; a.ps_y2 = hh * M[9]; a.ps_hw = hw; a.ps_hh = hh;
     a.vz_pitchw = (int)(ctx->viewz_pitch / 4);
-    a.legacy_fast = ctx->legacy_k1 || a.scaled;  // the fused fast kernel addresses texels by pixel index: a scaled target takes the general kernel
-    a.march_batch = ctx->k1_batch;
-    a.vz_tiles_x = (TW + 7) / 8;
-    a.vz_tiled = ctx->k1_vz_tiled && a.fast && !a.legacy_fast && ctx->k1_phase == 0;  // only the fused fast kernel reads the tiled layout
-    if (ctx->peer_accumulated) a.acc_peer = *ctx->peer_accumulated;
+    if (acc_peer) a.acc_peer = *acc_peer;
   }
-  a.phase = a.scaled ? 0 : ctx->k1_phase;
-  if (a.phase != 0 && !a.fast) {  // the split phases exist for the fast variant: otherwise phase 1 is empty and phase 2 is the fused kernel
-    if (a.phase == 1) return RFX_OK;
-    a.phase = 0;
-  }
-  if (a.phase != 0) {
-    if (!ctx->k1rec || ctx->k1rec_w != a.W || ctx->k1rec_h != a.H) {
-      CU(cudaStreamSynchronize(ctx->stream));
-      cudaFree(ctx->k1rec);
-      ctx->k1rec = nullptr;
-      ctx->k1rec_pitch = (size_t)a.W * 32;
-      CU(cudaMalloc(&ctx->k1rec, ctx->k1rec_pitch * a.H));
-      ctx->k1rec_w = a.W; ctx->k1rec_h = a.H;
-    }
-    a.rec = (unsigned char*)ctx->k1rec;
-    a.rec_pitch = (long long)ctx->k1rec_pitch;
-  }
-  if (!ctx->viewz_reuse && a.phase != 2) LAUNCHED(launch_viewz(a, OutV{(unsigned char*)ctx->viewz, (long long)ctx->viewz_pitch}, pick(ctx, stream)));
+  LAUNCHED(launch_viewz(a, OutV{(unsigned char*)ctx->viewz, (long long)ctx->viewz_pitch}, pick(ctx, stream)));
   a.viewz = PV{(const unsigned char*)ctx->viewz, TW, TH, (long long)ctx->viewz_pitch};
   LAUNCHED(launch_ssgi(a, pick(ctx, stream)));
   return RFX_OK;
 }
+rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_params* p, const rfx_plane* depth, const rfx_plane* gbuffer,
+                                 const rfx_plane* velocity, const rfx_plane* direct_light, const rfx_plane* accumulated, const rfx_plane* out,
+                                 uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ssgi_trace: null argument");
+  int r0, r1;
+  rows(row0, row1, out->height, r0, r1);
+  return ssgi_trace(ctx, stream, p, depth, gbuffer, velocity, direct_light, accumulated, out, r0, r1, nullptr);
+}
 
-rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_temporal_params* p, const rfx_plane* input, const rfx_plane* velocity,
-                                         const rfx_plane* history0, const rfx_plane* history1, const rfx_plane* out0, const rfx_plane* out1,
-                                         uint32_t row0, uint32_t row1) {
-  if (!ctx || !p || !input || !out0) return fail(ctx, RFX_ERR_INVALID_ARG, "temporal: null argument");
+// K2
+static rfx_status temporal_reproject(rfx_ctx* ctx, void* stream, const rfx_temporal_params* p, const rfx_plane* input, const rfx_plane* velocity,
+                                     const rfx_plane* history0, const rfx_plane* history1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1) {
   TemporalArgs a{};
   if (p->texture_count != 1 && p->texture_count != 2) return fail(ctx, RFX_ERR_INVALID_ARG, "temporal: texture_count must be 1 or 2");
   a.input_half = input->format == RFX_FMT_RGBA16F;
@@ -548,17 +512,23 @@ rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_t
     return fail(ctx, RFX_ERR_SIZE_MISMATCH, "temporal: plane sizes differ (only the input may be smaller: resolutionScale < 1)");
   a.in_scaled = a.input.w != a.W || a.input.h != a.H;
   if (a.in_scaled && a.input_half) return fail(ctx, RFX_ERR_UNSUPPORTED, "temporal: a scaled input is the RGBA32F SSGI target");
-  rows(row0, row1, out0->height, a.row0, a.row1);
-  set_segs(ctx, a.row0, a.row1, a.segs);
+  a.row0 = r0; a.row1 = r1;
   temporal_uniforms(ctx, p, a);
   LAUNCHED(launch_temporal(a, pick(ctx, stream)));
   return RFX_OK;
 }
+rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_temporal_params* p, const rfx_plane* input, const rfx_plane* velocity,
+                                         const rfx_plane* history0, const rfx_plane* history1, const rfx_plane* out0, const rfx_plane* out1,
+                                         uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !input || !out0) return fail(ctx, RFX_ERR_INVALID_ARG, "temporal: null argument");
+  int r0, r1;
+  rows(row0, row1, out0->height, r0, r1);
+  return temporal_reproject(ctx, stream, p, input, velocity, history0, history1, out0, out1, r0, r1);
+}
 
-rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p, const rfx_plane* depth, const rfx_plane* gb,
-                                      const rfx_plane* in0, const rfx_plane* in1, const rfx_plane* out0, const rfx_plane* out1, uint32_t row0,
-                                      uint32_t row1) {
-  if (!ctx || !p || !in0 || !out0) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: null argument");
+// K3.  decoded: the context's G-buffer scratch already holds this frame's decode (the chain decodes once per frame)
+static rfx_status poisson_denoise(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p, const rfx_plane* depth, const rfx_plane* gb, const rfx_plane* in0,
+                                  const rfx_plane* in1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1, bool decoded) {
   if (p->texture_count != 1 && p->texture_count != 2) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: texture_count must be 1 or 2");
   PoissonArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gb, RFX_FMT_RGBA32F, a.gb)) return fail(ctx, RFX_ERR_BAD_FORMAT, "poisson: depth R32F + gbuffer/normal RGBA32F required");
@@ -577,8 +547,7 @@ rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_pois
   // LINEAR inputs are sampled by uv and may have any size (the AO denoiser's first pass reads a reduced-resolution AO target)
   if (!p->input_linear && (a.in0.w != a.W || a.in0.h != a.H)) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "poisson: NEAREST inputs must have the output's size");
   if (out0->ptr == in0->ptr || (out1 && in1 && out1->ptr == in1->ptr)) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: in-place filtering is not allowed");
-  rows(row0, row1, out0->height, a.row0, a.row1);
-  set_segs(ctx, a.row0, a.row1, a.segs);
+  a.row0 = r0; a.row1 = r1;
   a.radius = p->radius; a.phi = p->phi; a.luma_phi = p->luma_phi; a.depth_phi = p->depth_phi; a.normal_phi = p->normal_phi;
   a.roughness_phi = p->roughness_phi; a.specular_phi = p->specular_phi;
   a.texture_count = p->texture_count; a.spec0 = p->is_texture_specular[0]; a.spec1 = p->is_texture_specular[1];
@@ -600,10 +569,10 @@ rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_pois
     ctx->nrd_pitch = ((size_t)a.W * 16 + 255) & ~(size_t)255;
     CU(cudaMalloc(&ctx->nrd, ctx->nrd_pitch * a.H));
     ctx->nrd_w = a.W; ctx->nrd_h = a.H;
-    ctx->nrd_reuse = false;
+    decoded = false;
   }
-  if (!ctx->nrd_reuse)  // (the chain's first pass of a frame has the widest rows of all its passes, so its decode serves the later ones)
-    LAUNCHED(launch_gbuffer_decode(a.gb, OutV{(unsigned char*)ctx->nrd, (long long)ctx->nrd_pitch}, a.W, a.H, p->gbuffer_texture ? 1 : 0, a.segs,
+  if (!decoded)  // (the chain's first pass of a frame has the widest rows of all its passes, so its decode serves the later ones)
+    LAUNCHED(launch_gbuffer_decode(a.gb, OutV{(unsigned char*)ctx->nrd, (long long)ctx->nrd_pitch}, a.W, a.H, p->gbuffer_texture ? 1 : 0, a.row0, a.row1,
                                    (int)std::ceil(p->radius * std::max(1.0f, (float)a.H / (float)a.W)) + 1, pick(ctx, stream)));
   a.nrd = PV{(const unsigned char*)ctx->nrd, a.W, a.H, (long long)ctx->nrd_pitch};
   {
@@ -615,10 +584,18 @@ rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_pois
   LAUNCHED(launch_poisson_fast(a, pick(ctx, stream)));
   return RFX_OK;
 }
+rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p, const rfx_plane* depth, const rfx_plane* gb,
+                                      const rfx_plane* in0, const rfx_plane* in1, const rfx_plane* out0, const rfx_plane* out1, uint32_t row0,
+                                      uint32_t row1) {
+  if (!ctx || !p || !in0 || !out0) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: null argument");
+  int r0, r1;
+  rows(row0, row1, out0->height, r0, r1);
+  return poisson_denoise(ctx, stream, p, depth, gb, in0, in1, out0, out1, r0, r1, false);
+}
 
-rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_params* p, const rfx_plane* depth, const rfx_plane* gb,
-                                 const rfx_plane* dgi, const rfx_plane* sgi, const rfx_plane* scene, const rfx_plane* out, uint32_t row0, uint32_t row1) {
-  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "gi_compose: null argument");
+// K4
+static rfx_status gi_compose(rfx_ctx* ctx, void* stream, const rfx_compose_params* p, const rfx_plane* depth, const rfx_plane* gb, const rfx_plane* dgi,
+                             const rfx_plane* sgi, const rfx_plane* scene, const rfx_plane* out, int r0, int r1) {
   ComposeArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gb, RFX_FMT_RGBA32F, a.gb) || !ov(out, RFX_FMT_RGBA32F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "gi_compose: depth R32F, gbuffer RGBA32F, out RGBA32F required");
@@ -636,13 +613,19 @@ rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_p
   if (a.depth.w != a.W || a.depth.h != a.H || a.gb.w != a.W || a.gb.h != a.H || (a.diffuse.p && (a.diffuse.w != a.W || a.diffuse.h != a.H)) ||
       (a.specular.p && (a.specular.w != a.W || a.specular.h != a.H)) || (a.scene.p && (a.scene.w != a.W || a.scene.h != a.H)))
     return fail(ctx, RFX_ERR_SIZE_MISMATCH, "gi_compose: plane sizes differ");
-  rows(row0, row1, out->height, a.row0, a.row1);
-  set_segs(ctx, a.row0, a.row1, a.segs);
+  a.row0 = r0; a.row1 = r1;
   cam_to_dev(p->cam, a.cam);
   a.input_type = p->input_type;
   a.fast = ctx->fast_math;
   LAUNCHED(launch_gi_compose(a, pick(ctx, stream)));
   return RFX_OK;
+}
+rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_params* p, const rfx_plane* depth, const rfx_plane* gb,
+                                 const rfx_plane* dgi, const rfx_plane* sgi, const rfx_plane* scene, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "gi_compose: null argument");
+  int r0, r1;
+  rows(row0, row1, out->height, r0, r1);
+  return gi_compose(ctx, stream, p, depth, gb, dgi, sgi, scene, out, r0, r1);
 }
 
 rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_compose_params* p, const rfx_plane* depth, const rfx_plane* gi, const rfx_plane* scene,
@@ -1056,19 +1039,9 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* o
   return RFX_OK;
 }
 
-// installs the row-segment table of launch k (all owned blocks) for the duration of one launch call
-struct SegScope {
-  rfx_ctx* ctx;
-  RowSegs segs;
-  SegScope(rfx_ctx* c, const uint32_t* ranges, uint32_t n_blocks, uint32_t n_launches, uint32_t k) : ctx(c) {
-    if (!ranges || n_blocks <= 1) return;
-    int r0[RFX_MAX_SEGS], r1[RFX_MAX_SEGS];
-    for (uint32_t b = 0; b < n_blocks; b++) { r0[b] = (int)ranges[(b * n_launches + k) * 2]; r1[b] = (int)ranges[(b * n_launches + k) * 2 + 1]; }
-    segs = make_segs(r0, r1, (int)n_blocks);
-    ctx->segs_override = &segs;
-  }
-  ~SegScope() { ctx->segs_override = nullptr; }
-};
+// Output rows [r0, r1) of chain launch k: ranges[2k], ranges[2k+1] in a row-sharded frame (rfx_shard_ranges), else all H rows
+struct Rows { int r0, r1; };
+static Rows launch_rows(const uint32_t* ranges, uint32_t k, int H) { return ranges ? Rows{(int)ranges[2 * k], (int)ranges[2 * k + 1]} : Rows{0, H}; }
 
 // ------------------------------------------------------------------------------------------
 // fast chain (k_chain.cu): same frame logic as chain_render_impl below, interleaved internal planes, compose fused into the
@@ -1078,12 +1051,6 @@ struct SegScope {
 static PV ipv(const IPlane& p, int w, int h) { return PV{(const unsigned char*)p.p, w, h, (long long)p.pitch}; }
 static OutV iov(const IPlane& p) { return OutV{(unsigned char*)p.p, (long long)p.pitch}; }
 static PV rpv(const rfx_plane& p) { return PV{(const unsigned char*)p.ptr, (int)p.width, (int)p.height, (long long)p.pitch}; }
-static RowSegs segs_for(const uint32_t* ranges, uint32_t n_blocks, uint32_t n_launches, uint32_t k, int H) {
-  int r0[RFX_MAX_SEGS], r1[RFX_MAX_SEGS];
-  if (!ranges) { r0[0] = 0; r1[0] = H; return make_segs(r0, r1, 1); }
-  for (uint32_t b = 0; b < n_blocks; b++) { r0[b] = (int)ranges[(b * n_launches + k) * 2]; r1[b] = (int)ranges[(b * n_launches + k) * 2 + 1]; }
-  return make_segs(r0, r1, (int)n_blocks);
-}
 static void peer_single(PeerPV& pp, PV local) {
   pp = PeerPV{};
   pp.local = local;
@@ -1104,10 +1071,10 @@ static void keep_traa_camera(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
 // rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
 // K2 on them +- 1).
-static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane* composed, const uint32_t* ranges,
-                                    uint32_t n_blocks, uint32_t n_launches, uint32_t k) {
+static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane* composed, const uint32_t* ranges, uint32_t k) {
   rfx_ctx* ctx = ch->ctx;
   const int W = (int)ch->opt.width, H = (int)ch->opt.height;
+  const Rows kr = launch_rows(ranges, k, H);
   const int cur = (int)(ch->traa_frames & 1), prev = cur ^ 1;
   rfx_temporal_params tp = ch->traa_tp;  // TRAAEffect's forced options over the TemporalReprojectPass defaults (TRAAEffect.js:21-31)
   tp.max_blend = ch->traa.max_blend; tp.neighborhood_clamp_intensity = ch->traa.neighborhood_clamp_intensity;
@@ -1120,8 +1087,7 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     CTraaArgs a{};
     TemporalArgs& t = a.t;
     if (!pv(f->velocity, RFX_FMT_RGBA32F, t.velocity)) return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: velocity must be RGBA32F");
-    t.W = W; t.H = H;
-    t.segs = segs_for(ranges, n_blocks, n_launches, k, H);
+    t.W = W; t.H = H; t.row0 = kr.r0; t.row1 = kr.r1;
     temporal_uniforms(ctx, &tp, t);
     t.input_half = 1; t.out_half = 1;
     SsgiComposeArgs& c = a.k5;
@@ -1139,16 +1105,13 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
   } else {
     const int halo = RFX_TRAA_TAIL_ROWS;
-    for (uint32_t b = 0; b < (ranges ? n_blocks : 1u); b++) {
-      const int r0 = ranges ? (int)ranges[(b * n_launches + k) * 2] : 0, r1 = ranges ? (int)ranges[(b * n_launches + k) * 2 + 1] : H;
-      rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
-                                              (uint32_t)std::max(0, r0 - halo), (uint32_t)std::min(H, r1 + halo));
-      if (st == RFX_OK)
-        st = rfx_temporal_reproject_launch(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
-                                           (uint32_t)std::max(0, r0 - 1), (uint32_t)std::min(H, r1 + 1));
-      if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc[cur], &ch->traa_out, (uint32_t)r0, (uint32_t)r1);
-      if (st != RFX_OK) return st;
-    }
+    rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
+                                            (uint32_t)std::max(0, kr.r0 - halo), (uint32_t)std::min(H, kr.r1 + halo));
+    if (st == RFX_OK)
+      st = rfx_temporal_reproject_launch(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
+                                         (uint32_t)std::max(0, kr.r0 - 1), (uint32_t)std::min(H, kr.r1 + 1));
+    if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc[cur], &ch->traa_out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    if (st != RFX_OK) return st;
   }
   ch->traa_keep = 1.0f;
   ch->traa_frames++;
@@ -1175,13 +1138,10 @@ static bool encode_texel_map(CUtensorMap* map, const void* base, int W, int H, s
             CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_blocks,
-                                    uint32_t k_begin, uint32_t k_end, int k1_phase) {
+static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t k_begin, uint32_t k_end) {
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
   const int W = (int)o.width, H = (int)o.height;
-  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations + (ch->traa_on ? 1u : 0u);
-  if (!ranges) n_blocks = 1;
   auto on = [&](uint32_t k) { return k >= k_begin && k < k_end; };
   const cudaStream_t cs = stream ? (cudaStream_t)stream : ctx->stream;
   const int cur = (int)(ch->frame_idx & 1), prev = cur ^ 1;
@@ -1201,17 +1161,13 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     sp.ray_distance = o.distance; sp.thickness = o.thickness; sp.env_blur = o.env_blur;
     sp.max_env_map_mip_level = ctx->env_set ? (float)((int)std::floor(std::log2((double)std::max(ctx->env.size_x, ctx->env.size_y))) + 1) : 0.0f;
     sp.steps = o.steps; sp.refine_steps = o.refine_steps; sp.mode = o.mode; sp.flags = o.ssgi_flags;
-    sp.blue_noise_index = k1_phase == 2 ? ch->bn_trace : next_blue(o.blue_noise_start, ch->bn_trace);
-    SegScope seg_scope(ctx, ranges, n_blocks, n_launches, k);
-    ctx->k1_phase = k1_phase;
-    ctx->peer_accumulated = ch->group ? &ch->peer_composed[prev] : nullptr;
+    sp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_trace);
+    const Rows kr = launch_rows(ranges, k, H);
     {
       SpanGuard g(ch, cs, 0);
-      st = rfx_ssgi_trace_launch(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, &ch->composed2[prev], &ch->ssgi_out, ranges ? ranges[k * 2] : 0u,
-                                 ranges ? ranges[k * 2 + 1] : 0u);
+      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, &ch->composed2[prev], &ch->ssgi_out, kr.r0, kr.r1,
+                      ch->group ? &ch->peer_composed[prev] : nullptr);
     }
-    ctx->k1_phase = 0;
-    ctx->peer_accumulated = nullptr;
     if (st != RFX_OK) return st;
   }
   k++;
@@ -1222,7 +1178,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     if (ch->group) a.hist = ch->peer_dn[prev]; else peer_single(a.hist, ipv(ch->dnB16[prev], W, H));
     a.out = iov(ch->tr32);
     a.W = W; a.H = H;
-    a.segs = segs_for(ranges, n_blocks, n_launches, k, H);
+    const Rows kr = launch_rows(ranges, k, H);
+    a.row0 = kr.r0; a.row1 = kr.r1;
     a.cam = cam;
     if (!ch->have_prev) {
       memcpy(ch->prev_view, f->cam.view_matrix, 64); memcpy(ch->prev_world, f->cam.camera_matrix_world, 64);
@@ -1251,10 +1208,10 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
   const int n_pass = 2 * o.denoise_iterations;
   const int halo = (int)std::ceil(o.radius * std::max(1.0f, (float)H / (float)W)) + 1;  // rows a Poisson tap can reach (the offset is rotated AFTER the division by the resolution)
   bool decoded = false;
-  auto decode = [&](const RowSegs& segs) -> rfx_status {
+  auto decode = [&](int row0, int row1) -> rfx_status {
     if (decoded) return RFX_OK;
     CDecodeArgs d{gb, depth, iov(ch->nrdz), W, H};
-    LAUNCHED(launch_cdecode(d, segs, halo, cs));
+    LAUNCHED(launch_cdecode(d, row0, row1, halo, cs));
     decoded = true;
     return RFX_OK;
   };
@@ -1263,19 +1220,20 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     if (!on(k)) continue;
     const bool horizontal = (i % 2) == 0, last = i == n_pass - 1;
     CPoissonArgs a{};
-    a.segs = segs_for(ranges, n_blocks, n_launches, k, H);
-    if ((st = decode(a.segs)) != RFX_OK) return st;  // the first pass of a frame has the widest rows of all its passes
+    const Rows kr = launch_rows(ranges, k, H);
+    a.row0 = kr.r0; a.row1 = kr.r1;
+    if ((st = decode(a.row0, a.row1)) != RFX_OK) return st;  // the first pass of a frame has the widest rows of all its passes
     a.nrdz = ipv(ch->nrdz, W, H);
     a.first = i == 0;
     // Target A (even passes).  A `discard`ed pixel keeps its texel = last frame's LAST even pass there (A2), and the LINEAR taps of the next
     // pass read such texels at silhouettes.  One GPU: A is single-buffered and a discard is simply no write.  In a row-sharded group a
     // rank's A rows outside its band hold the result of whichever even pass last covered them (the ranges shrink pass by pass), not the
     // last one's, so A is double-buffered by frame parity like B and the discarded texel is carried from the rank that OWNS the row.
-    const int acur = (ch->group && !ctx->debug_no_a_carry) ? cur : 0;  // RFX_DEBUG_NO_A_CARRY: the pre-fix behaviour (single-buffered A, discard = no write)
+    const int acur = ch->group ? cur : 0;
     a.in = i == 0 ? ipv(ch->tr32, W, H) : ipv(horizontal ? ch->dnB16[cur] : ch->dnA16[acur], W, H);
     a.out = iov(horizontal ? ch->dnA16[acur] : ch->dnB16[cur]);
     if (!horizontal) { if (ch->group) a.carry = ch->peer_dn[prev]; else peer_single(a.carry, ipv(ch->dnB16[prev], W, H)); }
-    else if (ch->group && !ctx->debug_no_a_carry) a.carry = ch->peer_dnA[prev];
+    else if (ch->group) a.carry = ch->peer_dnA[prev];
     a.W = W; a.H = H;
     a.radius = o.radius; a.phi = o.phi; a.luma_phi = o.luma_phi; a.depth_phi = o.depth_phi; a.normal_phi = o.normal_phi;
     a.roughness_phi = o.roughness_phi; a.specular_phi = o.specular_phi;
@@ -1291,8 +1249,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     }
     if (last && on(k_compose)) {
       a.compose = 1;
-      a.compose_mode = ctx->compose_mode;
-      a.csegs = segs_for(ranges, n_blocks, n_launches, k_compose, H);
+      const Rows cr = launch_rows(ranges, k_compose, H);
+      a.crow0 = cr.r0; a.crow1 = cr.r1;
       a.gb = gb;
       a.composed = OutV{(unsigned char*)ch->composed2[cur].ptr, (long long)ch->composed2[cur].pitch};
       if (ch->group) a.composed_carry = ch->peer_composed[prev]; else peer_single(a.composed_carry, rpv(ch->composed2[prev]));
@@ -1315,44 +1273,39 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
   k = k_compose;
   if (on(k) && (n_pass == 0 || !on(k - 1))) {
     CComposeArgs a{};
-    a.segs = segs_for(ranges, n_blocks, n_launches, k, H);
-    if ((st = decode(a.segs)) != RFX_OK) return st;
+    const Rows kr = launch_rows(ranges, k, H);
+    a.row0 = kr.r0; a.row1 = kr.r1;
+    if ((st = decode(a.row0, a.row1)) != RFX_OK) return st;
     a.nrdz = ipv(ch->nrdz, W, H); a.gb = gb; a.dn = ipv(ch->dnB16[cur], W, H);
     a.composed = OutV{(unsigned char*)ch->composed2[cur].ptr, (long long)ch->composed2[cur].pitch};
     if (ch->group) a.composed_carry = ch->peer_composed[prev]; else peer_single(a.composed_carry, rpv(ch->composed2[prev]));
     a.W = W; a.H = H; a.cam = cam;
-    a.compose_mode = ctx->compose_mode;
     SpanGuard g(ch, cs, 4);
     LAUNCHED(launch_ccompose(a, cs));
   }
   // ---- TRAA tail (reads this frame's `composed`, so it runs before the planes change parity)
-  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed2[cur], ranges, n_blocks, n_launches, k_compose + 1)) != RFX_OK) return st;
+  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed2[cur], ranges, k_compose + 1)) != RFX_OK) return st;
   if (on(ch->traa_on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
   return RFX_OK;
 }
 
-// One frame of the chain.  `ranges` == nullptr: whole planes, one block.  Otherwise ranges[(blk*n_launches + k)*2 + {0,1}] =
-// output rows [a,b) of launch k (chain order: K1, K2, K3 pass 0..2*iterations-1, K4) for row block `blk` of this rank
-// (row-block sharding with locally recomputed halos, realism_effects_b200/parallel.py).  Only launches k in
-// [k_begin, k_end) are issued, so a frame can be split into phases (K1 | the rest) between which the caller waits for a
-// different all-gather; per-frame state advances with the launch that consumes it.
-static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_blocks,
-                                    uint32_t k_begin, uint32_t k_end, int k1_phase = 0) {
+// One frame of the chain.  `ranges` == nullptr: whole planes.  Otherwise ranges[2k], ranges[2k+1] = output rows [a,b) of launch k
+// (chain order: K1, K2, K3 pass 0..2*iterations-1, K4, the TRAA tail) of this rank's band, widened by the halos the next launches
+// recompute locally (rfx_shard_ranges).  Only launches k in [k_begin, k_end) are issued, so a caller can wait between two
+// launches of a frame (rfx_ssgi_chain_submit_host waits before K4); per-frame state advances with the launch that consumes it.
+static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t k_begin, uint32_t k_end) {
   if (ch->traa_on && !f->direct_light) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail composes over the direct light plane (the composer input buffer): it may not be NULL");
-  if (ch->fastpath) return chain_render_fast(ch, stream, f, ranges, n_blocks, k_begin, k_end, k1_phase);
+  if (ch->fastpath) return chain_render_fast(ch, stream, f, ranges, k_begin, k_end);
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
   rfx_status st = RFX_OK;
   const bool dm_full = o.denoise_mode == RFX_DENOISE_FULL;
   if (!dm_full && ranges) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for denoise_mode full only");
   if (ranges && ch->ssgi_out.height != o.height) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for resolution_scale 1 only");
-  // K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too), then the TRAA tail when it is on
-  const uint32_t n_launches = 3u + 2u * (uint32_t)o.denoise_iterations + (ch->traa_on ? 1u : 0u);
-  if (!ranges) n_blocks = 1;
+  // launches: K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too), then the TRAA tail when it is on
+  const int H = (int)o.height;
   // what SSGIPass samples as accumulatedTexture = denoiser.texture (Denoiser.js:67-78): the compose target, or the temporal pass's first texture
   rfx_plane* accumulated = o.denoise_mode == RFX_DENOISE_TEMPORAL ? &ch->tr[0] : &ch->composed;
-  auto R0 = [&](uint32_t blk, uint32_t k) -> uint32_t { return ranges ? ranges[(blk * n_launches + k) * 2] : 0u; };
-  auto R1 = [&](uint32_t blk, uint32_t k) -> uint32_t { return ranges ? ranges[(blk * n_launches + k) * 2 + 1] : 0u; };
   auto on = [&](uint32_t k) { return k >= k_begin && k < k_end; };
   const cudaStream_t cs = stream ? (cudaStream_t)stream : ctx->stream;
   uint32_t k = 0;
@@ -1363,17 +1316,12 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     sp.ray_distance = o.distance; sp.thickness = o.thickness; sp.env_blur = o.env_blur;
     sp.max_env_map_mip_level = ctx->env_set ? (float)((int)std::floor(std::log2((double)std::max(ctx->env.size_x, ctx->env.size_y))) + 1) : 0.0f;  // Utils.js:30-34
     sp.steps = o.steps; sp.refine_steps = o.refine_steps; sp.mode = o.mode; sp.flags = o.ssgi_flags;
-    sp.blue_noise_index = k1_phase == 2 ? ch->bn_trace : next_blue(o.blue_noise_start, ch->bn_trace);  // the shading phase reuses the march phase's index
-    // velocityTexture is a null sampler in the shipped wiring (SURVEY.md D4)
-    for (uint32_t blk = 0; blk < 1; blk++) {  // ONE launch covers every owned row block (SegScope installs the segment table)
-      SegScope seg_scope(ctx, ranges, n_blocks, n_launches, k);
-      ctx->viewz_reuse = blk > 0;  // the view-z plane depends on the depth plane only: one prepass per frame
-      ctx->k1_phase = k1_phase;
-      SpanGuard g(ch, cs, 0);
-      st = rfx_ssgi_trace_launch(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, accumulated, &ch->ssgi_out, R0(blk, k), R1(blk, k));
+    sp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_trace);
+    const Rows kr = launch_rows(ranges, k, (int)ch->ssgi_out.height);
+    {
+      SpanGuard g(ch, cs, 0);  // velocityTexture is a null sampler in the shipped wiring (SURVEY.md D4)
+      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, accumulated, &ch->ssgi_out, kr.r0, kr.r1, nullptr);
     }
-    ctx->viewz_reuse = false;
-    ctx->k1_phase = 0;
     if (st != RFX_OK) return st;
   }
   k++;
@@ -1397,14 +1345,13 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     tp.log_transform = 1; tp.history_linear = 1;
     if (o.mode == RFX_MODE_SSGI) { tp.texture_count = 2; tp.input_type = RFX_INPUT_DIFFUSE_SPECULAR; tp.reproject_specular[0] = 0; tp.reproject_specular[1] = 1; }
     else { tp.texture_count = 1; tp.input_type = RFX_INPUT_SPECULAR; tp.reproject_specular[0] = 1; tp.reproject_specular[1] = 1; }
-    for (uint32_t blk = 0; blk < 1; blk++) {  // ONE launch covers every owned row block (SegScope installs the segment table)
-      SegScope seg_scope(ctx, ranges, n_blocks, n_launches, k);
+    {
+      const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, 1);
       // without a denoise pass overrideAccumulatedTextures stays empty: BOTH accumulated textures are the one FramebufferTexture
       rfx_plane* h0 = dm_full ? &ch->dnB[0] : &ch->fb;
       rfx_plane* h1 = dm_full ? &ch->dnB[1] : &ch->fb;
-      st = rfx_temporal_reproject_launch(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0],
-                                         tc == 2 ? &ch->tr[1] : nullptr, R0(blk, k), R1(blk, k));
+      st = temporal_reproject(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0], tc == 2 ? &ch->tr[1] : nullptr, kr.r0, kr.r1);
     }
     if (st != RFX_OK) return st;
     if (!dm_full)  // renderer.copyFramebufferToTexture(tmpVec2, this.framebufferTexture) after the draw (:197-200)
@@ -1429,15 +1376,14 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     rfx_plane* outp = horizontal ? ch->dnA : ch->dnB;
     pp.input_linear = i == 0 ? 0 : 1;
     pp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_poisson);
-    for (uint32_t blk = 0; blk < 1; blk++) {  // ONE launch covers every owned row block (SegScope installs the segment table)
-      SegScope seg_scope(ctx, ranges, n_blocks, n_launches, k);
-      ctx->nrd_reuse = decoded;  // the G-buffer does not change within a frame: decode it once, reuse it afterwards
+    {
+      const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, i == 0 ? 2 : 3);
-      st = rfx_poisson_denoise_launch(ctx, stream, &pp, f->depth, f->gbuffer, &inp[0], tc == 2 ? &inp[1] : nullptr, &outp[0], tc == 2 ? &outp[1] : nullptr,
-                                      R0(blk, k), R1(blk, k));
+      // the G-buffer does not change within a frame: decode it once, reuse it afterwards
+      st = poisson_denoise(ctx, stream, &pp, f->depth, f->gbuffer, &inp[0], tc == 2 ? &inp[1] : nullptr, &outp[0], tc == 2 ? &outp[1] : nullptr, kr.r0, kr.r1,
+                           decoded);
       decoded = true;
     }
-    ctx->nrd_reuse = false;
     if (st != RFX_OK) return st;
   }
   // ---- K4  DenoiserComposePass.render ("full" and "full_temporal": Denoiser.js:55-64)
@@ -1446,59 +1392,23 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     rfx_compose_params cp{};
     cp.cam = f->cam;
     cp.input_type = o.mode == RFX_MODE_SSGI ? RFX_INPUT_DIFFUSE_SPECULAR : RFX_INPUT_SPECULAR;  // SSGIEffect.js:70-77
-    for (uint32_t blk = 0; blk < 1; blk++) {  // ONE launch covers every owned row block (SegScope installs the segment table)
-      SegScope seg_scope(ctx, ranges, n_blocks, n_launches, k);
+    {
+      const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, 4);
-      if (o.mode == RFX_MODE_SSGI) st = rfx_gi_compose_launch(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0], &gi[1], nullptr, &ch->composed, R0(blk, k), R1(blk, k));
-      else st = rfx_gi_compose_launch(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0], f->direct_light, &ch->composed, R0(blk, k), R1(blk, k));  // scene = the composer input buffer (Denoiser.js:100-102)
+      if (o.mode == RFX_MODE_SSGI) st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0], &gi[1], nullptr, &ch->composed, kr.r0, kr.r1);
+      else st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0], f->direct_light, &ch->composed, kr.r0, kr.r1);  // scene = the composer input buffer (Denoiser.js:100-102)
     }
     if (st != RFX_OK) return st;
   }
   k++;
   // ---- TRAA tail over the effect's output (`composed`, or the temporal texture in denoiseMode "temporal")
-  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, accumulated, ranges, n_blocks, n_launches, k);
+  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, accumulated, ranges, k);
   return RFX_OK;
 }
 
 rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f) {
   if (!ch || !f) return RFX_ERR_INVALID_ARG;
-  return chain_render_impl(ch, stream, f, nullptr, 1, 0, 0xffffffffu);
-}
-static rfx_status check_ranges(rfx_ssgi_chain* ch, const uint32_t* ranges, uint32_t n_launches, uint32_t n_blocks) {
-  const uint32_t expect = 3u + 2u * (uint32_t)ch->opt.denoise_iterations + (ch->traa_on ? 1u : 0u);
-  if (n_launches != expect || n_blocks == 0 || n_blocks > RFX_MAX_SEGS) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain ranges: expected %u launches per block, got %u (blocks %u)", expect, n_launches, n_blocks);
-  for (uint32_t i = 0; i < n_launches * n_blocks; i++)
-    if (ranges[2 * i] >= ranges[2 * i + 1] || ranges[2 * i + 1] > ch->opt.height) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain ranges: bad range %u", i);
-  return RFX_OK;
-}
-rfx_status rfx_ssgi_chain_render_ranges(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_launches) {
-  if (!ch || !f || !ranges) return RFX_ERR_INVALID_ARG;
-  rfx_status st = check_ranges(ch, ranges, n_launches, 1);
-  return st != RFX_OK ? st : chain_render_impl(ch, stream, f, ranges, 1, 0, 0xffffffffu);
-}
-rfx_status rfx_ssgi_chain_render_blocks(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_launches,
-                                        uint32_t n_blocks, uint32_t k_begin, uint32_t k_end) {
-  if (!ch || !f || !ranges) return RFX_ERR_INVALID_ARG;
-  rfx_status st = check_ranges(ch, ranges, n_launches, n_blocks);
-  return st != RFX_OK ? st : chain_render_impl(ch, stream, f, ranges, n_blocks, k_begin, k_end);
-}
-
-// A frame in three parts, so a row-sharded caller can put its waits for the exchanged planes exactly where the data is needed:
-// part 0 = K1 ray march (reads depth / G-buffer only), part 1 = K1 shading (samples last frame's `composed`), part 2 = K2..K4
-// (K2 samples last frame's dnB history).  Parts 0+1 together write the same bytes as the fused K1.  ranges may be NULL.
-rfx_status rfx_ssgi_chain_render_part(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t n_launches,
-                                      uint32_t n_blocks, uint32_t part) {
-  if (!ch || !f || part > 2) return RFX_ERR_INVALID_ARG;
-  if (ranges) {
-    rfx_status st = check_ranges(ch, ranges, n_launches, n_blocks);
-    if (st != RFX_OK) return st;
-  }
-  if (part == 2) return chain_render_impl(ch, stream, f, ranges, ranges ? n_blocks : 1, 1, 0xffffffffu);
-  if (ch->fastpath) {  // the fast K1 is one fused kernel (its diffuse rays are compacted inside the block): part 0 is empty, part 1 is K1
-    if (part == 0) return RFX_OK;
-    return chain_render_impl(ch, stream, f, ranges, ranges ? n_blocks : 1, 0, 1, 0);
-  }
-  return chain_render_impl(ch, stream, f, ranges, ranges ? n_blocks : 1, 0, 1, part == 0 ? 1 : 2);
+  return chain_render_impl(ch, stream, f, nullptr, 0, 0xffffffffu);
 }
 
 // Host-buffer path.  submit enqueues one frame and returns: the four input planes go H2D on a copy stream into staging set
@@ -1546,15 +1456,15 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     const int cur = (int)(ch->frame_idx & 1);
     for (int q = 0; q < 2; q++)
       if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, ch->ev_dn[q], 0));
-    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 1, 0, 0xffffffffu)) != RFX_OK) return st;
+    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, 0xffffffffu)) != RFX_OK) return st;
     result = &ch->composed2[cur];
     ch->dn_buf[set] = cur;
   } else {
     const uint32_t n_launches = 3u + 2u * (uint32_t)ch->opt.denoise_iterations;
     const uint32_t split = n_launches - 1;  // K4 is the only launch that writes `composed`
-    if (split && (st = chain_render_impl(ch, nullptr, &f, nullptr, 1, 0, split)) != RFX_OK) return st;
+    if (split && (st = chain_render_impl(ch, nullptr, &f, nullptr, 0, split)) != RFX_OK) return st;
     if (ch->host_submitted >= 1) CU(cudaStreamWaitEvent(ctx->stream, ch->ev_dn[set ^ 1], 0));
-    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 1, split, 0xffffffffu)) != RFX_OK) return st;
+    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, split, 0xffffffffu)) != RFX_OK) return st;
   }
   CU(cudaEventRecord(ch->ev_rendered[set], ctx->stream));
   CU(cudaStreamWaitEvent(ch->s_dn, ch->ev_rendered[set], 0));

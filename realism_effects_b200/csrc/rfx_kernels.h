@@ -13,16 +13,6 @@ struct OutV {  // writable plane view
   long long pitch;
 };
 
-// Output rows of one launch: up to RFX_MAX_SEGS disjoint row segments [r0,r1) (one per row block this rank owns), covered by a
-// single grid: blockIdx.y walks the 16-row tiles of segment 0, then segment 1, ...  One launch per pass regardless of how
-// many row blocks a rank owns (a launch per block costs ~10 % in launch gaps and partial last waves).
-#define RFX_MAX_SEGS 16
-struct RowSegs {
-  int n, tiles;                  // segments, total 16-row tiles (= gridDim.y)
-  int r0[RFX_MAX_SEGS], r1[RFX_MAX_SEGS];
-  int tile0[RFX_MAX_SEGS + 1];   // first tile index of each segment
-};
-
 #define RFX_MAX_PEERS 8
 struct PeerPV {
   PV local;                                    // this rank's allocation (full-frame sized); rows [own0, own1) are valid here
@@ -77,7 +67,6 @@ struct PoissonArgs {
   PV depth, gb, in0, in1;
   OutV out0, out1;
   int W, H, row0, row1;
-  RowSegs segs;
   float radius, phi, luma_phi, depth_phi, normal_phi, roughness_phi, specular_phi;
   int texture_count, spec0, spec1, gbuffer_texture, input_linear, in_half;
   BlueD blue;
@@ -88,14 +77,13 @@ struct PoissonArgs {
 };
 cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s);       // exact-libm variant (any configuration)
 cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s);  // SFU variant (GBUFFER_TEXTURE configurations)
-cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_texture, const RowSegs& segs, int halo, cudaStream_t s);
+cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_texture, int row0, int row1, int halo, cudaStream_t s);
 
 // ---- K4 / K5 -------------------------------------------------------------------------------
 struct ComposeArgs {
   PV depth, gb, diffuse, specular, scene;  // diffuse / specular / scene: p == nullptr = not bound (null sampler)
   OutV out;
   int W, H, row0, row1;
-  RowSegs segs;
   CamD cam;
   int input_type;
   int gi_f32;  // diffuse / specular are RGBA32F NEAREST (denoiseMode "full_temporal": the temporal pass's targets)
@@ -138,7 +126,6 @@ struct TemporalArgs {
   PV input, velocity, hist0, hist1;
   OutV out0, out1;
   int W, H, row0, row1;
-  RowSegs segs;
   CamD cam;
   M4 prev_view, prev_world, prev_proj, prev_proj_inv;
   M4 prev_proj_view;  // prevProjectionMatrix * prevViewMatrix (reproject.frag:183), fma-lowered on the host
@@ -153,7 +140,7 @@ struct TemporalArgs {
 };
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
 
-// TRAA frame tail of the fast chain (k_temporal.cu: ctraa_kernel): K5 -> K2 (TRAA form) -> K9 in one launch over the rows of `t.segs`.
+// TRAA frame tail of the fast chain (k_temporal.cu: ctraa_kernel): K5 -> K2 (TRAA form) -> K9 in one launch over rows [t.row0, t.row1).
 // `t` carries the TRAA K2 uniforms exactly as rfx_temporal_reproject_launch fills them (input_half = out_half = history_linear = 1,
 // texture_count 1, input_type DIFFUSE); `k5.gi` is `composed`, `k5.scene` the direct light; history rows live on their owners.
 struct CTraaArgs {
@@ -170,7 +157,6 @@ struct SsgiArgs {
   PV depth, gb, velocity, direct, accumulated;  // velocity/direct/accumulated may have p == nullptr
   OutV out;
   int W, H, row0, row1;
-  RowSegs segs;
   CamD cam;
   float ray_distance, thickness, env_blur, max_env_mip;
   float near_minus_far, near_mul_far, far_minus_near;
@@ -183,17 +169,10 @@ struct SsgiArgs {
   PV viewz;                  // R32F: getViewZ(depth) per texel (launch_viewz prepass)
   int proj_sparse;           // projection matrix has the perspective sparsity pattern (exact-zero terms dropped)
   int fast;                  // SFU variants of the continuous transcendentals
-  int phase;                 // 0 fused; 1 ray march only -> rec; 2 shading from rec (k_ssgi.cu "Split-phase K1")
-  unsigned char* rec;        // 2 x float4 per pixel (diffuse ray, specular ray)
-  long long rec_pitch;
   // fast fused kernel (ssgi_fast_kernel)
   float ps_x0, ps_x2, ps_y1, ps_y2, ps_hw, ps_hh;  // projection rows scaled to texel units: tx = (ps_x0*x + ps_x2*z) / -z + ps_hw
   int vz_pitchw;             // viewZ pitch in 4-byte words
-  int vz_tiled;              // experiment (RFX_K1_VZ_TILED=1): the viewZ scratch is stored as 8x4-texel tiles (one 128-B line each) for the fast kernel's gathers
-  int vz_tiles_x;            // tiles per tile row
-  int legacy_fast;           // 1: use the round-1 fast kernel (tools/ A/B comparisons)
   int scaled;                // the render target (W x H) is smaller than the input planes (resolutionScale < 1): texels are fetched by uv
-  int march_batch;           // march steps fetched together before they are tested: 1, 2 or 4
   PeerPV acc_peer;           // `accumulated` in a row-sharded group (n > 1): rows live on their owners
 };
 cudaError_t launch_ssgi(const SsgiArgs& a, cudaStream_t s);
@@ -299,14 +278,13 @@ cudaError_t launch_env_cdf(PV map, int flip_y, float* cdf_c, float* cdf_m, doubl
 // Row-sharded multi-GPU frames read last frame's `composed` / `dn` rows owned by other ranks in place over NVLink (PeerPV).
 // ==========================================================================================
 struct CDecodeArgs { PV gb, depth; OutV nrdz; int W, H; };
-cudaError_t launch_cdecode(const CDecodeArgs& a, const RowSegs& segs, int halo, cudaStream_t s);
+cudaError_t launch_cdecode(const CDecodeArgs& a, int row0, int row1, int halo, cudaStream_t s);
 
 struct CTemporalArgs {
   PV input, velocity;   // K1 output (packed), velocity plane
   PeerPV hist;          // dn of the previous frame
   OutV out;             // tr
-  int W, H;
-  RowSegs segs;
+  int W, H, row0, row1;
   CamD cam;
   M4 prev_world, prev_proj_inv, prev_proj_view;
   float camera_pos[3];
@@ -319,8 +297,7 @@ cudaError_t launch_ctemporal(const CTemporalArgs& a, cudaStream_t s);
 struct CPoissonArgs {
   PV nrdz, in;          // in: tr (pass 0) or dn (passes >= 1)
   OutV out;             // dn
-  int W, H;
-  RowSegs segs;
+  int W, H, row0, row1;
   float radius, phi, luma_phi, depth_phi, normal_phi, roughness_phi, specular_phi;
   BlueD blue;
   const float2* rot_table;
@@ -330,10 +307,9 @@ struct CPoissonArgs {
   // `out` is double-buffered by frame parity when it is the history plane: a discarded pixel (the reference's "target keeps its
   // texel", SURVEY.md A2) then copies last frame's texel forward.  carry.local.p == nullptr: single-buffered target, no write.
   PeerPV carry;
-  // fused GI compose (last pass): rows of `csegs` also write `composed` (discarded pixels carry last frame's texel forward)
+  // fused GI compose (last pass): rows [crow0, crow1) also write `composed` (discarded pixels carry last frame's texel forward)
   int compose;
-  int compose_mode;     // arithmetic of the fused K4: 0 IEEE, 1 SFU, 2 SFU + one Newton step (k_chain.cu: c_compose_t)
-  RowSegs csegs;
+  int crow0, crow1;
   PV gb;
   OutV composed;
   PeerPV composed_carry;
@@ -348,12 +324,10 @@ struct CPoissonTmaArgs {  // passes >= 1 with TMA-staged tiles (experiment, RFX_
 cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s);
 
 struct CComposeArgs {   // stand-alone K4 over dn (denoiseIterations == 0)
-  int compose_mode;
   PV nrdz, gb, dn;
   OutV composed;
   PeerPV composed_carry;
-  int W, H;
-  RowSegs segs;
+  int W, H, row0, row1;
   CamD cam;
 };
 cudaError_t launch_ccompose(const CComposeArgs& a, cudaStream_t s);
@@ -370,30 +344,12 @@ RFX_D void block_pixel(int& x, int& y, int row_base) {
   x = blockIdx.x * kTileW + ((warp & 1) << 3) + lx;
   y = row_base + blockIdx.y * kTileH + ((warp >> 1) << 2) + ly;
 }
-// pixel of this thread for a multi-segment launch; returns whether its row lies inside the segment (quads stay aligned to
-// even rows because every segment's tiles start at r0 & ~1)
-RFX_D bool seg_pixel(const RowSegs& s, int& x, int& y) {
-  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lx, ly;
-  lane_to_pixel(lane, lx, ly);
-  int k = 0;
-  const int ty = blockIdx.y;
-  while (k + 1 < s.n && ty >= s.tile0[k + 1]) k++;
-  x = blockIdx.x * kTileW + ((warp & 1) << 3) + lx;
-  y = (s.r0[k] & ~1) + (ty - s.tile0[k]) * kTileH + ((warp >> 1) << 2) + ly;
-  return y >= s.r0[k] && y < s.r1[k];
+// A launch over output rows [row0, row1) covers them with 16-row tiles starting at row0 & ~1, so that quads stay aligned to
+// even rows.  range_pixel: the pixel of this thread; returns whether its row lies inside the range.  row_tiles: gridDim.y.
+RFX_D bool range_pixel(int row0, int row1, int& x, int& y) {
+  block_pixel(x, y, row0 & ~1);
+  return y >= row0 && y < row1;
 }
-// host: build the segment table
-inline RowSegs make_segs(const int* r0, const int* r1, int n) {
-  RowSegs s{};
-  s.n = n;
-  int t = 0;
-  for (int i = 0; i < n; i++) {
-    s.r0[i] = r0[i]; s.r1[i] = r1[i]; s.tile0[i] = t;
-    t += (r1[i] - (r0[i] & ~1) + kTileH - 1) / kTileH;
-  }
-  s.tile0[n] = t;
-  s.tiles = t;
-  return s;
-}
+inline int row_tiles(int row0, int row1) { return (row1 - (row0 & ~1) + kTileH - 1) / kTileH; }
 
 }  // namespace rfx

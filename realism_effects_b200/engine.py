@@ -268,31 +268,9 @@ class SsgiChain:
         f.camera_moved = int(camera_moved)
         return f
 
-    def render(self, cam: abi.CameraS, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None, ranges=None, launches=None):
-        """ranges: optional list of (row0, row1) per launch (K1, K2, K3 passes..., K4) for row-block sharding, or a list of such
-        lists (one per owned row block); launches = (k_begin, k_end) restricts the call to a window of launches (frame phases)."""
+    def render(self, cam: abi.CameraS, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None):
         f = self._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
-        if ranges is None:
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render(self.h, stream, C.byref(f)))
-        elif ranges and isinstance(ranges[0][0], (tuple, list)):  # [block][launch] -> (row0, row1), optional launch window
-            nb, nl = len(ranges), len(ranges[0])
-            flat = (C.c_uint32 * (2 * nb * nl))(*[int(v) for blk in ranges for r in blk for v in r])
-            k0, k1 = launches if launches is not None else (0, nl)
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_blocks(self.h, stream, C.byref(f), flat, nl, nb, k0, k1))
-        else:
-            flat = (C.c_uint32 * (2 * len(ranges)))(*[int(v) for r in ranges for v in r])
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_ranges(self.h, stream, C.byref(f), flat, len(ranges)))
-
-    def render_part(self, part: int, cam: abi.CameraS, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None, ranges=None):
-        """One of the three parts of a frame (include/rfx.h: rfx_ssgi_chain_render_part): 0 = K1 ray march, 1 = K1 shading,
-        2 = K2..K4.  ranges: None (whole planes) or [block][launch] -> (row0, row1)."""
-        f = self._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
-        if ranges is None:
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_part(self.h, stream, C.byref(f), None, 0, 0, part))
-        else:
-            nb, nl = len(ranges), len(ranges[0])
-            flat = (C.c_uint32 * (2 * nb * nl))(*[int(v) for blk in ranges for r in blk for v in r])
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_part(self.h, stream, C.byref(f), flat, nl, nb, part))
+        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render(self.h, stream, C.byref(f)))
 
     def output(self, which: int = 0) -> Plane:
         """0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA accumulated plane"""

@@ -13,7 +13,8 @@ from realism_effects_b200 import abi
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_exports_every_declared_symbol(built):
+def test_library_exports_the_declared_abi(built):
+    """Every rfx_* function include/rfx.h declares is exported and listed in abi.EXPORTS, and the library reports ABI version 3."""
     hdr = open(os.path.join(ROOT, "include", "rfx.h")).read()
     declared = sorted(set(re.findall(r"\b(rfx_[a-z0-9_]+)\s*\(", hdr)))
     assert len(declared) >= 30
@@ -21,7 +22,7 @@ def test_library_exports_every_declared_symbol(built):
     missing = [n for n in declared if not hasattr(lib, n)]
     assert not missing, missing
     assert sorted(set(abi.EXPORTS)) == declared
-    assert lib.rfx_version() == 2
+    assert lib.rfx_version() == 3
     assert [lib.rfx_format_bytes(f) for f in range(4)] == [4, 16, 8, 4]
 
 

@@ -94,33 +94,6 @@ def test_host_buffer_paths_match_device_path(built):
             ctx.close()
 
 
-@pytest.mark.parametrize("fast", [True, False])
-def test_three_part_frame_equals_fused_frame(built, fast):
-    """rfx_ssgi_chain_render_part: K1 ray march -> K1 shading from the march records -> K2..K4 writes, frame after frame, the bytes
-    of the fused chain (the exact variant has no split kernels: part 0 is empty, part 1 the fused K1)."""
-    from realism_effects_b200 import abi, engine
-
-    o = ch.Opts(denoise_iterations=1)
-    for kw in (dict(), dict(refine_steps=0, missed_rays=True), dict(importance_sampling=False)):
-        o = ch.Opts(denoise_iterations=1, **kw)
-        inp = ch.make_inputs(176, 100, 3)
-        want, _ = ch.run_cuda_chain(inp, o, fast_math=fast)
-        ctx = engine.Context(0, inp.blue)
-        ctx.set_fast_math(fast)
-        try:
-            ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
-            chain = engine.SsgiChain(ctx, ch.chain_options(inp, o))
-            for t, fr in enumerate(inp.frames):
-                pl = [ctx.upload(fr[k]) for k in ("depth", "gbuffer", "velocity", "direct")]
-                for part in (0, 1, 2):
-                    chain.render_part(part, abi.make_camera(fr["cam"]), *pl, fr["cam"]["position"], fr["moved"])
-                for k, which in (("composed", 0), ("ssgi", 1), ("tr0", 2), ("tr1", 3), ("dn0", 4), ("dn1", 5)):
-                    assert chain.download(which).tobytes() == want[t][k].tobytes(), (kw, t, k)
-            chain.close()
-        finally:
-            ctx.close()
-
-
 def test_group_of_one_rank_equals_plain_chain(built):
     """rfx_group_* with world = 1 on a single GPU: NCCL is loaded and initialised, the chain is attached, every frame ends with the
     group's collective, the band is the whole frame — and the bytes are those of rfx_ssgi_chain_render.  (The peer-mapped reads need
