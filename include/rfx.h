@@ -489,14 +489,21 @@ rfx_status rfx_ssgi_chain_wait_host(rfx_ssgi_chain* chain, int32_t max_in_flight
  * IN PLACE on the rank that owns the row, through CUDA-IPC peer mappings over NVLink, instead of being replicated.  The group
  * owns an NCCL communicator for its one collective per frame (an all-gather of every rank's device-timed kernel cost, which is
  * also the frame barrier) and the band table with its cost-driven rebalancing.  Results are bit-identical to the single-GPU
- * chain.  NCCL is loaded at run time (libnccl.so.2); without it every entry below returns RFX_ERR_NCCL. */
+ * chain.  NCCL is loaded at run time (libnccl.so.2); without it every entry below returns RFX_ERR_NCCL.
+ * A group takes chains created with fast_math on and resolution_scale 1, in every mode and denoise_mode: the fast SSGI chain, and the
+ * per-pass chain (mode SSR; denoise_mode full_temporal / temporal).  In a group of n > 1 the per-pass chain double-buffers every plane
+ * it keeps across frames by frame parity (at attach time), reads last frame's rows on their owners (K1, K2 and the TRAA history) and
+ * carries the texel of a discarded pixel from the owner (K2, K3, K4).  fast_math off or resolution_scale < 1: RFX_ERR_UNSUPPORTED,
+ * returned on the refusing rank before any collective, so every rank must pass chains the group takes. */
 typedef struct rfx_group rfx_group;
 #define RFX_GROUP_ID_BYTES 128
 rfx_status rfx_group_get_unique_id(void* id128);   /* rank 0; hand the 128 bytes to the other ranks by any means */
 rfx_status rfx_group_create(rfx_ctx* ctx, const void* id128, int32_t rank, int32_t world, rfx_group** out);  /* collective */
 /* The same group without NCCL / CUDA IPC: `world` members that live in ONE process (one context each — on one device or on several
  * devices with peer access — or all on the same context).  Create every member with rfx_group_create_inprocess, give every member a
- * fast SSGI chain with identical options, then attach them all at once: the members read each other's history planes through plain
+ * chain with identical options (a chain the group does not take - fast_math off, resolution_scale < 1 - is RFX_ERR_UNSUPPORTED; members
+ * whose mode, denoise_mode or chain path differ: RFX_ERR_INVALID_ARG), then attach them all at
+ * once: the members read each other's history planes through plain
  * device pointers.  The host renders a frame by calling rfx_ssgi_chain_render_sharded for every member (any order, same stream or
  * streams it orders itself) before any member starts the next frame.  Bands are static unless moved with rfx_group_set_bounds.
  * Besides single-process multi-GPU hosts, this is what lets a 1-GPU box exercise the N-band logic (tests/test_gpu_chain.py). */
@@ -505,7 +512,8 @@ rfx_status rfx_group_attach_chains_inprocess(rfx_group* const* groups, rfx_ssgi_
 void rfx_group_destroy(rfx_group* group);
 int32_t rfx_group_rank(const rfx_group* group);
 int32_t rfx_group_world(const rfx_group* group);
-/* collective: maps every rank's history planes of `chain` (a fast SSGI chain with the same options on every rank) */
+/* collective: maps every rank's history planes of `chain` (the same options on every rank: a mode, denoise_mode, fast_math or TRAA
+ * tail that differs between ranks is RFX_ERR_INVALID_ARG on every rank) */
 rfx_status rfx_group_attach_chain(rfx_group* group, rfx_ssgi_chain* chain);
 /* band borders: world + 1 ascending rows, bounds[0] = 0, bounds[world] = height; rank r owns rows [bounds[r], bounds[r+1]) */
 rfx_status rfx_group_get_bounds(const rfx_group* group, uint32_t* bounds);
@@ -514,7 +522,7 @@ rfx_status rfx_group_set_bounds(rfx_group* group, const uint32_t* bounds);   /* 
 rfx_status rfx_group_set_rebalance(rfx_group* group, int32_t every, int32_t lag);
 rfx_status rfx_group_last_costs(const rfx_group* group, float* ms_per_rank);  /* the times the last rebalance used */
 /* 1: history rows are read in place on their owner (CUDA IPC peer mappings); 0: the mappings could not be opened on some rank (or
- * RFX_GROUP_EXCHANGE=allgather is set) and the group replicates the two history planes with an NCCL exchange after every frame */
+ * RFX_GROUP_EXCHANGE=allgather is set) and the group replicates the history planes with an NCCL exchange after every frame */
 int32_t rfx_group_uses_peer_reads(const rfx_group* group);
 /* in lockstep on every rank, no communication: applies the border move that is due and returns the borders of the NEXT frame
  * (render_sharded calls it implicitly; a host path calls it first to size its uploads) */
@@ -528,7 +536,10 @@ rfx_status rfx_ssgi_chain_render_sharded(rfx_ssgi_chain* chain, void* stream, co
 /* pure host arithmetic, exported for hosts that plan their bands with it (and for the CPU tests): the ranges render_sharded uses,
  * rows [ranges[2k], ranges[2k+1]) of launch k (K1, K2, K3 pass 0.., K4) for the band [own0, own1); n_launches = 3 + n_poisson_passes.
  * n_launches = 4 + n_poisson_passes: the same with the TRAA tail as the last launch; it runs on the band and K4 on the band widened
- * by RFX_TRAA_TAIL_ROWS (every earlier launch widens with it). */
+ * by RFX_TRAA_TAIL_ROWS (every earlier launch widens with it).
+ * denoise_mode full_temporal / temporal run no Poisson pass: render_sharded plans them with n_poisson_passes = 0 (K1, K2, K4 and the
+ * tail, 3 or 4 launches), so K1 / K2 widen only by K2's window, and maps the chain's launches onto them (K1, K2, then K4 and the tail
+ * after the 2 * denoise_iterations Poisson slots, which are not launched).  "temporal" launches no K4 either; its range is K2's. */
 #define RFX_TRAA_TAIL_ROWS 4  /* 2: the 5x5 clamp window; 1: its LINEAR fetches at texel centres touch row y +- 1; 1: K9's LINEAR fetch
                                  of the accumulated plane at the pixel centre (same reason).  The TRAA form takes no derivative,
                                  so no quad row is added. */

@@ -550,7 +550,7 @@ export class TAAPass {
 }
 
 // ---- one Node process, several GPUs: a row-sharded group whose members live in this process (rfx_group_create_inprocess) -------------------------
-// Every member owns a context (one per device), a fast SSGI chain with identical options and a band of rows; halo rows are recomputed, last
+// Every member owns a context (one per device), a chain with identical options (fast_math on, resolutionScale 1) and a band of rows; halo rows are recomputed, last
 // frame's history rows are read in place on the member that owns them.  The per-device planes come from the caller (one PlaneSource per device).
 export class InProcessGroup {
 	constructor(devices, chainOptions) {

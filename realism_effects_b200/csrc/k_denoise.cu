@@ -18,8 +18,9 @@ RFX_D v4 fetch_in(const PV& t, v2 uv) {
   return f4v(tex_f4_nearest(t, uv));        // pass 0 reads the NEAREST fp32 temporal targets
 }
 
-template <int TC, bool GB, bool LINEAR, bool HALF>
-__global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant__ PoissonArgs a) {
+// CARRY (row-sharded group): out0 / out1 are double-buffered and a discarded pixel copies last frame's texels from their owner (`c`)
+template <int TC, bool GB, bool LINEAR, bool HALF, bool CARRY>
+__global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant__ PoissonArgs a, const __grid_constant__ PeerCarry c) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
@@ -33,7 +34,10 @@ __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant
   const v3 normal = unpackNormal(GB ? gbc.y : gbc.z);      // getNormal()  :80-87
   const float fwn = length(fwidth_3(normal));              // :172
   if (!active) return;
-  if (depth == 1.0f && fwd == 0.0f) return;                // discard :129-132 (target keeps its texel)
+  if (depth == 1.0f && fwd == 0.0f) {                      // discard :129-132 (target keeps its texel)
+    if (CARRY) { carry_texel<8>(c.p[0], a.out0, x, y); if (TC == 2) carry_texel<8>(c.p[1], a.out1, x, y); }
+    return;
+  }
 
   // mat = getMaterial(gBufferTexture, vUv) — without GBUFFER_TEXTURE the sampler is null => texel (0,0,0,1)
   const float roughness = GB ? gb_roughness(gbc.z) : gb_roughness(0.0f);
@@ -187,11 +191,12 @@ RFX_D void fetch2(const PoissonArgs& a, v2 uv, bool two, v3& c0, v3& c1, float* 
 }
 
 // TC planes; plane j is "specular" per a.spec0/spec1; with TC == 2 plane 1 reads in1, with TC == 1 the single plane reads in0.
-template <int TC, bool LINEAR, bool GB>
+// CARRY: as poisson_kernel's
+template <int TC, bool LINEAR, bool GB, bool CARRY>
 #ifndef RFX_K3_MIN_BLOCKS
 #define RFX_K3_MIN_BLOCKS 4
 #endif
-__global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kernel(const __grid_constant__ PoissonArgs a) {
+__global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kernel(const __grid_constant__ PoissonArgs a, const __grid_constant__ PeerCarry c) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
@@ -203,7 +208,10 @@ __global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kern
   const v3 normal = mk3(nc.x, nc.y, nc.z);
   const float fwn = length(fwidth_3(normal));
   if (!active) return;
-  if (depth == 1.0f && fwd == 0.0f) return;
+  if (depth == 1.0f && fwd == 0.0f) {
+    if (CARRY) { carry_texel<8>(c.p[0], a.out0, x, y); if (TC == 2) carry_texel<8>(c.p[1], a.out1, x, y); }
+    return;
+  }
   const float roughness = GB ? nc.w : 0.0f;  // without GBUFFER_TEXTURE getMaterial() decodes the null sampler's (0,0,0,1): roughness 0 (A8)
 
   v3 rgb[2];
@@ -280,20 +288,24 @@ __global__ void __launch_bounds__(kThreads, RFX_K3_MIN_BLOCKS) poisson_fast_kern
   }
 }
 
-cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s) {
+cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s, const PeerCarry* carry) {
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
   if (a.input_linear && !a.in_half) return cudaErrorInvalidValue;
   if (!a.input_linear && a.in_half) return cudaErrorNotSupported;
-#define RFX_PF(TC, LIN) do { if (a.gbuffer_texture) poisson_fast_kernel<TC, LIN, true><<<grid, kThreads, 0, s>>>(a); else poisson_fast_kernel<TC, LIN, false><<<grid, kThreads, 0, s>>>(a); } while (0)
+  const PeerCarry c = carry ? *carry : PeerCarry{};
+#define RFX_PF2(TC, LIN, GB) do { if (carry) poisson_fast_kernel<TC, LIN, GB, true><<<grid, kThreads, 0, s>>>(a, c); else poisson_fast_kernel<TC, LIN, GB, false><<<grid, kThreads, 0, s>>>(a, c); } while (0)
+#define RFX_PF(TC, LIN) do { if (a.gbuffer_texture) RFX_PF2(TC, LIN, true); else RFX_PF2(TC, LIN, false); } while (0)
   if (a.texture_count == 2) { if (a.input_linear) RFX_PF(2, true); else RFX_PF(2, false); }
   else { if (a.input_linear) RFX_PF(1, true); else RFX_PF(1, false); }
 #undef RFX_PF
+#undef RFX_PF2
   return cudaGetLastError();
 }
 
-cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s) {
+cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s, const PeerCarry* carry) {
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
-#define RFX_LP(TC, GB, LIN, HALF) poisson_kernel<TC, GB, LIN, HALF><<<grid, kThreads, 0, s>>>(a)
+  const PeerCarry c = carry ? *carry : PeerCarry{};
+#define RFX_LP(TC, GB, LIN, HALF) do { if (carry) poisson_kernel<TC, GB, LIN, HALF, true><<<grid, kThreads, 0, s>>>(a, c); else poisson_kernel<TC, GB, LIN, HALF, false><<<grid, kThreads, 0, s>>>(a, c); } while (0)
   const bool lin = a.input_linear, half = a.in_half, gb = a.gbuffer_texture;
   if (lin && !half) return cudaErrorInvalidValue;
   if (a.texture_count == 2) {
@@ -307,7 +319,9 @@ cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
-__global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_constant__ ComposeArgs a) {
+// CARRY: `out` is double-buffered and a discarded pixel copies last frame's texel from its owner (`c`), as in poisson_kernel
+template <bool CARRY>
+__global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_constant__ ComposeArgs a, const __grid_constant__ PeerPV c) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
   const bool active = x < a.W && y < a.H && in_rows;
@@ -315,7 +329,10 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
   const float depth = ld_r32f(a.depth, xc, yc);
   const float fwd = fwidth_f(depth);
   if (!active) return;
-  if (depth == 1.0f && fwd == 0.0f) return;  // DenoiserComposePass.js:61-64
+  if (depth == 1.0f && fwd == 0.0f) {  // DenoiserComposePass.js:61-64
+    if (CARRY) carry_texel<16>(c, a.out, x, y);
+    return;
+  }
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
   const float4 g = ld_f4(a.gb, x, y);
   const v3 diffuse = xyz(floatToVec4(g.x));
@@ -376,9 +393,10 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
   st_f4(a.out.p, a.out.pitch, x, y, make_float4(gi.x, gi.y, gi.z, 1.0f));
 }
 
-cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s) {
+cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s, const PeerPV* carry) {
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
-  gi_compose_kernel<<<grid, kThreads, 0, s>>>(a);
+  if (carry) gi_compose_kernel<true><<<grid, kThreads, 0, s>>>(a, *carry);
+  else gi_compose_kernel<false><<<grid, kThreads, 0, s>>>(a, PeerPV{});
   return cudaGetLastError();
 }
 

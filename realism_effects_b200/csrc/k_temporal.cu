@@ -95,6 +95,16 @@ RFX_D v4 fetch_hist(const TemporalArgs&, const PeerPV& t, v2 uv) {  // the fused
   return peer_h4_linear(t, uv);
 }
 
+// the per-pass chain in a row-sharded group: its history (RGBA16F `dn`, or the RGBA32F temporal target) with rows on their owners
+struct PeerHist {
+  const PeerPV& p;
+};
+template <bool HLIN>
+RFX_D v4 fetch_hist(const TemporalArgs& a, const PeerHist& t, v2 uv) {
+  static_assert(HLIN, "the chain's history is sampled LINEAR");
+  return a.hist_f32 ? peer_f4_linear(t.p, uv) : peer_h4_linear(t.p, uv);
+}
+
 // BiCubicCatmullRom5Tap  reproject.frag:212-255
 template <bool HLIN, class Hist>
 RFX_D v4 catmull5(const TemporalArgs& a, const Hist& tex, v2 P) {
@@ -307,6 +317,43 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(c
   s.curvature = length(fwidth_3(s.worldNormal));  // getCurvature :265-269
   if (!active) return;
   temporal_px<TC, ITYPE, LOG, HLIN, FAST>(a, PlaneH4{a.input}, a.hist0, a.hist1, s, fwd, x, y, PlaneStore{a, x, y});
+}
+
+// K2 with the history read on the owners and the carry of discarded pixels (TemporalPeer).  temporal_px returns without a store
+// exactly where the shader discards, so a pixel whose planes were not stored copies last frame's texels of out0 / out1.
+struct StoreSeen {
+  PlaneStore s;
+  bool* seen;
+  RFX_D void operator()(int i, v4 v) const { *seen = true; s(i, v); }
+};
+template <int TC, int ITYPE, bool LOG>
+__global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_peer_kernel(const __grid_constant__ TemporalArgs a, const __grid_constant__ TemporalPeer p) {
+  int x, y;
+  const bool in_rows = range_pixel(a.row0, a.row1, x, y);
+  const bool active = x < a.W && y < a.H && in_rows;
+  TState s;
+  temporal_state(a, x, y, min(x, a.W - 1), min(y, a.H - 1), s);
+  const float fwd = fwidth_f(s.depth);
+  s.curvature = length(fwidth_3(s.worldNormal));
+  if (!active) return;
+  bool seen = false;
+  temporal_px<TC, ITYPE, LOG, true, true>(a, PlaneH4{a.input}, PeerHist{p.hist0}, PeerHist{p.hist1}, s, fwd, x, y, StoreSeen{PlaneStore{a, x, y}, &seen});
+  if (ITYPE != RFX_INPUT_DIFFUSE && !seen) {
+    if (a.out_half) { carry_texel<8>(p.carry.p[0], a.out0, x, y); if (TC == 2) carry_texel<8>(p.carry.p[1], a.out1, x, y); }
+    else { carry_texel<16>(p.carry.p[0], a.out0, x, y); if (TC == 2) carry_texel<16>(p.carry.p[1], a.out1, x, y); }
+  }
+}
+
+cudaError_t launch_temporal_peer(const TemporalArgs& a, const TemporalPeer& p, cudaStream_t s) {
+  if (!a.history_linear || !a.fast || a.in_scaled) return cudaErrorNotSupported;
+  dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
+#define RFX_LTP(TC, IT) do { if (a.log_transform) temporal_peer_kernel<TC, IT, true><<<grid, kThreads, 0, s>>>(a, p); else temporal_peer_kernel<TC, IT, false><<<grid, kThreads, 0, s>>>(a, p); } while (0)
+  if (a.input_type == RFX_INPUT_DIFFUSE_SPECULAR && a.texture_count == 2) RFX_LTP(2, RFX_INPUT_DIFFUSE_SPECULAR);
+  else if (a.input_type == RFX_INPUT_DIFFUSE && a.texture_count == 1) RFX_LTP(1, RFX_INPUT_DIFFUSE);
+  else if (a.input_type == RFX_INPUT_SPECULAR && a.texture_count == 1) RFX_LTP(1, RFX_INPUT_SPECULAR);
+  else return cudaErrorNotSupported;
+#undef RFX_LTP
+  return cudaGetLastError();
 }
 
 template <int TC, int IT, bool FAST>

@@ -492,7 +492,8 @@ rfx_status rfx_ssgi_trace_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_para
 
 // K2
 static rfx_status temporal_reproject(rfx_ctx* ctx, void* stream, const rfx_temporal_params* p, const rfx_plane* input, const rfx_plane* velocity,
-                                     const rfx_plane* history0, const rfx_plane* history1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1) {
+                                     const rfx_plane* history0, const rfx_plane* history1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1,
+                                     const TemporalPeer* peer = nullptr) {  // peer: history on the owners + carry (launch_temporal_peer)
   TemporalArgs a{};
   if (p->texture_count != 1 && p->texture_count != 2) return fail(ctx, RFX_ERR_INVALID_ARG, "temporal: texture_count must be 1 or 2");
   a.input_half = input->format == RFX_FMT_RGBA16F;
@@ -514,7 +515,8 @@ static rfx_status temporal_reproject(rfx_ctx* ctx, void* stream, const rfx_tempo
   if (a.in_scaled && a.input_half) return fail(ctx, RFX_ERR_UNSUPPORTED, "temporal: a scaled input is the RGBA32F SSGI target");
   a.row0 = r0; a.row1 = r1;
   temporal_uniforms(ctx, p, a);
-  LAUNCHED(launch_temporal(a, pick(ctx, stream)));
+  if (peer) LAUNCHED(launch_temporal_peer(a, *peer, pick(ctx, stream)));
+  else LAUNCHED(launch_temporal(a, pick(ctx, stream)));
   return RFX_OK;
 }
 rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_temporal_params* p, const rfx_plane* input, const rfx_plane* velocity,
@@ -528,7 +530,8 @@ rfx_status rfx_temporal_reproject_launch(rfx_ctx* ctx, void* stream, const rfx_t
 
 // K3.  decoded: the context's G-buffer scratch already holds this frame's decode (the chain decodes once per frame)
 static rfx_status poisson_denoise(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p, const rfx_plane* depth, const rfx_plane* gb, const rfx_plane* in0,
-                                  const rfx_plane* in1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1, bool decoded) {
+                                  const rfx_plane* in1, const rfx_plane* out0, const rfx_plane* out1, int r0, int r1, bool decoded,
+                                  const PeerCarry* carry = nullptr) {
   if (p->texture_count != 1 && p->texture_count != 2) return fail(ctx, RFX_ERR_INVALID_ARG, "poisson: texture_count must be 1 or 2");
   PoissonArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gb, RFX_FMT_RGBA32F, a.gb)) return fail(ctx, RFX_ERR_BAD_FORMAT, "poisson: depth R32F + gbuffer/normal RGBA32F required");
@@ -558,7 +561,7 @@ static rfx_status poisson_denoise(rfx_ctx* ctx, void* stream, const rfx_poisson_
   a.rot_table = ctx->rot_table;
   const bool fast = ctx->fast_math && ((p->input_linear && a.in_half) || (!p->input_linear && !a.in_half));
   if (!fast) {
-    LAUNCHED(launch_poisson(a, pick(ctx, stream)));
+    LAUNCHED(launch_poisson(a, pick(ctx, stream), carry));
     return RFX_OK;
   }
   // fast variant: decode the G-buffer once into the context scratch (the native chain reuses it across the passes of a frame)
@@ -581,7 +584,7 @@ static rfx_status poisson_denoise(rfx_ctx* ctx, void* stream, const rfx_poisson_
     const float py[8] = {0.0f, -1.0f, 0.0f, 1.0f, -0.25f * SQ, -0.25f * SQ, 0.25f * SQ, 0.25f * SQ};
     for (int i = 0; i < 8; i++) { a.tap_ox[i] = px[i] / (float)a.W; a.tap_oy[i] = py[i] / (float)a.H; }  // offset / resolution
   }
-  LAUNCHED(launch_poisson_fast(a, pick(ctx, stream)));
+  LAUNCHED(launch_poisson_fast(a, pick(ctx, stream), carry));
   return RFX_OK;
 }
 rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_poisson_params* p, const rfx_plane* depth, const rfx_plane* gb,
@@ -595,7 +598,7 @@ rfx_status rfx_poisson_denoise_launch(rfx_ctx* ctx, void* stream, const rfx_pois
 
 // K4
 static rfx_status gi_compose(rfx_ctx* ctx, void* stream, const rfx_compose_params* p, const rfx_plane* depth, const rfx_plane* gb, const rfx_plane* dgi,
-                             const rfx_plane* sgi, const rfx_plane* scene, const rfx_plane* out, int r0, int r1) {
+                             const rfx_plane* sgi, const rfx_plane* scene, const rfx_plane* out, int r0, int r1, const PeerPV* carry = nullptr) {
   ComposeArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gb, RFX_FMT_RGBA32F, a.gb) || !ov(out, RFX_FMT_RGBA32F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "gi_compose: depth R32F, gbuffer RGBA32F, out RGBA32F required");
@@ -617,7 +620,7 @@ static rfx_status gi_compose(rfx_ctx* ctx, void* stream, const rfx_compose_param
   cam_to_dev(p->cam, a.cam);
   a.input_type = p->input_type;
   a.fast = ctx->fast_math;
-  LAUNCHED(launch_gi_compose(a, pick(ctx, stream)));
+  LAUNCHED(launch_gi_compose(a, pick(ctx, stream), carry));
   return RFX_OK;
 }
 rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_params* p, const rfx_plane* depth, const rfx_plane* gb,
@@ -843,12 +846,27 @@ struct rfx_ssgi_chain {
   float traa_keep = 0.0f;               // keepData of the TRAA pass
   rfx_temporal_params traa_tp{};        // the frame's camera and the previous-frame matrices its K2 used
   PeerPV peer_traa[2]{};
+  // per-pass chain (not the fast one) in a row-sharded group of n > 1: every plane a frame keeps - read at arbitrary uv by the next
+  // frame, or keeping its texel where a pixel is discarded - is double-buffered by group frame parity (gbuf[i][b], allocated and
+  // peer-mapped at attach time).  A frame writes the buffers of parity 1 - gprev (the chain's slots point at them); its kernels read
+  // last frame's rows on their owners (gpeer[i][gprev]) and carry the texels of discarded pixels from there.  Index i: gplane().
+  static constexpr int kGroupPlanes = 7;  // composed, tr[0], tr[1], dnA[0], dnA[1], dnB[0], dnB[1]
+  rfx_plane gbuf[kGroupPlanes][2]{};
+  PeerPV gpeer[kGroupPlanes][2]{};
+  int gprev = 1;
+  bool group_peer = false;  // attached to a group of n > 1: the peer / carry instantiations and the parity buffers are in use
   // optional per-pass event timing
   bool profiling = false;
   struct Span { cudaEvent_t a, b; int slot; };
   std::vector<Span> spans;
   std::vector<cudaEvent_t> event_pool;
 };
+
+// the chain's slot of group plane i (rfx_ssgi_chain::gbuf)
+static rfx_plane* gplane(rfx_ssgi_chain* ch, int i) {
+  rfx_plane* s[rfx_ssgi_chain::kGroupPlanes] = {&ch->composed, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1]};
+  return s[i];
+}
 
 static cudaEvent_t chain_event(rfx_ssgi_chain* ch) {
   if (!ch->event_pool.empty()) { cudaEvent_t e = ch->event_pool.back(); ch->event_pool.pop_back(); return e; }
@@ -915,6 +933,8 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   cudaStreamSynchronize(ctx->stream);
   if (ch->s_up) cudaStreamSynchronize(ch->s_up);
   if (ch->s_dn) cudaStreamSynchronize(ch->s_dn);
+  for (int i = 0; i < rfx_ssgi_chain::kGroupPlanes; i++)  // group buffers: the one in the chain's slot is freed with the slot below
+    for (rfx_plane& p : ch->gbuf[i]) if (p.ptr && p.ptr != gplane(ch, i)->ptr) rfx_plane_free(ctx, &p);
   rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->composed,
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
@@ -1107,9 +1127,12 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     const int halo = RFX_TRAA_TAIL_ROWS;
     rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
                                             (uint32_t)std::max(0, kr.r0 - halo), (uint32_t)std::min(H, kr.r1 + halo));
+    TemporalPeer tpeer{};  // in a row-sharded group of n > 1 the TRAA history is read on the rank that owns each row
+    tpeer.hist0 = tpeer.hist1 = ch->peer_traa[prev];
+    const bool peer = ch->group_peer;
     if (st == RFX_OK)
-      st = rfx_temporal_reproject_launch(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
-                                         (uint32_t)std::max(0, kr.r0 - 1), (uint32_t)std::min(H, kr.r1 + 1));
+      st = temporal_reproject(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
+                              std::max(0, kr.r0 - 1), std::min(H, kr.r1 + 1), peer ? &tpeer : nullptr);
     if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc[cur], &ch->traa_out, (uint32_t)kr.r0, (uint32_t)kr.r1);
     if (st != RFX_OK) return st;
   }
@@ -1300,12 +1323,17 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   const rfx_ssgi_chain_options& o = ch->opt;
   rfx_status st = RFX_OK;
   const bool dm_full = o.denoise_mode == RFX_DENOISE_FULL;
-  if (!dm_full && ranges) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for denoise_mode full only");
   if (ranges && ch->ssgi_out.height != o.height) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain: row-range rendering is implemented for resolution_scale 1 only");
   // launches: K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too), then the TRAA tail when it is on
   const int H = (int)o.height;
   // what SSGIPass samples as accumulatedTexture = denoiser.texture (Denoiser.js:67-78): the compose target, or the temporal pass's first texture
   rfx_plane* accumulated = o.denoise_mode == RFX_DENOISE_TEMPORAL ? &ch->tr[0] : &ch->composed;
+  // row-sharded group of n > 1 (rfx_group.inl): last frame's planes are gbuf[i][gp], read on the rank that owns each row; the peer
+  // and carry instantiations are chosen for every launch of such a frame, and never otherwise
+  const bool peer = ch->group_peer;
+  const int gp = ch->gprev;
+  const int acc_i = o.denoise_mode == RFX_DENOISE_TEMPORAL ? 1 : 0;  // gbuf index of `accumulated`
+  auto carry2 = [&](int i0, int i1) { PeerCarry c{}; c.p[0] = ch->gpeer[i0][gp]; c.p[1] = ch->gpeer[i1][gp]; return c; };
   auto on = [&](uint32_t k) { return k >= k_begin && k < k_end; };
   const cudaStream_t cs = stream ? (cudaStream_t)stream : ctx->stream;
   uint32_t k = 0;
@@ -1320,7 +1348,8 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     const Rows kr = launch_rows(ranges, k, (int)ch->ssgi_out.height);
     {
       SpanGuard g(ch, cs, 0);  // velocityTexture is a null sampler in the shipped wiring (SURVEY.md D4)
-      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, accumulated, &ch->ssgi_out, kr.r0, kr.r1, nullptr);
+      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, peer ? &ch->gbuf[acc_i][gp] : accumulated, &ch->ssgi_out, kr.r0, kr.r1,
+                      peer ? &ch->gpeer[acc_i][gp] : nullptr);
     }
     if (st != RFX_OK) return st;
   }
@@ -1351,10 +1380,20 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
       // without a denoise pass overrideAccumulatedTextures stays empty: BOTH accumulated textures are the one FramebufferTexture
       rfx_plane* h0 = dm_full ? &ch->dnB[0] : &ch->fb;
       rfx_plane* h1 = dm_full ? &ch->dnB[1] : &ch->fb;
-      st = temporal_reproject(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0], tc == 2 ? &ch->tr[1] : nullptr, kr.r0, kr.r1);
+      TemporalPeer tpeer{};
+      if (peer) {  // last frame's dnB, or last frame's tr[0] (of which `fb` is a byte copy on one GPU), on the owners; tr carried
+        const int i0 = dm_full ? 5 : 1, i1 = dm_full ? 6 : 1;
+        h0 = &ch->gbuf[i0][gp]; h1 = &ch->gbuf[tc == 2 ? i1 : i0][gp];
+        tpeer.hist0 = ch->gpeer[i0][gp]; tpeer.hist1 = ch->gpeer[tc == 2 ? i1 : i0][gp];
+        tpeer.carry = carry2(1, tc == 2 ? 2 : 1);
+      }
+      st = temporal_reproject(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0], tc == 2 ? &ch->tr[1] : nullptr, kr.r0, kr.r1,
+                              peer ? &tpeer : nullptr);
     }
     if (st != RFX_OK) return st;
-    if (!dm_full)  // renderer.copyFramebufferToTexture(tmpVec2, this.framebufferTexture) after the draw (:197-200)
+    // renderer.copyFramebufferToTexture(tmpVec2, this.framebufferTexture) after the draw (:197-200).  In a group the next frame reads
+    // this frame's tr[0] buffer on its owners instead.
+    if (!dm_full && !peer)
       CU(cudaMemcpy2DAsync(ch->fb.ptr, ch->fb.pitch, ch->tr[0].ptr, ch->tr[0].pitch, (size_t)ch->tr[0].width * 16, ch->tr[0].height, cudaMemcpyDeviceToDevice, cs));
     ch->keep_data = 1.0f;  // :195
     memcpy(ch->prev_world, f->cam.camera_matrix_world, 64); memcpy(ch->prev_view, f->cam.view_matrix, 64);
@@ -1380,8 +1419,9 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
       const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, i == 0 ? 2 : 3);
       // the G-buffer does not change within a frame: decode it once, reuse it afterwards
+      const PeerCarry pc = horizontal ? carry2(3, 4) : carry2(5, 6);  // dnA / dnB of last frame
       st = poisson_denoise(ctx, stream, &pp, f->depth, f->gbuffer, &inp[0], tc == 2 ? &inp[1] : nullptr, &outp[0], tc == 2 ? &outp[1] : nullptr, kr.r0, kr.r1,
-                           decoded);
+                           decoded, peer ? &pc : nullptr);
       decoded = true;
     }
     if (st != RFX_OK) return st;
@@ -1395,8 +1435,9 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     {
       const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, 4);
-      if (o.mode == RFX_MODE_SSGI) st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0], &gi[1], nullptr, &ch->composed, kr.r0, kr.r1);
-      else st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0], f->direct_light, &ch->composed, kr.r0, kr.r1);  // scene = the composer input buffer (Denoiser.js:100-102)
+      const PeerPV* cc = peer ? &ch->gpeer[0][gp] : nullptr;  // last frame's `composed`
+      if (o.mode == RFX_MODE_SSGI) st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0], &gi[1], nullptr, &ch->composed, kr.r0, kr.r1, cc);
+      else st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0], f->direct_light, &ch->composed, kr.r0, kr.r1, cc);  // scene = the composer input buffer (Denoiser.js:100-102)
     }
     if (st != RFX_OK) return st;
   }

@@ -37,6 +37,27 @@ RFX_D v4 peer_h4_linear(const PeerPV& p, v2 uv) {
   return bilin_blend4(b, ld(r0, b.x0), ld(r0, b.x1), ld(r1, b.x0), ld(r1, b.x1));
 }
 
+// LINEAR fetch of an RGBA32F plane whose rows live on their owners: tex_f4_linear's arithmetic, each row from peer_row_base
+RFX_D v4 peer_f4_linear(const PeerPV& p, v2 uv) {
+  const Bilin b = bilin_setup(uv, p.local.w, p.local.h);
+  const unsigned char* r0 = peer_row_base(p, b.y0) + (unsigned)b.y0 * (unsigned)p.local.pitch;
+  const unsigned char* r1 = peer_row_base(p, b.y1) + (unsigned)b.y1 * (unsigned)p.local.pitch;
+  auto ld = [](const unsigned char* r, int x) { return f4v(__ldg((const float4*)(r + (unsigned)x * 16u))); };
+  return bilin_blend4(b, ld(r0, b.x0), ld(r0, b.x1), ld(r1, b.x0), ld(r1, b.x1));
+}
+// Carry on discard (per-pass chain in a row-sharded group): a target is double-buffered by frame parity, and a pixel the shader
+// `discard`s (the reference's "target keeps its texel") copies last frame's texel of each target plane from the rank that owns the row.
+struct PeerCarry {
+  PeerPV p[2];  // last frame's planes of target 0 / 1 (p[1] unused with one plane)
+};
+template <int BYTES>
+RFX_D void carry_texel(const PeerPV& src, const OutV& dst, int x, int y) {
+  const size_t off = (size_t)y * (size_t)dst.pitch + (size_t)x * BYTES;  // src and dst: the same format and width, hence the same pitch
+  const unsigned char* s = peer_row_base(src, y) + off;
+  if (BYTES == 16) *(uint4*)(dst.p + off) = __ldg((const uint4*)s);
+  else *(uint2*)(dst.p + off) = __ldg((const uint2*)s);
+}
+
 struct CamD {  // device copy of rfx_camera
   M4 projection, projection_inverse, camera_matrix_world, view_matrix;
   float near_plane, far_plane;
@@ -75,8 +96,9 @@ struct PoissonArgs {
   PV nrd;                       // float4 (normal.xyz, roughness) from the decode prepass
   float tap_ox[8], tap_oy[8];   // POISSON[i] / resolution
 };
-cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s);       // exact-libm variant (any configuration)
-cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s);  // SFU variant (GBUFFER_TEXTURE configurations)
+// carry != nullptr: the carry-on-discard instantiation (out0 / out1 double-buffered in a row-sharded group, see PeerCarry)
+cudaError_t launch_poisson(const PoissonArgs& a, cudaStream_t s, const PeerCarry* carry = nullptr);       // exact-libm variant (any configuration)
+cudaError_t launch_poisson_fast(const PoissonArgs& a, cudaStream_t s, const PeerCarry* carry = nullptr);  // SFU variant (GBUFFER_TEXTURE configurations)
 cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_texture, int row0, int row1, int halo, cudaStream_t s);
 
 // ---- K4 / K5 -------------------------------------------------------------------------------
@@ -89,7 +111,7 @@ struct ComposeArgs {
   int gi_f32;  // diffuse / specular are RGBA32F NEAREST (denoiseMode "full_temporal": the temporal pass's targets)
   int fast;
 };
-cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s);
+cudaError_t launch_gi_compose(const ComposeArgs& a, cudaStream_t s, const PeerPV* carry = nullptr);  // carry: as launch_poisson's, `out`
 
 struct SsgiComposeArgs {
   PV depth, gi, scene;
@@ -139,6 +161,14 @@ struct TemporalArgs {
   int fast;  // SFU variants of log/exp/pow
 };
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
+// K2 of the per-pass chain in a row-sharded group: the history planes are read on the rank that owns each row (RGBA16F through
+// peer_h4_linear, RGBA32F through peer_f4_linear), and a discarded pixel carries last frame's texel of out0 / out1 (double-buffered)
+// from the owner.  a.hist0 / a.hist1 are ignored; history_linear and fast must be on.
+struct TemporalPeer {
+  PeerPV hist0, hist1;
+  PeerCarry carry;
+};
+cudaError_t launch_temporal_peer(const TemporalArgs& a, const TemporalPeer& p, cudaStream_t s);
 
 // TRAA frame tail of the fast chain (k_temporal.cu: ctraa_kernel): K5 -> K2 (TRAA form) -> K9 in one launch over rows [t.row0, t.row1).
 // `t` carries the TRAA K2 uniforms exactly as rfx_temporal_reproject_launch fills them (input_half = out_half = history_linear = 1,

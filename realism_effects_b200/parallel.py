@@ -47,6 +47,7 @@ class ShardPlan:
     bounds: tuple | None = None  # explicit band borders (world + 1 ascending rows, 0 .. height): one contiguous band per rank
     width: int | None = None     # frame width: portrait frames (H > W) stretch the Poisson taps' row reach by H / W
     traa: bool = False           # the TRAA tail runs as one more launch after K4 (rfx_ssgi_chain_enable_traa)
+    denoise_mode: int = 0        # 0 "full"; 1 "full_temporal" / 2 "temporal" run no Poisson pass, so their ranges are those of 0 passes
 
     K2_NEIGHBOURHOOD_ROWS = 2  # 5x5 clamp window (reproject.frag:57-59)
     K4_INPUT_ROWS = 1          # literal bilinear fetch of the LINEAR Poisson targets at the pixel centre
@@ -102,8 +103,14 @@ class ShardPlan:
     def _expand(self, rng, rows):
         return (max(0, rng[0] - rows), min(self.height, rng[1] + rows))
 
+    @property
+    def passes(self) -> int:
+        """Poisson passes the ranges are planned for: n_poisson_passes in denoiseMode "full", else none (Denoiser.js:47-52).  The native
+        chain maps a full_temporal / temporal frame's K1, K2, K4 (and tail) launches onto these ranges (rfx_ssgi_chain_render_sharded)."""
+        return self.n_poisson_passes if self.denoise_mode == 0 else 0
+
     def ranges_for(self, own) -> list:
-        n = self.n_poisson_passes
+        n = self.passes
         k4 = self._expand(own, self.TRAA_TAIL_ROWS) if self.traa else own
         k3 = [None] * n
         nxt = k4
@@ -128,7 +135,7 @@ class ShardPlan:
 
     @property
     def n_launches(self) -> int:
-        return 3 + self.n_poisson_passes + (1 if self.traa else 0)
+        return 3 + self.passes + (1 if self.traa else 0)
 
     def super_block(self, j: int):
         """rows of super-block j: N consecutive blocks, one per rank, in rank order (an in-place all-gather unit)"""
@@ -336,6 +343,10 @@ class ShardedSsgiChain:
         (local_input_rows) are sized for the chain without it."""
         if self.chain.traa is not None:
             raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path does not render the TRAA tail")
+        o = self.chain.opt
+        if o.mode != self._abi.MODE_SSGI or o.denoise_mode != 0:
+            raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path renders the fast SSGI chain only "
+                                     "(mode SSGI, denoiseMode \"full\"): its upload rows are planned for that chain")
         if self._host is None:
             self._host_init()
         h = self._host
@@ -406,7 +417,7 @@ class ShardedSsgiChain:
 
 class InProcessGroup:
     """`world` members of a row-sharded group inside ONE process (rfx_group_create_inprocess / rfx_group_attach_chains_inprocess): every member
-    owns a fast SSGI chain and a band; the members read each other's history planes through plain device pointers.  With one context this
+    owns a chain (any options a group takes: fast_math on, resolution_scale 1) and a band; the members read each other's history planes through plain device pointers.  With one context this
     renders the bands one after the other on one GPU — the N-band logic (halo recomputation, owner lookup of history rows, carried texels,
     moving borders) without N GPUs; with one context per device it is a single-process multi-GPU host."""
 
@@ -445,14 +456,16 @@ class InProcessGroup:
         for c, g in zip(self.ctxs, self.groups):
             c._chk(self.lib.rfx_group_set_bounds(g, b))
 
-    def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool):
-        """one frame: every member renders its band; all of them finish before the next frame starts (the host is the barrier)"""
+    def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, wait: bool = True):
+        """one frame: every member renders its band; all of them finish before the next frame starts (the host is the barrier).
+        wait=False skips the host wait: only for members that share one context, whose stream orders the members and the frames."""
         self._last_bounds = self.bounds
         for c, ch in zip(self.ctxs, self.chains):
             f = ch._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
             c._chk(self.lib.rfx_ssgi_chain_render_sharded(ch.h, None, self._C.byref(f)))
-        for c in set(self.ctxs):
-            c.sync()
+        if wait or len(set(self.ctxs)) > 1:
+            for c in set(self.ctxs):
+                c.sync()
 
     def download(self, which: int = 0):
         """output `which` of the last frame, assembled from the members' bands"""
