@@ -563,16 +563,30 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_
   else cpoisson_body<false, COMPOSE, false, false>(a, x, y, nc, fwn);
 }
 
+static constexpr size_t kTmaSmemCap = 100 * 1024;  // dynamic shared memory cpoisson_tma_kernel may take
+static size_t cpoisson_tma_smem(int box_w, int box_h) {  // the `in` tile, then the `nrdz` tile at the next 128-byte boundary
+  const size_t tile_bytes = (size_t)box_w * box_h * 16;
+  return ((tile_bytes + 127) & ~(size_t)127) + tile_bytes;
+}
+
+bool cpoisson_tma_fits(int box_w, int box_h) {
+  return box_w * 4 <= 256 && box_h <= 256 && cpoisson_tma_smem(box_w, box_h) <= kTmaSmemCap;  // box rows count 4-byte elements, 4 per texel
+}
+
 cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s) {
+  if (!cpoisson_tma_fits(t.box_w, t.box_h)) return cudaErrorInvalidValue;
   dim3 grid((t.a.W + kTileW - 1) / kTileW, row_tiles(t.a.row0, t.a.row1));
-  const size_t tile_bytes = (size_t)t.box_w * t.box_h * 16, smem = ((tile_bytes + 127) & ~(size_t)127) + tile_bytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(cpoisson_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    cudaFuncSetAttribute(cpoisson_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
-    attr_set = true;
+  const size_t smem = cpoisson_tma_smem(t.box_w, t.box_h);
+  // the shared-memory limit is an attribute of the kernel on the CURRENT device: raise it once on every device that launches it
+  static bool attr_set[64] = {};
+  int dev = 0;
+  const cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev >= 64 || !attr_set[dev]) {
+    cudaFuncSetAttribute(cpoisson_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemCap);
+    cudaFuncSetAttribute(cpoisson_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemCap);
+    if (dev < 64) attr_set[dev] = true;
   }
-  if (smem > 100 * 1024) return cudaErrorInvalidValue;
   if (t.a.compose) cpoisson_tma_kernel<true><<<grid, kThreads, smem, s>>>(t); else cpoisson_tma_kernel<false><<<grid, kThreads, smem, s>>>(t);
   return cudaGetLastError();
 }

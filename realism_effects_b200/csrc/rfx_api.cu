@@ -1141,7 +1141,7 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   return RFX_OK;
 }
 
-// 2-D TMA descriptor over a plane of 16-byte texels, addressed as rows of 4-byte elements (box dims are limited to 256 elements)
+// 2-D TMA descriptor over a plane of 16-byte texels, addressed as rows of 4-byte elements (the box must pass cpoisson_tma_fits)
 static bool encode_texel_map(CUtensorMap* map, const void* base, int W, int H, size_t pitch, int box_w, int box_h) {
   typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1152,7 +1152,6 @@ static bool encode_texel_map(CUtensorMap* map, const void* base, int W, int H, s
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess || !p) return false;
     fn = (EncodeFn)p;
   }
-  if (box_w * 4 > 256 || box_h > 256) return false;
   const cuuint64_t dims[2] = {(cuuint64_t)W * 4, (cuuint64_t)H};
   const cuuint64_t strides[1] = {(cuuint64_t)pitch};
   const cuuint32_t box[2] = {(cuuint32_t)box_w * 4, (cuuint32_t)box_h};
@@ -1280,11 +1279,12 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
       a.cam = cam;
     }
     SpanGuard g(ch, cs, i == 0 ? 2 : 3);
-    if (ctx->k3_tma && i > 0) {  // experiment: TMA-staged tap tiles for the LINEAR passes
+    const int box_w = (kTileW + 2 * a.reach_x) | 1, box_h = kTileH + 2 * a.reach_y;  // odd row pitch in texels: consecutive tile rows start 4 banks apart
+    if (ctx->k3_tma && i > 0 && cpoisson_tma_fits(box_w, box_h)) {  // TMA-staged tap tiles for the LINEAR passes, where the tiles fit
       CPoissonTmaArgs t{};
       t.a = a;
-      t.box_w = (kTileW + 2 * a.reach_x) | 1;  // odd row pitch in texels: consecutive tile rows start 4 banks apart
-      t.box_h = kTileH + 2 * a.reach_y;
+      t.box_w = box_w;
+      t.box_h = box_h;
       if (encode_texel_map(&t.map_in, a.in.p, W, H, (size_t)a.in.pitch, t.box_w, t.box_h) && encode_texel_map(&t.map_nrdz, a.nrdz.p, W, H, (size_t)a.nrdz.pitch, t.box_w, t.box_h)) {
         LAUNCHED(launch_cpoisson_tma(t, cs));
         continue;

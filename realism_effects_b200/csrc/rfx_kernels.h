@@ -351,7 +351,10 @@ struct CPoissonTmaArgs {  // passes >= 1 with TMA-staged tiles (experiment, RFX_
   CUtensorMap map_in, map_nrdz;  // 2-D maps over the 16-byte texel planes as rows of 4-byte elements; box = box_w*4 x box_h
   int box_w, box_h;              // texels: 16 + 2 * reach_x, 16 + 2 * reach_y
 };
-cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s);
+// Whether a box_w x box_h texel tile can be staged through TMA: each box dimension at most 256 elements, and both tiles within the
+// kernel's dynamic shared memory.  When it cannot, the pass runs launch_cpoisson (same bytes out).
+bool cpoisson_tma_fits(int box_w, int box_h);
+cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s);  // cudaErrorInvalidValue unless cpoisson_tma_fits
 
 struct CComposeArgs {   // stand-alone K4 over dn (denoiseIterations == 0)
   PV nrdz, gb, dn;
