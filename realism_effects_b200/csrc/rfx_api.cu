@@ -5,6 +5,7 @@
 // SSGI chain (the mirror of SSGIEffect.update / Denoiser.render frame logic).  No torch types, no
 // exceptions across the boundary, no CPU fallback: every compute entry point launches a kernel.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -809,18 +810,29 @@ struct IPlane {  // chain-internal plane (formats of k_chain.cu): raw pitched al
   void* p = nullptr;
   size_t pitch = 0;
 };
+// A plane the chain may keep from one frame to the next (hist_planes lists the ones its configuration keeps).  Such a plane is
+// double-buffered by a frame parity so that, in a row-sharded group, no rank overwrites rows a peer may still be reading; view[b]
+// reads buffer b, each row on the rank that owns it.  Alone, view[b] is the n = 1 view of the local buffer.
+struct HistPlane {
+  rfx_plane buf[2]{};
+  PeerPV view[2]{};
+};
 struct rfx_ssgi_chain {
   rfx_ctx* ctx;
   rfx_ssgi_chain_options opt;
-  rfx_plane ssgi_out{}, tr[2]{}, dnA[2]{}, dnB[2]{}, composed{};
+  rfx_plane ssgi_out{};
+  // per-pass chain: single-buffered alone (buffer 0, rendered in place); buffer 1 of each plane the chain keeps is added by a group of
+  // n > 1 (group_alloc_history).  The fast chain uses buffer 0 of tr[] and dnB[] for the reference-format views of chain_output,
+  // and `composed` double-buffered by frame parity (composed.buf[cur] is output 0).
+  HistPlane composed, tr[2], dnA[2], dnB[2];
   rfx_plane fb{};  // denoise_mode != full: the FramebufferTexture copy of the temporal target's attachment 0 (TemporalReprojectPass.js:134-152,197-200)
-  // fast chain (fast_math on at creation, mode SSGI): interleaved internal planes; history planes are double-buffered by frame
-  // parity so that, in a row-sharded group, no rank overwrites rows a peer may still be reading (see rfx_group_*)
+  // fast chain (fast_math on at creation, mode SSGI): interleaved internal planes
   bool fastpath = false;
-  IPlane nrdz, tr32, dnA16[2], dnB16[2];  // dnA16[1] is used by row-sharded groups only (the A target double-buffered like B, see chain_render_fast)
-  rfx_plane composed2[2]{};  // fast chain: composed of frame parity 0 / 1 (composed2[cur] is output 0)
+  IPlane nrdz, tr32;
+  // the Poisson targets A / B of the fast chain, both planes of a target interleaved in one 16-byte texel (typed RGBA32F for their
+  // size).  fdnA.buf[1] is used by row-sharded groups only (the A target double-buffered like B, see chain_render_fast).
+  HistPlane fdnA, fdnB;
   struct rfx_group* group = nullptr;  // row-sharded group this chain is attached to (rfx_group_attach_chain)
-  PeerPV peer_composed[2]{}, peer_dn[2]{}, peer_dnA[2]{};
   uint64_t frame_idx = 0;    // frames completed (advances with the frame's last launch)
   bool views_valid = false;  // tr[]/dnB[] hold the split views of the current frame's interleaved planes
   // host-buffer entry points: two staging sets so frame i+1 uploads while frame i renders; H2D, kernels and D2H each get
@@ -830,7 +842,7 @@ struct rfx_ssgi_chain {
   cudaStream_t s_up = nullptr, s_dn = nullptr;
   cudaEvent_t ev_up[2]{}, ev_rendered[2]{}, ev_dn[2]{};
   uint64_t host_submitted = 0;
-  int dn_buf[2] = {-1, -1};  // fast chain: which composed2[] buffer the D2H of staging set 0 / 1 reads
+  int dn_buf[2] = {-1, -1};  // fast chain: which composed buffer the D2H of staging set 0 / 1 reads
   // cross-frame state (TemporalReprojectPass.js:203-213)
   bool have_prev = false;
   float prev_view[16], prev_world[16], prev_proj[16], prev_proj_inv[16], prev_pos[3];
@@ -840,21 +852,15 @@ struct rfx_ssgi_chain {
   // TRAA frame tail (rfx_ssgi_chain_enable_traa): one more launch after K4
   bool traa_on = false;
   rfx_traa_tail_options traa{};
-  rfx_plane traa_acc[2]{}, traa_out{};  // accumulated plane by tail parity (acc[prev] is the history), K9 output
+  HistPlane traa_acc;                   // accumulated plane by tail parity (buf[prev] is the history)
+  rfx_plane traa_out{};                 // K9 output
   rfx_plane traa_k5{};                  // K5 plane of the per-pass tail (chains other than the fast one)
-  uint64_t traa_frames = 0;             // tails rendered; acc[traa_frames & 1] is written next
+  uint64_t traa_frames = 0;             // tails rendered; traa_acc.buf[traa_frames & 1] is written next
   float traa_keep = 0.0f;               // keepData of the TRAA pass
   rfx_temporal_params traa_tp{};        // the frame's camera and the previous-frame matrices its K2 used
-  PeerPV peer_traa[2]{};
-  // per-pass chain (not the fast one) in a row-sharded group of n > 1: every plane a frame keeps - read at arbitrary uv by the next
-  // frame, or keeping its texel where a pixel is discarded - is double-buffered by group frame parity (gbuf[i][b], allocated and
-  // peer-mapped at attach time).  A frame writes the buffers of parity 1 - gprev (the chain's slots point at them); its kernels read
-  // last frame's rows on their owners (gpeer[i][gprev]) and carry the texels of discarded pixels from there.  Index i: gplane().
-  static constexpr int kGroupPlanes = 7;  // composed, tr[0], tr[1], dnA[0], dnA[1], dnB[0], dnB[1]
-  rfx_plane gbuf[kGroupPlanes][2]{};
-  PeerPV gpeer[kGroupPlanes][2]{};
-  int gprev = 1;
-  bool group_peer = false;  // attached to a group of n > 1: the peer / carry instantiations and the parity buffers are in use
+  // per-pass chain (not the fast one) attached to a group of n > 1: the peer / carry instantiations and both buffers of every plane
+  // it keeps are in use.  A frame's kernels read last frame's rows on their owners and carry the texels of discarded pixels from there.
+  bool group_peer = false;
   // optional per-pass event timing
   bool profiling = false;
   struct Span { cudaEvent_t a, b; int slot; };
@@ -862,11 +868,25 @@ struct rfx_ssgi_chain {
   std::vector<cudaEvent_t> event_pool;
 };
 
-// the chain's slot of group plane i (rfx_ssgi_chain::gbuf)
-static rfx_plane* gplane(rfx_ssgi_chain* ch, int i) {
-  rfx_plane* s[rfx_ssgi_chain::kGroupPlanes] = {&ch->composed, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1]};
-  return s[i];
+static PV rpv(const rfx_plane& p) { return PV{(const unsigned char*)p.ptr, (int)p.width, (int)p.height, (long long)p.pitch}; }
+static OutV rov(const rfx_plane& p) { return OutV{(unsigned char*)p.ptr, (long long)p.pitch}; }
+// view[b] of `h` in a group of n ranks; base[r]: rank r's buffer b.  n = 1 with this rank's buffer: the view a chain reads alone.
+static void set_view(HistPlane& h, int b, const void* const* base, int n) {
+  PeerPV& v = h.view[b];
+  v = PeerPV{};
+  v.local = rpv(h.buf[b]);
+  v.n = n;
+  for (int r = 0; r < n; r++) v.base[r] = (const unsigned char*)base[r];
+  v.own0 = 0; v.own1 = v.local.h;
 }
+static void local_views(HistPlane& h) {
+  for (int b = 0; b < 2; b++) set_view(h, b, &h.buf[b].ptr, 1);
+}
+static std::array<HistPlane*, 10> every_hist_plane(rfx_ssgi_chain* ch) {  // whether the chain's configuration keeps it or not
+  return {&ch->composed, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->fdnA, &ch->fdnB, &ch->traa_acc};
+}
+// per-pass chain: the buffer of every plane it keeps that holds the latest frame (rfx_group.inl)
+static int pass_latest(const rfx_ssgi_chain* ch);
 
 static cudaEvent_t chain_event(rfx_ssgi_chain* ch) {
   if (!ch->event_pool.empty()) { cudaEvent_t e = ch->event_pool.back(); ch->event_pool.pop_back(); return e; }
@@ -916,13 +936,15 @@ rfx_status rfx_ssgi_chain_create(rfx_ctx* ctx, const rfx_ssgi_chain_options* opt
   if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, sw, sh, &ch->ssgi_out);
   if (opt->denoise_mode != RFX_DENOISE_FULL) alloc(RFX_FMT_RGBA32F, &ch->fb);
   if (ch->fastpath) {
-    ialloc(16, &ch->nrdz); ialloc(32, &ch->tr32); ialloc(16, &ch->dnA16[0]); ialloc(16, &ch->dnA16[1]); ialloc(16, &ch->dnB16[0]); ialloc(16, &ch->dnB16[1]);
-    alloc(RFX_FMT_RGBA32F, &ch->composed2[0]); alloc(RFX_FMT_RGBA32F, &ch->composed2[1]);
+    ialloc(16, &ch->nrdz); ialloc(32, &ch->tr32);
+    for (HistPlane* h : {&ch->fdnA, &ch->fdnB, &ch->composed})
+      for (rfx_plane& b : h->buf) alloc(RFX_FMT_RGBA32F, &b);
   } else {
-    for (int i = 0; i < 2; i++) { alloc(RFX_FMT_RGBA32F, &ch->tr[i]); alloc(RFX_FMT_RGBA16F, &ch->dnA[i]); alloc(RFX_FMT_RGBA16F, &ch->dnB[i]); }
-    alloc(RFX_FMT_RGBA32F, &ch->composed);
+    for (int i = 0; i < 2; i++) { alloc(RFX_FMT_RGBA32F, &ch->tr[i].buf[0]); alloc(RFX_FMT_RGBA16F, &ch->dnA[i].buf[0]); alloc(RFX_FMT_RGBA16F, &ch->dnB[i].buf[0]); }
+    alloc(RFX_FMT_RGBA32F, &ch->composed.buf[0]);
   }
   if (st != RFX_OK) { rfx_ssgi_chain_destroy(ch); return st; }
+  for (HistPlane* h : every_hist_plane(ch)) local_views(*h);
   *out = ch;
   return RFX_OK;
 }
@@ -933,13 +955,12 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   cudaStreamSynchronize(ctx->stream);
   if (ch->s_up) cudaStreamSynchronize(ch->s_up);
   if (ch->s_dn) cudaStreamSynchronize(ch->s_dn);
-  for (int i = 0; i < rfx_ssgi_chain::kGroupPlanes; i++)  // group buffers: the one in the chain's slot is freed with the slot below
-    for (rfx_plane& p : ch->gbuf[i]) if (p.ptr && p.ptr != gplane(ch, i)->ptr) rfx_plane_free(ctx, &p);
-  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->composed,
+  for (HistPlane* h : every_hist_plane(ch))
+    for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ctx, &p);
+  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->traa_out, &ch->traa_k5,
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
-  for (rfx_plane* p : {&ch->composed2[0], &ch->composed2[1], &ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
-  for (IPlane* p : {&ch->nrdz, &ch->tr32, &ch->dnA16[0], &ch->dnA16[1], &ch->dnB16[0], &ch->dnB16[1]}) if (p->p) cudaFree(p->p);
+  for (IPlane* p : {&ch->nrdz, &ch->tr32}) if (p->p) cudaFree(p->p);
   for (int i = 0; i < 2; i++) for (cudaEvent_t e : {ch->ev_up[i], ch->ev_rendered[i], ch->ev_dn[i]}) if (e) cudaEventDestroy(e);
   if (ch->s_up) cudaStreamDestroy(ch->s_up);
   if (ch->s_dn) cudaStreamDestroy(ch->s_dn);
@@ -995,19 +1016,20 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_op
   if (ch->group) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
   if (!opt) {
     CU(cudaStreamSynchronize(ctx->stream));
-    for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
+    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
     ch->traa_on = false;
     return RFX_OK;
   }
   if (!ch->traa_out.ptr) {
     rfx_status st = RFX_OK;
-    for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out})
+    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out})
       if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
     if (st == RFX_OK && !ch->fastpath) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
     if (st != RFX_OK) {
-      for (rfx_plane* p : {&ch->traa_acc[0], &ch->traa_acc[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
+      for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
       return st;
     }
+    local_views(ch->traa_acc);
   }
   ch->traa = *opt;
   ch->traa_on = true;
@@ -1021,40 +1043,42 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* o
   if (which < 0 || which > 7) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..7");
   if (which >= 6) {
     if (!ch->traa_on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
-    *out = which == 6 ? ch->traa_out : ch->traa_acc[(ch->traa_frames + 1) & 1];
+    *out = which == 6 ? ch->traa_out : ch->traa_acc.buf[(ch->traa_frames + 1) & 1];
     return RFX_OK;
   }
   if (ch->fastpath) {
     const int last = (int)((ch->frame_idx + 1) & 1);  // parity of the most recently completed frame
-    if (which == 0) { *out = ch->composed2[last]; return RFX_OK; }
+    if (which == 0) { *out = ch->composed.buf[last]; return RFX_OK; }
     if (which == 1) { *out = ch->ssgi_out; return RFX_OK; }
     // views of the interleaved planes in the reference's formats, refreshed on the context stream
-    if (!ch->tr[0].ptr) {
+    rfx_plane *tr0 = &ch->tr[0].buf[0], *tr1 = &ch->tr[1].buf[0], *dn0 = &ch->dnB[0].buf[0], *dn1 = &ch->dnB[1].buf[0];
+    if (!tr0->ptr) {
       rfx_status st = RFX_OK;
       for (int i = 0; i < 2 && st == RFX_OK; i++) {
-        st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->tr[i]);
-        if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->dnB[i]);
+        st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->tr[i].buf[0]);
+        if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->dnB[i].buf[0]);
       }
       if (st != RFX_OK) return st;
     }
     if (!ch->views_valid) {
       const int W = (int)ch->opt.width, H = (int)ch->opt.height;
-      LAUNCHED(launch_split_tr(PV{(const unsigned char*)ch->tr32.p, W, H, (long long)ch->tr32.pitch}, OutV{(unsigned char*)ch->tr[0].ptr, (long long)ch->tr[0].pitch},
-                               OutV{(unsigned char*)ch->tr[1].ptr, (long long)ch->tr[1].pitch}, W, H, ctx->stream));
-      LAUNCHED(launch_split_dn(PV{(const unsigned char*)ch->dnB16[last].p, W, H, (long long)ch->dnB16[last].pitch}, OutV{(unsigned char*)ch->dnB[0].ptr, (long long)ch->dnB[0].pitch},
-                               OutV{(unsigned char*)ch->dnB[1].ptr, (long long)ch->dnB[1].pitch}, W, H, ctx->stream));
+      LAUNCHED(launch_split_tr(PV{(const unsigned char*)ch->tr32.p, W, H, (long long)ch->tr32.pitch}, rov(*tr0), rov(*tr1), W, H, ctx->stream));
+      LAUNCHED(launch_split_dn(rpv(ch->fdnB.buf[last]), rov(*dn0), rov(*dn1), W, H, ctx->stream));
       ch->views_valid = true;
     }
-    *out = which == 2 ? ch->tr[0] : which == 3 ? ch->tr[1] : which == 4 ? ch->dnB[0] : ch->dnB[1];
+    *out = which == 2 ? *tr0 : which == 3 ? *tr1 : which == 4 ? *dn0 : *dn1;
     return RFX_OK;
   }
+  // a plane the chain keeps holds the latest frame in buffer pass_latest; the others are single-buffered
+  const int b = pass_latest(ch);
+  auto latest = [&](const HistPlane& h) { return h.buf[h.buf[1].ptr ? b : 0]; };
   switch (which) {
-    case 0: *out = ch->opt.denoise_mode == RFX_DENOISE_TEMPORAL ? ch->tr[0] : ch->composed; break;  // denoiser.texture (Denoiser.js:67-78)
+    case 0: *out = latest(ch->opt.denoise_mode == RFX_DENOISE_TEMPORAL ? ch->tr[0] : ch->composed); break;  // denoiser.texture (Denoiser.js:67-78)
     case 1: *out = ch->ssgi_out; break;
-    case 2: *out = ch->tr[0]; break;
-    case 3: *out = ch->tr[1]; break;
-    case 4: *out = ch->dnB[0]; break;
-    default: *out = ch->dnB[1]; break;
+    case 2: *out = latest(ch->tr[0]); break;
+    case 3: *out = latest(ch->tr[1]); break;
+    case 4: *out = latest(ch->dnB[0]); break;
+    default: *out = latest(ch->dnB[1]); break;
   }
   return RFX_OK;
 }
@@ -1070,22 +1094,42 @@ static Rows launch_rows(const uint32_t* ranges, uint32_t k, int H) { return rang
 // ------------------------------------------------------------------------------------------
 static PV ipv(const IPlane& p, int w, int h) { return PV{(const unsigned char*)p.p, w, h, (long long)p.pitch}; }
 static OutV iov(const IPlane& p) { return OutV{(unsigned char*)p.p, (long long)p.pitch}; }
-static PV rpv(const rfx_plane& p) { return PV{(const unsigned char*)p.ptr, (int)p.width, (int)p.height, (long long)p.pitch}; }
-static void peer_single(PeerPV& pp, PV local) {
-  pp = PeerPV{};
-  pp.local = local;
-  pp.n = 1;
-  pp.own0 = 0; pp.own1 = local.h;
+
+// K1's uniforms of this frame (SSGIPass.render, src/ssgi/pass/SSGIPass.js:68-95)
+static rfx_ssgi_params trace_params(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
+  const rfx_ctx* ctx = ch->ctx;
+  const rfx_ssgi_chain_options& o = ch->opt;
+  rfx_ssgi_params sp{};
+  sp.cam = f->cam;
+  sp.ray_distance = o.distance; sp.thickness = o.thickness; sp.env_blur = o.env_blur;
+  sp.max_env_map_mip_level = ctx->env_set ? (float)((int)std::floor(std::log2((double)std::max(ctx->env.size_x, ctx->env.size_y))) + 1) : 0.0f;  // Utils.js:30-34
+  sp.steps = o.steps; sp.refine_steps = o.refine_steps; sp.mode = o.mode; sp.flags = o.ssgi_flags;
+  sp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_trace);
+  return sp;
 }
 
-// K2's camera state of this frame, kept for the TRAA tail: the current (un-jittered) camera and the previous-frame matrices before
-// K2 replaces them (the TRAA TemporalReprojectPass tracks the same camera, so its previous frame is the chain's)
-static void keep_traa_camera(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
+// Before K2: the first frame's previous camera is the current one (the constructor clones the current camera matrices,
+// TemporalReprojectPass.js:94-97).  The current (un-jittered) camera and the previous-frame matrices are also kept for the TRAA tail
+// (its TemporalReprojectPass tracks the same camera, so its previous frame is the chain's).
+static void prev_camera_init(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
+  if (!ch->have_prev) {
+    memcpy(ch->prev_view, f->cam.view_matrix, 64); memcpy(ch->prev_world, f->cam.camera_matrix_world, 64);
+    memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
+    memcpy(ch->prev_pos, f->camera_pos, 12);
+    ch->have_prev = true;
+  }
   rfx_temporal_params& tp = ch->traa_tp;
   tp.cam = f->cam;
   memcpy(tp.prev_view_matrix, ch->prev_view, 64); memcpy(tp.prev_camera_matrix_world, ch->prev_world, 64);
   memcpy(tp.prev_projection, ch->prev_proj, 64); memcpy(tp.prev_projection_inverse, ch->prev_proj_inv, 64);
   memcpy(tp.camera_pos, f->camera_pos, 12); memcpy(tp.prev_camera_pos, ch->prev_pos, 12);
+}
+// After K2 (TemporalReprojectPass.js:195,203-213): keep the history from now on, and this frame's camera is the next one's previous
+static void prev_camera_roll(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
+  ch->keep_data = 1.0f;
+  memcpy(ch->prev_world, f->cam.camera_matrix_world, 64); memcpy(ch->prev_view, f->cam.view_matrix, 64);
+  memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
+  memcpy(ch->prev_pos, f->camera_pos, 12);
 }
 
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
@@ -1119,21 +1163,20 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     c.use_fog = q.use_fog; c.fog_exp2 = q.fog_exp2; c.perspective = q.perspective; c.is_debug = q.is_debug;
     memcpy(c.fog_color, q.fog_color, 12);
     c.fog_near = q.fog_near; c.fog_far = q.fog_far; c.fog_density = q.fog_density; c.camera_near = q.camera_near; c.camera_far = q.camera_far;
-    if (ch->group) a.hist = ch->peer_traa[prev]; else peer_single(a.hist, rpv(ch->traa_acc[prev]));
-    a.acc = OutV{(unsigned char*)ch->traa_acc[cur].ptr, (long long)ch->traa_acc[cur].pitch};
-    a.out = OutV{(unsigned char*)ch->traa_out.ptr, (long long)ch->traa_out.pitch};
+    a.hist = ch->traa_acc.view[prev];
+    a.acc = rov(ch->traa_acc.buf[cur]);
+    a.out = rov(ch->traa_out);
     LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
   } else {
     const int halo = RFX_TRAA_TAIL_ROWS;
     rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
                                             (uint32_t)std::max(0, kr.r0 - halo), (uint32_t)std::min(H, kr.r1 + halo));
     TemporalPeer tpeer{};  // in a row-sharded group of n > 1 the TRAA history is read on the rank that owns each row
-    tpeer.hist0 = tpeer.hist1 = ch->peer_traa[prev];
-    const bool peer = ch->group_peer;
+    tpeer.hist0 = tpeer.hist1 = ch->traa_acc.view[prev];
     if (st == RFX_OK)
-      st = temporal_reproject(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc[prev], nullptr, &ch->traa_acc[cur], nullptr,
-                              std::max(0, kr.r0 - 1), std::min(H, kr.r1 + 1), peer ? &tpeer : nullptr);
-    if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc[cur], &ch->traa_out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+      st = temporal_reproject(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc.buf[prev], nullptr, &ch->traa_acc.buf[cur], nullptr,
+                              std::max(0, kr.r0 - 1), std::min(H, kr.r1 + 1), ch->group_peer ? &tpeer : nullptr);
+    if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc.buf[cur], &ch->traa_out, (uint32_t)kr.r0, (uint32_t)kr.r1);
     if (st != RFX_OK) return st;
   }
   ch->traa_keep = 1.0f;
@@ -1178,17 +1221,12 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
   ch->views_valid = false;
   // ---- K1
   if (on(k)) {
-    rfx_ssgi_params sp{};
-    sp.cam = f->cam;
-    sp.ray_distance = o.distance; sp.thickness = o.thickness; sp.env_blur = o.env_blur;
-    sp.max_env_map_mip_level = ctx->env_set ? (float)((int)std::floor(std::log2((double)std::max(ctx->env.size_x, ctx->env.size_y))) + 1) : 0.0f;
-    sp.steps = o.steps; sp.refine_steps = o.refine_steps; sp.mode = o.mode; sp.flags = o.ssgi_flags;
-    sp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_trace);
+    const rfx_ssgi_params sp = trace_params(ch, f);
     const Rows kr = launch_rows(ranges, k, H);
     {
       SpanGuard g(ch, cs, 0);
-      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, &ch->composed2[prev], &ch->ssgi_out, kr.r0, kr.r1,
-                      ch->group ? &ch->peer_composed[prev] : nullptr);
+      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, &ch->composed.buf[prev], &ch->ssgi_out, kr.r0, kr.r1,
+                      &ch->composed.view[prev]);
     }
     if (st != RFX_OK) return st;
   }
@@ -1197,19 +1235,13 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
   if (on(k)) {
     CTemporalArgs a{};
     a.input = rpv(ch->ssgi_out); a.velocity = vel;
-    if (ch->group) a.hist = ch->peer_dn[prev]; else peer_single(a.hist, ipv(ch->dnB16[prev], W, H));
+    a.hist = ch->fdnB.view[prev];
     a.out = iov(ch->tr32);
     a.W = W; a.H = H;
     const Rows kr = launch_rows(ranges, k, H);
     a.row0 = kr.r0; a.row1 = kr.r1;
     a.cam = cam;
-    if (!ch->have_prev) {
-      memcpy(ch->prev_view, f->cam.view_matrix, 64); memcpy(ch->prev_world, f->cam.camera_matrix_world, 64);
-      memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
-      memcpy(ch->prev_pos, f->camera_pos, 12);
-      ch->have_prev = true;
-    }
-    keep_traa_camera(ch, f);
+    prev_camera_init(ch, f);
     memcpy(a.prev_world.m, ch->prev_world, 64); memcpy(a.prev_proj_inv.m, ch->prev_proj_inv, 64);
     matmul(ch->prev_proj, ch->prev_view, a.prev_proj_view.m);
     memcpy(a.camera_pos, f->camera_pos, 12);
@@ -1220,10 +1252,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
       SpanGuard g(ch, cs, 1);
       LAUNCHED(launch_ctemporal(a, cs));
     }
-    ch->keep_data = 1.0f;
-    memcpy(ch->prev_world, f->cam.camera_matrix_world, 64); memcpy(ch->prev_view, f->cam.view_matrix, 64);
-    memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
-    memcpy(ch->prev_pos, f->camera_pos, 12);
+    prev_camera_roll(ch, f);
   }
   k++;
   // ---- K3 (+ fused K4)
@@ -1252,10 +1281,10 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     // rank's A rows outside its band hold the result of whichever even pass last covered them (the ranges shrink pass by pass), not the
     // last one's, so A is double-buffered by frame parity like B and the discarded texel is carried from the rank that OWNS the row.
     const int acur = ch->group ? cur : 0;
-    a.in = i == 0 ? ipv(ch->tr32, W, H) : ipv(horizontal ? ch->dnB16[cur] : ch->dnA16[acur], W, H);
-    a.out = iov(horizontal ? ch->dnA16[acur] : ch->dnB16[cur]);
-    if (!horizontal) { if (ch->group) a.carry = ch->peer_dn[prev]; else peer_single(a.carry, ipv(ch->dnB16[prev], W, H)); }
-    else if (ch->group) a.carry = ch->peer_dnA[prev];
+    a.in = i == 0 ? ipv(ch->tr32, W, H) : rpv(horizontal ? ch->fdnB.buf[cur] : ch->fdnA.buf[acur]);
+    a.out = rov(horizontal ? ch->fdnA.buf[acur] : ch->fdnB.buf[cur]);
+    if (!horizontal) a.carry = ch->fdnB.view[prev];
+    else if (ch->group) a.carry = ch->fdnA.view[prev];
     a.W = W; a.H = H;
     a.radius = o.radius; a.phi = o.phi; a.luma_phi = o.luma_phi; a.depth_phi = o.depth_phi; a.normal_phi = o.normal_phi;
     a.roughness_phi = o.roughness_phi; a.specular_phi = o.specular_phi;
@@ -1274,8 +1303,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
       const Rows cr = launch_rows(ranges, k_compose, H);
       a.crow0 = cr.r0; a.crow1 = cr.r1;
       a.gb = gb;
-      a.composed = OutV{(unsigned char*)ch->composed2[cur].ptr, (long long)ch->composed2[cur].pitch};
-      if (ch->group) a.composed_carry = ch->peer_composed[prev]; else peer_single(a.composed_carry, rpv(ch->composed2[prev]));
+      a.composed = rov(ch->composed.buf[cur]);
+      a.composed_carry = ch->composed.view[prev];
       a.cam = cam;
     }
     SpanGuard g(ch, cs, i == 0 ? 2 : 3);
@@ -1299,15 +1328,15 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     const Rows kr = launch_rows(ranges, k, H);
     a.row0 = kr.r0; a.row1 = kr.r1;
     if ((st = decode(a.row0, a.row1)) != RFX_OK) return st;
-    a.nrdz = ipv(ch->nrdz, W, H); a.gb = gb; a.dn = ipv(ch->dnB16[cur], W, H);
-    a.composed = OutV{(unsigned char*)ch->composed2[cur].ptr, (long long)ch->composed2[cur].pitch};
-    if (ch->group) a.composed_carry = ch->peer_composed[prev]; else peer_single(a.composed_carry, rpv(ch->composed2[prev]));
+    a.nrdz = ipv(ch->nrdz, W, H); a.gb = gb; a.dn = rpv(ch->fdnB.buf[cur]);
+    a.composed = rov(ch->composed.buf[cur]);
+    a.composed_carry = ch->composed.view[prev];
     a.W = W; a.H = H; a.cam = cam;
     SpanGuard g(ch, cs, 4);
     LAUNCHED(launch_ccompose(a, cs));
   }
   // ---- TRAA tail (reads this frame's `composed`, so it runs before the planes change parity)
-  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed2[cur], ranges, k_compose + 1)) != RFX_OK) return st;
+  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed.buf[cur], ranges, k_compose + 1)) != RFX_OK) return st;
   if (on(ch->traa_on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
   return RFX_OK;
 }
@@ -1327,29 +1356,24 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   // launches: K1, K2, K3 passes, K4 (both modes: DenoiserComposePass runs for inputType specular too), then the TRAA tail when it is on
   const int H = (int)o.height;
   // what SSGIPass samples as accumulatedTexture = denoiser.texture (Denoiser.js:67-78): the compose target, or the temporal pass's first texture
-  rfx_plane* accumulated = o.denoise_mode == RFX_DENOISE_TEMPORAL ? &ch->tr[0] : &ch->composed;
-  // row-sharded group of n > 1 (rfx_group.inl): last frame's planes are gbuf[i][gp], read on the rank that owns each row; the peer
-  // and carry instantiations are chosen for every launch of such a frame, and never otherwise
+  HistPlane& accumulated = o.denoise_mode == RFX_DENOISE_TEMPORAL ? ch->tr[0] : ch->composed;
+  // Alone the chain renders its planes in place.  In a row-sharded group of n > 1 (rfx_group.inl) the frame reads last frame's
+  // buffer `rd` of every plane it keeps, on the rank that owns each row, and writes buffer `wr`; the peer and carry instantiations
+  // are chosen for every launch of such a frame, and never otherwise.
   const bool peer = ch->group_peer;
-  const int gp = ch->gprev;
-  const int acc_i = o.denoise_mode == RFX_DENOISE_TEMPORAL ? 1 : 0;  // gbuf index of `accumulated`
-  auto carry2 = [&](int i0, int i1) { PeerCarry c{}; c.p[0] = ch->gpeer[i0][gp]; c.p[1] = ch->gpeer[i1][gp]; return c; };
+  const int rd = pass_latest(ch), wr = peer ? rd ^ 1 : rd;
+  auto carry2 = [&](const HistPlane& p0, const HistPlane& p1) { PeerCarry c{}; c.p[0] = p0.view[rd]; c.p[1] = p1.view[rd]; return c; };
   auto on = [&](uint32_t k) { return k >= k_begin && k < k_end; };
   const cudaStream_t cs = stream ? (cudaStream_t)stream : ctx->stream;
   uint32_t k = 0;
   // ---- K1  SSGIPass.render (src/ssgi/pass/SSGIPass.js:68-95)
   if (on(k)) {
-    rfx_ssgi_params sp{};
-    sp.cam = f->cam;
-    sp.ray_distance = o.distance; sp.thickness = o.thickness; sp.env_blur = o.env_blur;
-    sp.max_env_map_mip_level = ctx->env_set ? (float)((int)std::floor(std::log2((double)std::max(ctx->env.size_x, ctx->env.size_y))) + 1) : 0.0f;  // Utils.js:30-34
-    sp.steps = o.steps; sp.refine_steps = o.refine_steps; sp.mode = o.mode; sp.flags = o.ssgi_flags;
-    sp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_trace);
+    const rfx_ssgi_params sp = trace_params(ch, f);
     const Rows kr = launch_rows(ranges, k, (int)ch->ssgi_out.height);
     {
       SpanGuard g(ch, cs, 0);  // velocityTexture is a null sampler in the shipped wiring (SURVEY.md D4)
-      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, peer ? &ch->gbuf[acc_i][gp] : accumulated, &ch->ssgi_out, kr.r0, kr.r1,
-                      peer ? &ch->gpeer[acc_i][gp] : nullptr);
+      st = ssgi_trace(ctx, stream, &sp, f->depth, f->gbuffer, nullptr, f->direct_light, &accumulated.buf[rd], &ch->ssgi_out, kr.r0, kr.r1,
+                      &accumulated.view[rd]);
     }
     if (st != RFX_OK) return st;
   }
@@ -1359,13 +1383,7 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   if (on(k)) {
     rfx_temporal_params tp{};
     tp.cam = f->cam;
-    if (!ch->have_prev) {  // the constructor clones the current camera matrices (TemporalReprojectPass.js:94-97)
-      memcpy(ch->prev_view, f->cam.view_matrix, 64); memcpy(ch->prev_world, f->cam.camera_matrix_world, 64);
-      memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
-      memcpy(ch->prev_pos, f->camera_pos, 12);
-      ch->have_prev = true;
-    }
-    keep_traa_camera(ch, f);
+    prev_camera_init(ch, f);
     memcpy(tp.prev_view_matrix, ch->prev_view, 64); memcpy(tp.prev_camera_matrix_world, ch->prev_world, 64);
     memcpy(tp.prev_projection, ch->prev_proj, 64); memcpy(tp.prev_projection_inverse, ch->prev_proj_inv, 64);
     memcpy(tp.camera_pos, f->camera_pos, 12); memcpy(tp.prev_camera_pos, ch->prev_pos, 12);
@@ -1378,27 +1396,26 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
       const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, 1);
       // without a denoise pass overrideAccumulatedTextures stays empty: BOTH accumulated textures are the one FramebufferTexture
-      rfx_plane* h0 = dm_full ? &ch->dnB[0] : &ch->fb;
-      rfx_plane* h1 = dm_full ? &ch->dnB[1] : &ch->fb;
+      rfx_plane* h0 = dm_full ? &ch->dnB[0].buf[rd] : &ch->fb;
+      rfx_plane* h1 = dm_full ? &ch->dnB[1].buf[rd] : &ch->fb;
       TemporalPeer tpeer{};
       if (peer) {  // last frame's dnB, or last frame's tr[0] (of which `fb` is a byte copy on one GPU), on the owners; tr carried
-        const int i0 = dm_full ? 5 : 1, i1 = dm_full ? 6 : 1;
-        h0 = &ch->gbuf[i0][gp]; h1 = &ch->gbuf[tc == 2 ? i1 : i0][gp];
-        tpeer.hist0 = ch->gpeer[i0][gp]; tpeer.hist1 = ch->gpeer[tc == 2 ? i1 : i0][gp];
-        tpeer.carry = carry2(1, tc == 2 ? 2 : 1);
+        HistPlane& p0 = dm_full ? ch->dnB[0] : ch->tr[0];
+        HistPlane& p1 = tc == 2 && dm_full ? ch->dnB[1] : p0;
+        h0 = &p0.buf[rd]; h1 = &p1.buf[rd];
+        tpeer.hist0 = p0.view[rd]; tpeer.hist1 = p1.view[rd];
+        tpeer.carry = carry2(ch->tr[0], ch->tr[tc - 1]);
       }
-      st = temporal_reproject(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0], tc == 2 ? &ch->tr[1] : nullptr, kr.r0, kr.r1,
+      const rfx_plane* out1 = tc == 2 ? &ch->tr[1].buf[wr] : nullptr;
+      st = temporal_reproject(ctx, stream, &tp, &ch->ssgi_out, f->velocity, h0, tc == 2 ? h1 : nullptr, &ch->tr[0].buf[wr], out1, kr.r0, kr.r1,
                               peer ? &tpeer : nullptr);
     }
     if (st != RFX_OK) return st;
     // renderer.copyFramebufferToTexture(tmpVec2, this.framebufferTexture) after the draw (:197-200).  In a group the next frame reads
     // this frame's tr[0] buffer on its owners instead.
-    if (!dm_full && !peer)
-      CU(cudaMemcpy2DAsync(ch->fb.ptr, ch->fb.pitch, ch->tr[0].ptr, ch->tr[0].pitch, (size_t)ch->tr[0].width * 16, ch->tr[0].height, cudaMemcpyDeviceToDevice, cs));
-    ch->keep_data = 1.0f;  // :195
-    memcpy(ch->prev_world, f->cam.camera_matrix_world, 64); memcpy(ch->prev_view, f->cam.view_matrix, 64);
-    memcpy(ch->prev_proj, f->cam.projection, 64); memcpy(ch->prev_proj_inv, f->cam.projection_inverse, 64);
-    memcpy(ch->prev_pos, f->camera_pos, 12);
+    const rfx_plane& t0 = ch->tr[0].buf[wr];
+    if (!dm_full && !peer) CU(cudaMemcpy2DAsync(ch->fb.ptr, ch->fb.pitch, t0.ptr, t0.pitch, (size_t)t0.width * 16, t0.height, cudaMemcpyDeviceToDevice, cs));
+    prev_camera_roll(ch, f);
   }
   k++;
   // ---- K3  PoissonDenoisePass.render (PoissonDenoisePass.js:135-149)
@@ -1411,23 +1428,23 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   for (int i = 0; i < 2 * o.denoise_iterations; i++, k++) {
     if (!on(k) || !dm_full) continue;  // "full_temporal" / "temporal": no denoise pass (Denoiser.js:47-52)
     const bool horizontal = (i % 2) == 0;
-    rfx_plane* inp = i == 0 ? ch->tr : (horizontal ? ch->dnB : ch->dnA);
-    rfx_plane* outp = horizontal ? ch->dnA : ch->dnB;
+    HistPlane* inp = i == 0 ? ch->tr : (horizontal ? ch->dnB : ch->dnA);
+    HistPlane* outp = horizontal ? ch->dnA : ch->dnB;
     pp.input_linear = i == 0 ? 0 : 1;
     pp.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_poisson);
     {
       const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, i == 0 ? 2 : 3);
       // the G-buffer does not change within a frame: decode it once, reuse it afterwards
-      const PeerCarry pc = horizontal ? carry2(3, 4) : carry2(5, 6);  // dnA / dnB of last frame
-      st = poisson_denoise(ctx, stream, &pp, f->depth, f->gbuffer, &inp[0], tc == 2 ? &inp[1] : nullptr, &outp[0], tc == 2 ? &outp[1] : nullptr, kr.r0, kr.r1,
-                           decoded, peer ? &pc : nullptr);
+      const PeerCarry pc = carry2(outp[0], outp[1]);  // the target's planes of last frame
+      st = poisson_denoise(ctx, stream, &pp, f->depth, f->gbuffer, &inp[0].buf[wr], tc == 2 ? &inp[1].buf[wr] : nullptr, &outp[0].buf[wr],
+                           tc == 2 ? &outp[1].buf[wr] : nullptr, kr.r0, kr.r1, decoded, peer ? &pc : nullptr);
       decoded = true;
     }
     if (st != RFX_OK) return st;
   }
   // ---- K4  DenoiserComposePass.render ("full" and "full_temporal": Denoiser.js:55-64)
-  rfx_plane* gi = dm_full ? ch->dnB : ch->tr;  // composerInputTextures = denoisePass?.texture ?? the temporal textures
+  const HistPlane* gi = dm_full ? ch->dnB : ch->tr;  // composerInputTextures = denoisePass?.texture ?? the temporal textures
   if (on(k) && o.denoise_mode != RFX_DENOISE_TEMPORAL) {
     rfx_compose_params cp{};
     cp.cam = f->cam;
@@ -1435,15 +1452,16 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     {
       const Rows kr = launch_rows(ranges, k, H);
       SpanGuard g(ch, cs, 4);
-      const PeerPV* cc = peer ? &ch->gpeer[0][gp] : nullptr;  // last frame's `composed`
-      if (o.mode == RFX_MODE_SSGI) st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0], &gi[1], nullptr, &ch->composed, kr.r0, kr.r1, cc);
-      else st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0], f->direct_light, &ch->composed, kr.r0, kr.r1, cc);  // scene = the composer input buffer (Denoiser.js:100-102)
+      const PeerPV* cc = peer ? &ch->composed.view[rd] : nullptr;  // last frame's `composed`
+      rfx_plane* out = &ch->composed.buf[wr];
+      if (o.mode == RFX_MODE_SSGI) st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, &gi[0].buf[wr], &gi[1].buf[wr], nullptr, out, kr.r0, kr.r1, cc);
+      else st = gi_compose(ctx, stream, &cp, f->depth, f->gbuffer, nullptr, &gi[0].buf[wr], f->direct_light, out, kr.r0, kr.r1, cc);  // scene = the composer input buffer (Denoiser.js:100-102)
     }
     if (st != RFX_OK) return st;
   }
   k++;
   // ---- TRAA tail over the effect's output (`composed`, or the temporal texture in denoiseMode "temporal")
-  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, accumulated, ranges, k);
+  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, &accumulated.buf[wr], ranges, k);
   return RFX_OK;
 }
 
@@ -1490,15 +1508,15 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
   f.depth = &ch->in_depth[set]; f.gbuffer = &ch->in_gb[set]; f.velocity = &ch->in_vel[set]; f.direct_light = hf->direct_light ? &ch->in_direct[set] : nullptr;
   memcpy(f.camera_pos, hf->camera_pos, 12);
   f.camera_moved = hf->camera_moved;
-  const rfx_plane* result = &ch->composed;
+  const rfx_plane* result = &ch->composed.buf[0];
   if (ch->fastpath) {
-    // `composed` is double-buffered by frame parity: this frame writes composed2[cur], whose previous reader is the D2H of two
+    // `composed` is double-buffered by frame parity: this frame writes composed.buf[cur], whose previous reader is the D2H of two
     // frames ago (long finished in steady state); frame i-1's D2H keeps running under this frame's kernels
     const int cur = (int)(ch->frame_idx & 1);
     for (int q = 0; q < 2; q++)
       if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, ch->ev_dn[q], 0));
     if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, 0xffffffffu)) != RFX_OK) return st;
-    result = &ch->composed2[cur];
+    result = &ch->composed.buf[cur];
     ch->dn_buf[set] = cur;
   } else {
     const uint32_t n_launches = 3u + 2u * (uint32_t)ch->opt.denoise_iterations;
