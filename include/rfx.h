@@ -326,7 +326,11 @@ rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_p
 
 /* K5. src/ssgi/shader/ssgi_compose.frag:20-44.  gi RGBA32F, scene RGBA16F, out RGBA16F.  `p` may be NULL (no fog, no debug).
  * Fog = three.js <fog_fragment> as patched by src/ssgi/SSGIEffect.js:34-43 on vFogDepth = -getViewZ(depth) * 0.4:
- * FogExp2: 1 - exp(-density^2 * d^2); Fog: smoothstep(near, far, d); uniforms from scene.fog (SSGIEffect.js:404-412). */
+ * FogExp2: 1 - exp(-density^2 * d^2); Fog: smoothstep(near, far, d); uniforms from scene.fog (SSGIEffect.js:404-412).
+ * p->is_debug = 1 (ssgi_compose.frag:21-24, outputColor = textureLod(inputTexture, uv, 0.)): `gi` is the debug view and may be any
+ * plane of any size, fetched at the pixel centre with its own sampler: RGBA32F NEAREST (composed, the SSGI target, trOut, velocity,
+ * the G-buffer, the G-buffer debug target), RGBA16F LINEAR (dnB), R32F a depth texture, which reads (d, 0, 0, 1).  depth and
+ * scene are not read then and may be NULL. */
 typedef struct rfx_ssgi_compose_params {
   int32_t use_fog;      /* #define USE_FOG  (scene.fog != null)            */
   int32_t fog_exp2;     /* #define FOG_EXP2 (scene.fog.isFogExp2)          */
@@ -382,6 +386,15 @@ rfx_status rfx_effects_launch(rfx_ctx* ctx, void* stream, const rfx_effects_para
  * out RGBA8 (the canvas: clamp, round to nearest) */
 rfx_status rfx_taa_launch(rfx_ctx* ctx, void* stream, const rfx_taa_params* p, const rfx_plane* input, const rfx_plane* history,
                           const rfx_plane* out, uint32_t row0, uint32_t row1);
+
+/* GBufferDebugPass (src/gbuffer/debug/GBufferDebugPass.js): one channel of the packed G-buffer decoded by getMaterial
+ * (gbuffer_packing.glsl), rgb = the channel, a = 1.  gbuffer and out RGBA32F of the same size.  mode = the index of the channel in
+ * ["diffuse", "alpha", "normal", "roughness", "metalness", "emissive"] (SSGIEffect.js:237-239); any other value (an unknown string
+ * gives -1 there) shows emissive, the shader's `else` branch.  The pass's `depthTexture` sampler is never bound (it is missing from
+ * the material's uniforms, so it keeps unit 0, which is gBufferTexture's): a texel whose gBuffer.r compares equal to 0 - packed
+ * albedo bits 0x00000000 or 0x80000000, i.e. the background clear texel and transparent-black albedo - is written (0, 0, 0, 0). */
+rfx_status rfx_gbuffer_debug_launch(rfx_ctx* ctx, void* stream, int32_t mode, const rfx_plane* gbuffer, const rfx_plane* out,
+                                    uint32_t row0, uint32_t row1);
 
 /* K9. src/traa/shader/traa_compose.frag:3-6  accumulated RGBA16F -> out RGBA16F (a = 1) */
 rfx_status rfx_traa_compose_launch(rfx_ctx* ctx, void* stream, const rfx_plane* accumulated,
@@ -459,6 +472,25 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* chain, const rfx_traa_tail
 /* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the K9 output (RGBA16F), 7 the TRAA
  * accumulated plane of the latest frame (RGBA16F; next frame's history).  6 / 7 with the tail off: RFX_ERR_NOT_READY. */
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane* out);
+/* Debug view of the TRAA tail: SSGIEffect's `outputTexture` (src/ssgi/SSGIEffect.js:228-251, picked from the "Debug" list of
+ * example/SSGIDebugGUI.js:78-114).  With a view selected, the tail's K5 runs with isDebug and samples the view instead of `composed`
+ * (ssgi_compose.frag:21-24), and that image goes through the TRAA pass and K9 as in the demo's frame.  Views:
+ *   RFX_DEBUG_VIEW_NONE                    today's tail; also what RFX_DEBUG_VIEW_OUTPUT + 0 (denoiser.texture) selects, since
+ *                                          isDebug = outputTexture !== denoiser.texture (SSGIEffect.js:249)
+ *   RFX_DEBUG_VIEW_OUTPUT + 1..5           rfx_ssgi_chain_output's planes 1..5 (ssgiOut, trOut[0/1], dnB[0/1]); a plane the
+ *                                          configuration does not have is refused with rfx_ssgi_chain_output's status
+ *   RFX_DEBUG_VIEW_DEPTH / _VELOCITY / _GBUFFER   the frame's depth, velocity or packed G-buffer plane
+ *   RFX_DEBUG_VIEW_GBUFFER_CHANNEL + m     GBufferDebugPass mode m (0..5, see rfx_gbuffer_debug_launch) of the frame's G-buffer,
+ *                                          rendered into a chain-owned RGBA32F target every frame before the tail
+ * While a view is selected the fast chain runs its tail as the three per-pass launches.  Selecting a view does not reset any
+ * history (the reference's outputTexture setter calls no reset()).  A chain in a group of n > 1 takes no view: RFX_ERR_UNSUPPORTED. */
+#define RFX_DEBUG_VIEW_NONE (-1)
+#define RFX_DEBUG_VIEW_OUTPUT 0
+#define RFX_DEBUG_VIEW_DEPTH 8
+#define RFX_DEBUG_VIEW_VELOCITY 9
+#define RFX_DEBUG_VIEW_GBUFFER 10
+#define RFX_DEBUG_VIEW_GBUFFER_CHANNEL 16
+rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* chain, int32_t view);
 /* host-buffer frame: uploads the four input planes from (pinned) host memory, renders,
  * downloads `composed` into out_host.  This is the call `bench.py`'s e2e leg times. */
 typedef struct rfx_ssgi_host_frame {

@@ -16,6 +16,9 @@ const rfx = createRequire(import.meta.url)("./napi/rfx_napi.node")
 const FMT = { R32F: 0, RGBA32F: 1, RGBA16F: 2, RGBA8: 3 }
 const FLAG = { importanceSampling: 1, missedRays: 2, useDirectLight: 4, useEnvMap: 8 }
 const INPUT = { diffuseSpecular: 0, diffuse: 1, specular: 2 }
+// rfx_ssgi_chain_set_debug_view (include/rfx.h): chain output n is output + n, GBufferDebugPass mode m gbufferChannel + m
+export const DEBUG_VIEW = { none: -1, output: 0, depth: 8, velocity: 9, gbuffer: 10, gbufferChannel: 16 }
+export const GBUFFER_DEBUG_MODES = ["diffuse", "alpha", "normal", "roughness", "metalness", "emissive"]   // SSGIEffect.js:237
 let sharedCtx = null
 export const context = (device = 0) => (sharedCtx ??= rfx.ctxCreate(device))
 
@@ -134,8 +137,39 @@ export class SSGIEffect {
 		this.isUsingRenderPass = true
 		this._hasEnv = false
 		this.lastPos = null; this.lastQuat = null
+		// textures a debug view can name that outlive setSize: chain output n (the fast chain re-splits trOut / dnB when read) and the
+		// frame's planes of the plane source; denoiserTexture is chain output 0, denoiser.texture (Denoiser.js:67-78)
+		this._chainTextures = [0, 1, 2, 3, 4, 5].map(n => ({ chainOutput: n }))
+		this._frameTextures = { depth: { framePlane: "depth" }, velocity: { framePlane: "velocity" }, gbuffer: { framePlane: "gbuffer" } }
+		this.denoiserTexture = this._chainTextures[0]
+		this._view = null; this.isDebug = false; this.gBufferDebugTarget = null; this._gBufferDebugMode = 0
 		reactive(this, opts, key => (key === "resolutionScale" ? this.setSize(this.width, this.height, true) : this._setOptions()))
+		// outputTexture (SSGIEffect.js:228-251): not a chain option and no reset()
+		Object.defineProperty(this, "outputTexture", { get: () => this._view ?? this.denoiserTexture, set: v => this._setOutputTexture(v), configurable: true })
+		opts.outputTexture = this.denoiserTexture   // :139
 		this.setSize(options.width ?? composer?.inputBuffer?.width, options.height ?? composer?.inputBuffer?.height)
+	}
+	chainTexture(n) { return this._chainTextures[n] }            // chain output n (1 ssgiOut, 2/3 trOut, 4/5 dnB) as a debug view
+	frameTexture(name) { return this._frameTextures[name] }      // "depth" | "velocity" | "gbuffer": the frame's plane as a debug view
+	// falsy: ignored; a string: GBufferDebugPass mode (index in GBUFFER_DEBUG_MODES, -1 = emissive) rendered after the chain, whose target
+	// becomes the view; a texture (chainTexture / frameTexture / a plane the host holds): that texture.  isDebug = view !== denoiserTexture
+	_setOutputTexture(value) {
+		if (!value) return
+		if (typeof value === "string") {
+			this.gBufferDebugTarget ??= rfx.planeAlloc(this.ctx, FMT.RGBA32F, this.width, this.height)
+			this._gBufferDebugMode = GBUFFER_DEBUG_MODES.indexOf(value)
+			this._view = this.gBufferDebugTarget
+		} else {
+			if (this.gBufferDebugTarget && value !== this.gBufferDebugTarget) { rfx.planeFree(this.ctx, this.gBufferDebugTarget); this.gBufferDebugTarget = null }
+			this._view = value === this.denoiserTexture ? null : value
+		}
+		this.isDebug = this._view !== null
+		this._options.outputTexture = this.outputTexture
+	}
+	_resolve(t, planes) {
+		if (t.chainOutput !== undefined) return rfx.chainOutput(this.ctx, this.chain, t.chainOutput)
+		if (t.framePlane !== undefined) return planes[t.framePlane]
+		return t
 	}
 	_flags() {
 		const o = this._options
@@ -157,6 +191,10 @@ export class SSGIEffect {
 		this.planeSource = new ReadbackPlaneSource(this.ctx, width, height)
 		this.outputPlane = rfx.planeAlloc(this.ctx, FMT.RGBA16F, width, height)
 		this.outputHost = new Uint16Array(width * height * 4)
+		if (this.gBufferDebugTarget) {   // GBufferDebugPass.setSize at the effect's size
+			rfx.planeFree(this.ctx, this.gBufferDebugTarget)
+			this.gBufferDebugTarget = this._view = rfx.planeAlloc(this.ctx, FMT.RGBA32F, width, height)
+		}
 	}
 	// keepEnvMapUpdated (src/ssgi/SSGIEffect.js:309-366): equirect RGBA16F map; the CDF tables are built on the device
 	setEnvironment(mapF16, width, height) { rfx.envBuild(this.ctx, mapF16, width, height); this._hasEnv = true; this._setOptions() }
@@ -164,7 +202,7 @@ export class SSGIEffect {
 	initialize() {}
 	reset() { rfx.chainReset(this.chain) }
 	get depthTexture() { return this.gBufferPass?.depthTexture }
-	get outputTexture() { return this.outputHost }      // K5 output (RGBA16F), uploaded into the composer's output buffer by the glue
+	// outputHost: the K5 output (RGBA16F), uploaded into the composer's output buffer by the glue.  outputTexture: see the constructor.
 	// update(renderer, inputBuffer, deltaTime) — src/ssgi/SSGIEffect.js:372-404
 	update(renderer, inputBuffer, deltaTime) {
 		const cam = cameraBlock(this._camera)
@@ -175,10 +213,11 @@ export class SSGIEffect {
 			velocity: this.velocityDepthNormalPass?.renderTarget, directLight: inputBuffer })
 		rfx.chainRender(this.ctx, this.chain, cam, planes.depth, planes.gbuffer, planes.velocity, this.isUsingRenderPass ? planes.directLight : null,
 			new Float32Array(this._camera.position.toArray()), moved)
-		// K5: ssgi_compose.frag (mainImage of the effect)
+		if (this.gBufferDebugTarget) rfx.gbufferDebug(this.ctx, this._gBufferDebugMode, planes.gbuffer, this.gBufferDebugTarget)   // SSGIEffect.js:398-399
+		// K5: ssgi_compose.frag (mainImage of the effect); with isDebug the view itself, with its own sampler (:21-24)
 		const fog = this._scene.fog   // SSGIEffect.js:404-412
-		rfx.ssgiCompose(this.ctx, planes.depth, rfx.chainOutput(this.ctx, this.chain, 0), planes.directLight, this.outputPlane, {
-			near: this._camera.near, far: this._camera.far, perspective: this._camera.isPerspectiveCamera !== false, isDebug: false,
+		rfx.ssgiCompose(this.ctx, planes.depth, this._resolve(this.outputTexture, planes), planes.directLight, this.outputPlane, {
+			near: this._camera.near, far: this._camera.far, perspective: this._camera.isPerspectiveCamera !== false, isDebug: this.isDebug,
 			...(fog ? { fog: { color: fog.color.toArray(), near: fog.near, far: fog.far, density: fog.density, isFogExp2: !!fog.isFogExp2 } } : {})
 		})
 		rfx.planeDownload(this.ctx, this.outputPlane, this.outputHost)
@@ -188,6 +227,8 @@ export class SSGIEffect {
 		this.chain = null
 		this.planeSource?.dispose()
 		if (this.outputPlane) rfx.planeFree(this.ctx, this.outputPlane)
+		if (this.gBufferDebugTarget) rfx.planeFree(this.ctx, this.gBufferDebugTarget)
+		this.outputPlane = this.gBufferDebugTarget = null
 	}
 }
 SSGIEffect.DefaultOptions = defaultSSGIOptions

@@ -254,7 +254,9 @@ napi_value ChainEnableTraa(napi_env env, napi_callback_info info) {
 }
 
 // ---- per-pass launches (one per reference fullscreen draw; whole planes) ------------------------------------------------------------
-napi_value SsgiCompose(napi_env env, napi_callback_info info) {  // ssgiCompose(ctx, depth, gi, scene, out[, {fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug}])
+// ssgiCompose(ctx, depth, gi, scene, out[, {fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug}]); with isDebug, gi is the
+// debug view: any R32F / RGBA16F / RGBA32F plane of any size (depth / scene are not read then and may be null)
+napi_value SsgiCompose(napi_env env, napi_callback_info info) {
   ARGS(6); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
   rfx_ssgi_compose_params p{};
   napi_valuetype t = napi_undefined;
@@ -345,6 +347,19 @@ napi_value MotionBlur(napi_env env, napi_callback_info info) {  // motionBlur(ct
 napi_value TraaCompose(napi_env env, napi_callback_info info) {  // traaCompose(ctx, accumulated, out)
   ARGS(3); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
   CHECK(c, rfx_traa_compose_launch(c, nullptr, unwrap<rfx_plane>(env, argv[1]), unwrap<rfx_plane>(env, argv[2]), 0, 0), "rfx_traa_compose_launch");
+  return undefined(env);
+}
+
+napi_value GbufferDebug(napi_env env, napi_callback_info info) {  // gbufferDebug(ctx, mode, gbuffer, out): GBufferDebugPass (mode 0..5; other values show emissive)
+  ARGS(4); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  int32_t mode = 0; napi_get_value_int32(env, argv[1], &mode);
+  CHECK(c, rfx_gbuffer_debug_launch(c, nullptr, mode, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), 0, 0), "rfx_gbuffer_debug_launch");
+  return undefined(env);
+}
+napi_value ChainSetDebugView(napi_env env, napi_callback_info info) {  // chainSetDebugView(ctx, chain, view): RFX_DEBUG_VIEW_* (the TRAA tail's K5)
+  ARGS(3); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  int32_t view = RFX_DEBUG_VIEW_NONE; napi_get_value_int32(env, argv[2], &view);
+  CHECK(c, rfx_ssgi_chain_set_debug_view(unwrap<rfx_ssgi_chain>(env, argv[1]), view), "rfx_ssgi_chain_set_debug_view");
   return undefined(env);
 }
 
@@ -439,7 +454,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
       FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
       FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur),
-      FN("traaCompose", TraaCompose), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
+      FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),
       FN("groupDestroy", GroupDestroy), FN("chainRenderSharded", ChainRenderSharded),
   };

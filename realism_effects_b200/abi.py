@@ -24,6 +24,9 @@ ERR_NCCL = 7
 INPUT_DIFFUSE_SPECULAR, INPUT_DIFFUSE, INPUT_SPECULAR = 0, 1, 2
 DENOISE_FULL, DENOISE_FULL_TEMPORAL, DENOISE_TEMPORAL = 0, 1, 2  # option denoiseMode (src/denoise/Denoiser.js:7)
 DENOISE_MODES = {"full": 0, "full_temporal": 1, "temporal": 2}
+# rfx_ssgi_chain_set_debug_view (include/rfx.h): chain output n is DEBUG_VIEW_OUTPUT + n, GBufferDebugPass mode m DEBUG_VIEW_GBUFFER_CHANNEL + m
+DEBUG_VIEW_NONE, DEBUG_VIEW_OUTPUT, DEBUG_VIEW_DEPTH, DEBUG_VIEW_VELOCITY, DEBUG_VIEW_GBUFFER, DEBUG_VIEW_GBUFFER_CHANNEL = -1, 0, 8, 9, 10, 16
+GBUFFER_DEBUG_MODES = ["diffuse", "alpha", "normal", "roughness", "metalness", "emissive"]  # SSGIEffect.js:237
 
 F16 = C.c_float * 16
 F3 = C.c_float * 3
@@ -222,6 +225,8 @@ def _sig(lib):
     lib.rfx_ao_compose_launch.argtypes = [vp, vp, _P(AoComposeParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_motion_blur_launch.argtypes = [vp, vp, _P(MotionBlurParams), PP, PP, PP, u32, u32]
     lib.rfx_traa_compose_launch.argtypes = [vp, vp, PP, PP, u32, u32]
+    lib.rfx_gbuffer_debug_launch.argtypes = [vp, vp, C.c_int32, PP, PP, u32, u32]
+    lib.rfx_ssgi_chain_set_debug_view.argtypes = [vp, C.c_int32]
     lib.rfx_effects_launch.argtypes = [vp, vp, _P(EffectsParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_taa_launch.argtypes = [vp, vp, _P(TaaParams), PP, PP, PP, u32, u32]
     lib.rfx_gbuffer_ingest_launch.argtypes = [vp, vp, _P(IngestParams), PP, PP, PP, PP, PP, PP, PP, PP, u32, u32]
@@ -276,7 +281,7 @@ EXPORTS = [
     "rfx_plane_download_rows", "rfx_group_get_unique_id", "rfx_group_create", "rfx_group_create_inprocess", "rfx_group_attach_chains_inprocess", "rfx_group_destroy", "rfx_group_rank", "rfx_group_world", "rfx_group_uses_peer_reads",
     "rfx_group_attach_chain", "rfx_group_get_bounds", "rfx_group_set_bounds", "rfx_group_set_rebalance", "rfx_group_last_costs",
     "rfx_group_begin_frame", "rfx_group_get_last_bounds", "rfx_group_allgather_rows", "rfx_ssgi_chain_render_sharded", "rfx_shard_ranges",
-    "rfx_shard_rebalance",
+    "rfx_shard_rebalance", "rfx_gbuffer_debug_launch", "rfx_ssgi_chain_set_debug_view",
 ]
 
 

@@ -3,6 +3,8 @@
 // K6 replaces reference src/ao/AOPass.js:108-109 running src/hbao/shader/hbao.frag:64-96 (+ hbao_utils.glsl,
 // whose stale line-1 include is dropped, SURVEY.md D3); K7 src/ao/shader/ao_compose.frag:6-16;
 // K8 src/motion-blur/shader/motion_blur.frag:11-44; K9 src/traa/shader/traa_compose.frag:3-6.
+// Debug views: GBufferDebugPass (src/gbuffer/debug/GBufferDebugPass.js) and K5's isDebug branch (ssgi_compose.frag:21-24) for
+// the views ssgi_compose_kernel does not fetch.
 #include "rfx_kernels.h"
 
 namespace rfx {
@@ -248,6 +250,52 @@ cudaError_t launch_env_cdf(PV map, int flip_y, float* cdf_c, float* cdf_m, doubl
   env_row_scan_kernel<<<(map.h + 63) / 64, 64, 0, s>>>(map, flip_y, cdf_c, row_sum);
   env_totals_kernel<<<1, 1, 0, s>>>(map, flip_y, row_sum, cdf_m, total);
   env_inverse_cdf_kernel<<<(map.w * map.h + 255) / 256, 256, 0, s>>>(cdf_m, cdf_c, map.w, map.h, marginal, conditional);
+  return cudaGetLastError();
+}
+
+// GBufferDebugPass: getMaterial (gbuffer_packing.glsl:181-196) at the pixel's own texel (target and G-buffer have one size, NEAREST).
+// `depth` is gBuffer.r: the shader's depthTexture is not among the material's uniforms, so its sampler stays on unit 0, gBufferTexture's.
+__global__ void __launch_bounds__(256) gbuffer_debug_kernel(const __grid_constant__ GbufferDebugArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.W || y >= a.row1) return;
+  const float4 g = ld_f4(a.gb, x, y);
+  float4 o = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+  if (g.x != 0.0f) {
+    v3 c;
+    switch (a.mode) {
+      case 0: c = xyz(floatToVec4(g.x)); break;
+      case 1: c = mk3(floatToVec4(g.x).w); break;
+      case 2: c = unpackNormal(g.y); break;
+      case 3: c = mk3(gb_roughness(g.z)); break;
+      case 4: c = mk3(gb_metalness(g.z)); break;
+      default: c = decodeRGBE8<true>(floatToVec4(g.w)); break;
+    }
+    o = make_float4(c.x, c.y, c.z, 1.0f);
+  }
+  st_f4(a.out.p, a.out.pitch, x, y, o);
+}
+cudaError_t launch_gbuffer_debug(const GbufferDebugArgs& a, cudaStream_t s) {
+  dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
+  gbuffer_debug_kernel<<<grid, 256, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
+// K5 with isDebug: textureLod(inputTexture, vUv, 0.) rounded to the RGBA16F composer buffer.  A depth texture reads (d, 0, 0, 1)
+// (GLES 3.0 depth-texture swizzle).  NEAREST and LINEAR are those of every other pass (nearest_i, bilin_setup), so a source of
+// another size is resampled exactly as the reference's sampler would.
+__global__ void __launch_bounds__(256) ssgi_compose_debug_kernel(const __grid_constant__ SsgiComposeDebugArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.W || y >= a.row1) return;
+  const v2 uv = pixel_uv(x, y, a.W, a.H);
+  v4 c;
+  if (a.gi_fmt == RFX_FMT_R32F) c = mk4(tex_r32f_nearest(a.gi, uv), 0.0f, 0.0f, 1.0f);
+  else if (a.gi_fmt == RFX_FMT_RGBA16F) c = tex_h4_linear(a.gi, uv);
+  else c = f4v(tex_f4_nearest(a.gi, uv));
+  st_h4(a.out.p, a.out.pitch, x, y, c);
+}
+cudaError_t launch_ssgi_compose_debug(const SsgiComposeDebugArgs& a, cudaStream_t s) {
+  dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
+  ssgi_compose_debug_kernel<<<grid, 256, 0, s>>>(a);
   return cudaGetLastError();
 }
 

@@ -632,9 +632,22 @@ rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_p
   return gi_compose(ctx, stream, p, depth, gb, dgi, sgi, scene, out, r0, r1);
 }
 
+// K5 with isDebug for a view ssgi_compose_kernel does not fetch (another format or size): depth and scene are not read
+static rfx_status ssgi_compose_debug(rfx_ctx* ctx, void* stream, const rfx_plane* gi, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  SsgiComposeDebugArgs a{};
+  a.gi_fmt = (int)gi->format;
+  if ((a.gi_fmt != RFX_FMT_R32F && a.gi_fmt != RFX_FMT_RGBA16F && a.gi_fmt != RFX_FMT_RGBA32F) || !pv(gi, a.gi_fmt, a.gi) || !ov(out, RFX_FMT_RGBA16F, a.out))
+    return fail(ctx, RFX_ERR_BAD_FORMAT, "ssgi_compose: a debug view must be R32F, RGBA16F or RGBA32F and out RGBA16F");
+  a.W = (int)out->width; a.H = (int)out->height;
+  rows(row0, row1, out->height, a.row0, a.row1);
+  LAUNCHED(launch_ssgi_compose_debug(a, pick(ctx, stream)));
+  return RFX_OK;
+}
 rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_compose_params* p, const rfx_plane* depth, const rfx_plane* gi, const rfx_plane* scene,
                                    const rfx_plane* out, uint32_t row0, uint32_t row1) {
   if (!ctx || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ssgi_compose: null argument");
+  if (p && p->is_debug && gi && (!depth || !scene || !(gi->format == RFX_FMT_RGBA32F && gi->width == out->width && gi->height == out->height)))
+    return ssgi_compose_debug(ctx, stream, gi, out, row0, row1);
   SsgiComposeArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(gi, RFX_FMT_RGBA32F, a.gi) || !pv(scene, RFX_FMT_RGBA16F, a.scene) || !ov(out, RFX_FMT_RGBA16F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "ssgi_compose: depth R32F, gi RGBA32F, scene/out RGBA16F required");
@@ -718,6 +731,18 @@ rfx_status rfx_motion_blur_launch(rfx_ctx* ctx, void* stream, const rfx_motion_b
   rfx_status st = blue_for(ctx, p->frame, a.blue);
   if (st != RFX_OK) return st;
   LAUNCHED(launch_motion_blur(a, pick(ctx, stream)));
+  return RFX_OK;
+}
+
+rfx_status rfx_gbuffer_debug_launch(rfx_ctx* ctx, void* stream, int32_t mode, const rfx_plane* gbuffer, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  if (!ctx || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "gbuffer_debug: null argument");
+  GbufferDebugArgs a{};
+  if (!pv(gbuffer, RFX_FMT_RGBA32F, a.gb) || !ov(out, RFX_FMT_RGBA32F, a.out)) return fail(ctx, RFX_ERR_BAD_FORMAT, "gbuffer_debug: RGBA32F planes required");
+  a.W = (int)out->width; a.H = (int)out->height;
+  if (a.gb.w != a.W || a.gb.h != a.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "gbuffer_debug: plane sizes differ");
+  a.mode = mode >= 0 && mode <= 5 ? mode : 5;  // the shader's `else` branch: emissive
+  rows(row0, row1, out->height, a.row0, a.row1);
+  LAUNCHED(launch_gbuffer_debug(a, pick(ctx, stream)));
   return RFX_OK;
 }
 
@@ -854,10 +879,13 @@ struct rfx_ssgi_chain {
   rfx_traa_tail_options traa{};
   HistPlane traa_acc;                   // accumulated plane by tail parity (buf[prev] is the history)
   rfx_plane traa_out{};                 // K9 output
-  rfx_plane traa_k5{};                  // K5 plane of the per-pass tail (chains other than the fast one)
+  rfx_plane traa_k5{};                  // K5 plane of the per-pass tail (chains other than the fast one, and the fast one with a debug view)
   uint64_t traa_frames = 0;             // tails rendered; traa_acc.buf[traa_frames & 1] is written next
   float traa_keep = 0.0f;               // keepData of the TRAA pass
   rfx_temporal_params traa_tp{};        // the frame's camera and the previous-frame matrices its K2 used
+  // debug view of the tail's K5 (rfx_ssgi_chain_set_debug_view); RFX_DEBUG_VIEW_NONE: composed, isDebug off
+  int32_t debug_view = RFX_DEBUG_VIEW_NONE;
+  rfx_plane debug_gb{};                 // GBufferDebugPass target of the G-buffer channel views
   // per-pass chain (not the fast one) attached to a group of n > 1: the peer / carry instantiations and both buffers of every plane
   // it keeps are in use.  A frame's kernels read last frame's rows on their owners and carry the texels of discarded pixels from there.
   bool group_peer = false;
@@ -957,7 +985,7 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   if (ch->s_dn) cudaStreamSynchronize(ch->s_dn);
   for (HistPlane* h : every_hist_plane(ch))
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ctx, &p);
-  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->traa_out, &ch->traa_k5,
+  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->traa_out, &ch->traa_k5, &ch->debug_gb,
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
   for (IPlane* p : {&ch->nrdz, &ch->tr32}) if (p->p) cudaFree(p->p);
@@ -1024,7 +1052,8 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_op
     rfx_status st = RFX_OK;
     for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out})
       if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
-    if (st == RFX_OK && !ch->fastpath) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
+    if (st == RFX_OK && (!ch->fastpath || ch->debug_view != RFX_DEBUG_VIEW_NONE))  // the fast chain's fused tail needs no K5 plane
+      st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
     if (st != RFX_OK) {
       for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
       return st;
@@ -1036,6 +1065,27 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_op
   ch->traa_keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
   return RFX_OK;
 }
+
+}  // extern "C"
+// fast chain: tr[]/dnB[] buffer 0 := the reference-format views of the interleaved planes, dn from fdnB.buf[parity]
+static rfx_status split_views(rfx_ssgi_chain* ch, int parity, cudaStream_t s) {
+  rfx_ctx* ctx = ch->ctx;
+  const int W = (int)ch->opt.width, H = (int)ch->opt.height;
+  LAUNCHED(launch_split_tr(PV{(const unsigned char*)ch->tr32.p, W, H, (long long)ch->tr32.pitch}, rov(ch->tr[0].buf[0]), rov(ch->tr[1].buf[0]), W, H, s));
+  LAUNCHED(launch_split_dn(rpv(ch->fdnB.buf[parity]), rov(ch->dnB[0].buf[0]), rov(ch->dnB[1].buf[0]), W, H, s));
+  ch->views_valid = true;
+  return RFX_OK;
+}
+// fast chain: the reference-format planes tr[]/dnB[] buffer 0 that split_views fills (allocated once, on first use)
+static rfx_status alloc_split_views(rfx_ssgi_chain* ch) {
+  rfx_status st = RFX_OK;
+  for (int i = 0; i < 2 && st == RFX_OK; i++) {
+    if (!ch->tr[i].buf[0].ptr) st = rfx_plane_alloc(ch->ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->tr[i].buf[0]);
+    if (st == RFX_OK && !ch->dnB[i].buf[0].ptr) st = rfx_plane_alloc(ch->ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->dnB[i].buf[0]);
+  }
+  return st;
+}
+extern "C" {
 
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
@@ -1052,19 +1102,13 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* o
     if (which == 1) { *out = ch->ssgi_out; return RFX_OK; }
     // views of the interleaved planes in the reference's formats, refreshed on the context stream
     rfx_plane *tr0 = &ch->tr[0].buf[0], *tr1 = &ch->tr[1].buf[0], *dn0 = &ch->dnB[0].buf[0], *dn1 = &ch->dnB[1].buf[0];
-    if (!tr0->ptr) {
-      rfx_status st = RFX_OK;
-      for (int i = 0; i < 2 && st == RFX_OK; i++) {
-        st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->tr[i].buf[0]);
-        if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->dnB[i].buf[0]);
-      }
+    if (!tr0->ptr || !dn1->ptr) {
+      rfx_status st = alloc_split_views(ch);
       if (st != RFX_OK) return st;
     }
     if (!ch->views_valid) {
-      const int W = (int)ch->opt.width, H = (int)ch->opt.height;
-      LAUNCHED(launch_split_tr(PV{(const unsigned char*)ch->tr32.p, W, H, (long long)ch->tr32.pitch}, rov(*tr0), rov(*tr1), W, H, ctx->stream));
-      LAUNCHED(launch_split_dn(rpv(ch->fdnB.buf[last]), rov(*dn0), rov(*dn1), W, H, ctx->stream));
-      ch->views_valid = true;
+      rfx_status st = split_views(ch, last, ctx->stream);
+      if (st != RFX_OK) return st;
     }
     *out = which == 2 ? *tr0 : which == 3 ? *tr1 : which == 4 ? *dn0 : *dn1;
     return RFX_OK;
@@ -1080,6 +1124,28 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* o
     case 4: *out = latest(ch->dnB[0]); break;
     default: *out = latest(ch->dnB[1]); break;
   }
+  return RFX_OK;
+}
+
+rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* ch, int32_t view) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (view == RFX_DEBUG_VIEW_OUTPUT) view = RFX_DEBUG_VIEW_NONE;  // denoiser.texture: isDebug is false (SSGIEffect.js:249)
+  const bool plane = view > RFX_DEBUG_VIEW_OUTPUT && view <= RFX_DEBUG_VIEW_OUTPUT + 5;
+  const bool channel = view >= RFX_DEBUG_VIEW_GBUFFER_CHANNEL && view <= RFX_DEBUG_VIEW_GBUFFER_CHANNEL + 5;
+  if (!(view == RFX_DEBUG_VIEW_NONE || plane || channel || view == RFX_DEBUG_VIEW_DEPTH || view == RFX_DEBUG_VIEW_VELOCITY || view == RFX_DEBUG_VIEW_GBUFFER))
+    return fail(ctx, RFX_ERR_INVALID_ARG, "chain_set_debug_view: unknown view %d", view);
+  if (view != RFX_DEBUG_VIEW_NONE && ch->group && rfx_group_world(ch->group) > 1)
+    return fail(ctx, RFX_ERR_UNSUPPORTED, "chain_set_debug_view: a chain in a row-sharded group takes no debug view");
+  // Every plane a view needs is allocated here, and nothing is launched: the frame that shows the view fills them on its own stream.
+  // Every configuration has planes 1..5 (the per-pass chain allocates them all; the fast chain splits its interleaved ones).
+  rfx_status st = RFX_OK;
+  if (ch->fastpath && plane && view >= RFX_DEBUG_VIEW_OUTPUT + 2) st = alloc_split_views(ch);
+  if (st == RFX_OK && channel && !ch->debug_gb.ptr) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->debug_gb);
+  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->traa_on && !ch->traa_k5.ptr)  // the tail's K5 plane (the fused fast tail has none)
+    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
+  if (st != RFX_OK) return st;
+  ch->debug_view = view;
   return RFX_OK;
 }
 
@@ -1132,6 +1198,29 @@ static void prev_camera_roll(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f) {
   memcpy(ch->prev_pos, f->camera_pos, 12);
 }
 
+// The plane the tail's K5 shows for the chain's debug view in this frame (the fast chain splits this frame's interleaved planes; the
+// G-buffer channel views run GBufferDebugPass, which SSGIEffect.update renders right after SSGIPass, SSGIEffect.js:398-399)
+static rfx_status debug_view_plane(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane** out) {
+  const int v = ch->debug_view;
+  if (v == RFX_DEBUG_VIEW_DEPTH) *out = f->depth;
+  else if (v == RFX_DEBUG_VIEW_VELOCITY) *out = f->velocity;
+  else if (v == RFX_DEBUG_VIEW_GBUFFER) *out = f->gbuffer;
+  else if (v >= RFX_DEBUG_VIEW_GBUFFER_CHANNEL) {
+    rfx_status st = rfx_gbuffer_debug_launch(ch->ctx, stream, v - RFX_DEBUG_VIEW_GBUFFER_CHANNEL, f->gbuffer, &ch->debug_gb, 0, 0);
+    if (st != RFX_OK) return st;
+    *out = &ch->debug_gb;
+  } else if (v == RFX_DEBUG_VIEW_OUTPUT + 1) {
+    *out = &ch->ssgi_out;
+  } else if (ch->fastpath) {
+    rfx_status st = split_views(ch, (int)(ch->frame_idx & 1), pick(ch->ctx, stream));
+    if (st != RFX_OK) return st;
+    *out = v == 2 ? &ch->tr[0].buf[0] : v == 3 ? &ch->tr[1].buf[0] : v == 4 ? &ch->dnB[0].buf[0] : &ch->dnB[1].buf[0];
+  } else {
+    *out = v == 2 ? &ch->tr[0].buf[0] : v == 3 ? &ch->tr[1].buf[0] : v == 4 ? &ch->dnB[0].buf[0] : &ch->dnB[1].buf[0];  // alone: buffer 0
+  }
+  return RFX_OK;
+}
+
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
 // rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
 // K2 on them +- 1).
@@ -1147,7 +1236,8 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   tp.full_accumulate = ch->traa.full_accumulate && !f->camera_moved ? 1 : 0;
   tp.texture_count = 1; tp.input_type = RFX_INPUT_DIFFUSE; tp.history_linear = 1;
   tp.reproject_specular[0] = tp.reproject_specular[1] = 0;
-  if (ch->fastpath) {
+  const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
+  if (ch->fastpath && !debug) {
     CTraaArgs a{};
     TemporalArgs& t = a.t;
     if (!pv(f->velocity, RFX_FMT_RGBA32F, t.velocity)) return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: velocity must be RGBA32F");
@@ -1169,8 +1259,16 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
   } else {
     const int halo = RFX_TRAA_TAIL_ROWS;
-    rfx_status st = rfx_ssgi_compose_launch(ctx, stream, &ch->traa.compose, f->depth, composed, f->direct_light, &ch->traa_k5,
-                                            (uint32_t)std::max(0, kr.r0 - halo), (uint32_t)std::min(H, kr.r1 + halo));
+    rfx_status st = RFX_OK;
+    rfx_ssgi_compose_params q = ch->traa.compose;
+    const rfx_plane* view = composed;
+    if (debug && st == RFX_OK) {
+      q.is_debug = 1;
+      st = debug_view_plane(ch, stream, f, &view);
+    }
+    if (st == RFX_OK)
+      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &ch->traa_k5, (uint32_t)std::max(0, kr.r0 - halo),
+                                   (uint32_t)std::min(H, kr.r1 + halo));
     TemporalPeer tpeer{};  // in a row-sharded group of n > 1 the TRAA history is read on the rank that owns each row
     tpeer.hist0 = tpeer.hist1 = ch->traa_acc.view[prev];
     if (st == RFX_OK)

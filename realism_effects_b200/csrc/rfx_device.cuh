@@ -138,9 +138,13 @@ RFX_D float mod_gl(float x, float y) { return x - y * floorf(__fdiv_rn(x, y)); }
 // float2color(...).r / .g  = roughness / metalness  (:24-34,189-191)
 RFX_D float gb_roughness(float b) { return fmaxf(mod_gl(b, 257.0f) / 256.0f - RFX_NON_ZERO_OFFSET, 0.0f); }
 RFX_D float gb_metalness(float b) { return fmaxf(floorf(__fdiv_rn(b, 257.0f * 257.0f)) / 256.0f - RFX_NON_ZERO_OFFSET, 0.0f); }
+// EXACT_EXP2: exp2 rounded from double, as the oracle's exp2cr (oracle/glsl.h).  fExp is never an integer (floatToVec4 subtracts 1e-4),
+// where exp2f may be 2 ulp off; the G-buffer debug view shows the decoded value itself and takes the exact form.
+template <bool EXACT_EXP2 = false>
 RFX_D v3 decodeRGBE8(v4 rgbe) {  // :136-141
   float fExp = rgbe.w * 255.0f - 128.0f;
-  return xyz(rgbe) * exp2f(fExp);
+  if constexpr (EXACT_EXP2) return xyz(rgbe) * (float)exp2((double)fExp);
+  else return xyz(rgbe) * exp2f(fExp);
 }
 RFX_D void unpackTwoVec4(float4 e, v4& a, v4& b) {  // :85-98
   v2 p = unpackHalf2x16(__float_as_uint(e.x)), q = unpackHalf2x16(__float_as_uint(e.y));

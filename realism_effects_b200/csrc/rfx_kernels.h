@@ -142,6 +142,24 @@ RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
   }
   return mk4(c, 1.0f);
 }
+// K5 with isDebug for the views ssgi_compose_kernel does not fetch (its debug branch reads an RGBA32F plane of the output's size):
+// `gi` of any size and format, sampled at the pixel centre with its own sampler.
+struct SsgiComposeDebugArgs {
+  PV gi;
+  int gi_fmt;  // RFX_FMT_R32F (a depth texture: (d, 0, 0, 1)), RFX_FMT_RGBA16F (LINEAR), RFX_FMT_RGBA32F (NEAREST)
+  OutV out;
+  int W, H, row0, row1;
+};
+cudaError_t launch_ssgi_compose_debug(const SsgiComposeDebugArgs& a, cudaStream_t s);
+
+// GBufferDebugPass (k_post.cu)
+struct GbufferDebugArgs {
+  PV gb;
+  OutV out;
+  int W, H, row0, row1;
+  int mode;
+};
+cudaError_t launch_gbuffer_debug(const GbufferDebugArgs& a, cudaStream_t s);
 
 // ---- K2 ----------------------------------------------------------------------------------
 struct TemporalArgs {

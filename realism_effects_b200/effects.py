@@ -16,6 +16,7 @@ What stands in for three.js / postprocessing objects:
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 
 import numpy as np
@@ -89,6 +90,32 @@ class _Reactive:
 
 
 # ---------------------------------------------------------------------------------------------------
+def _debug_state(value):
+    """What SSGIEffect's outputTexture setter does with `value` (src/ssgi/SSGIEffect.js:228-251): None for a falsy value (the setter returns
+    early), ("gbuffer", mode) for a string (GBufferDebugPass mode = its index in the mode list, -1 when unknown, which shows emissive),
+    ("texture", None) for a plane"""
+    if value is None or (isinstance(value, str) and not value):
+        return None
+    if isinstance(value, str):
+        return ("gbuffer", abi.GBUFFER_DEBUG_MODES.index(value) if value in abi.GBUFFER_DEBUG_MODES else -1)
+    return ("texture", None)
+
+
+def _plane_ptr(p) -> int:
+    return int((p.p if hasattr(p, "p") else p).ptr or 0)
+
+
+class _ChainTexture(abi.Plane):
+    """Chain output `which` of one effect as an object that outlives the chain: the effect refreshes its fields from the current chain
+    whenever it hands it out, so a host can hold it across setSize / resolutionScale changes and set it back (the reference's
+    denoiser.texture is one object for the effect's life)."""
+
+    def __init__(self, owner, which: int):
+        super().__init__()
+        self.owner, self.which = owner, which
+
+
+# ---------------------------------------------------------------------------------------------------
 class VelocityDepthNormalPass:
     """src/temporal-reproject/pass/VelocityDepthNormalPass.js:66-194.  The reference rasterises the scene into
     (uv motion, packed oct normal, depth); here the plane is supplied by the host (`scene.velocity`)."""
@@ -130,7 +157,12 @@ class SSGIEffect(_Reactive):
     """new SSGIEffect(composer, scene, camera, options)   (src/ssgi/SSGIEffect.js:27-141; signature per D6)
 
     update() runs K1 -> K2 -> K3 x 2*denoiseIterations -> K4 natively (rfx_ssgi_chain) and then K5 into
-    composer.outputBuffer.  `outputTexture` is the composed GI plane (RGBA32F)."""
+    composer.outputBuffer.  `outputTexture` is the composed GI plane (RGBA32F), the denoiser's texture.
+
+    Debug views (SSGIEffect.js:228-251): setting `outputTexture` to another plane the host holds (a chain output, scene.depth, scene.velocity,
+    scene.gbuffer) makes K5 show that plane (isDebug); setting it to one of abi.GBUFFER_DEBUG_MODES (an unknown string shows emissive) renders
+    that G-buffer channel with GBufferDebugPass after the chain every frame and shows its target, which the getter then returns.  Setting the
+    denoiser's texture back ends debug mode; a falsy value is ignored.  No view resets the temporal history."""
 
     DefaultOptions = defaultSSGIOptions
 
@@ -157,6 +189,10 @@ class SSGIEffect(_Reactive):
         self._blue_start = int(opts.pop("blueNoiseStart", 1234567))
         self._last_cam = None
         self._chain = None
+        self._chain_textures = [_ChainTexture(self, n) for n in range(6)]  # chainTexture(n); 0 is the denoiser's texture
+        self._view = None  # debug view: None (the denoiser's texture), ("output", n), ("plane", plane) or ("gbuffer", mode)
+        self.gBufferDebugTarget = None
+        self.isDebug = False
         self._options = opts
         self.setSize(composer.width, composer.height)
 
@@ -189,6 +225,51 @@ class SSGIEffect(_Reactive):
         if self._chain is not None:
             self._chain.close()
         self._chain = engine.SsgiChain(self.ctx, self._chain_options())
+        if self.gBufferDebugTarget is not None:  # GBufferDebugPass.setSize at the effect's size
+            self.gBufferDebugTarget.free()
+            self.gBufferDebugTarget = self.ctx.alloc(abi.FMT_RGBA32F, *self._size)
+
+    def __setattr__(self, k, v):
+        if k == "outputTexture":  # SSGIEffect.js:228-251: no reset(), unlike the other setters
+            self._set_output_texture(v)
+        else:
+            super().__setattr__(k, v)
+
+    def _set_output_texture(self, v):
+        st = _debug_state(v)
+        if st is None:
+            return
+        kind, mode = st
+        if kind == "gbuffer":
+            if self.gBufferDebugTarget is None:
+                self.gBufferDebugTarget = self.ctx.alloc(abi.FMT_RGBA32F, *self._size)
+            self._view = ("gbuffer", mode)
+        elif v is not self.gBufferDebugTarget:
+            if isinstance(v, _ChainTexture) and v.owner is self:
+                n = v.which
+            else:
+                ptr = _plane_ptr(v)
+                if ptr == 0 or (isinstance(v, engine.DevPlane) and not v.owned):
+                    raise abi.RfxError("SSGIEffect.outputTexture: the plane has been freed")
+                # a chain plane is looked up again every frame: the fast chain re-splits trOut / dnB when they are read
+                n = next((i for i in range(6) if _plane_ptr(self._chain.output(i)) == ptr), None)
+            if self.gBufferDebugTarget is not None:
+                self.gBufferDebugTarget.free()
+                self.gBufferDebugTarget = None
+            self._view = None if n == 0 else ("output", n) if n is not None else ("plane", v)
+        self.isDebug = self._view is not None
+
+    def chainTexture(self, which: int) -> abi.Plane:
+        """chain output `which` (0 the denoiser's texture, 1 ssgiOut, 2/3 trOut, 4/5 dnB) as a texture that stays valid across setSize"""
+        t, p = self._chain_textures[which], self._chain.output(which)
+        C.memmove(C.addressof(t), C.addressof(p), C.sizeof(abi.Plane))
+        return t
+
+    def _view_plane(self):
+        if self._view is None:
+            return self.chainTexture(0)
+        kind, x = self._view
+        return self.gBufferDebugTarget if kind == "gbuffer" else self.chainTexture(x) if kind == "output" else x
 
     def _option_changed(self, k):
         if k == "resolutionScale":
@@ -214,7 +295,7 @@ class SSGIEffect(_Reactive):
 
     @property
     def outputTexture(self):
-        return self._chain.output(0)
+        return self._view_plane()
 
     def update(self, renderer=None, inputBuffer=None, deltaTime=None):
         cam_u = self._camera.uniforms()
@@ -224,8 +305,14 @@ class SSGIEffect(_Reactive):
         scene_buf = inputBuffer if inputBuffer is not None else self.composer.inputBuffer
         self._chain.render(abi.make_camera(cam_u), self._scene.depth, self._scene.gbuffer, self.velocityDepthNormalPass.texture,
                            scene_buf if self.isUsingRenderPass else None, cam_u["position"], moved)
+        if self._view is not None and self._view[0] == "gbuffer":  # GBufferDebugPass renders after SSGIPass (SSGIEffect.js:398-399)
+            self.ctx.gbuffer_debug(self._view[1], self._scene.gbuffer, self.gBufferDebugTarget)
         if getattr(self.composer, "outputBuffer", None) is not None:  # both modes: SSR composes with inputType "specular" (Denoiser.js:56-64)
-            self.ctx.ssgi_compose(self._scene.depth, self.outputTexture, scene_buf, self.composer.outputBuffer, params=self._compose_params(cam_u))  # K5 (mainImage of the effect)
+            params = self._compose_params(cam_u)
+            if self.isDebug:  # ssgi_compose.frag:21-24: the view itself, with its own sampler
+                params = params or abi.SsgiComposeParams()
+                params.is_debug = 1
+            self.ctx.ssgi_compose(self._scene.depth, self.outputTexture, scene_buf, self.composer.outputBuffer, params=params)  # K5 (mainImage of the effect)
 
     def _compose_params(self, cam_u):
         """scene.fog -> the fog uniforms of ssgi_compose.frag (src/ssgi/SSGIEffect.js:80-90, 404-412); fog = dict(color, near, far) or
@@ -244,6 +331,9 @@ class SSGIEffect(_Reactive):
         if self._chain is not None:
             self._chain.close()
             self._chain = None
+        if self.gBufferDebugTarget is not None:
+            self.gBufferDebugTarget.free()
+            self.gBufferDebugTarget = None
 
 
 class SSREffect(SSGIEffect):

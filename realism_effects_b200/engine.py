@@ -187,7 +187,8 @@ class Context:
                                                  rows[0], rows[1]))
 
     def ssgi_compose(self, depth, gi, scene, out, rows=(0, 0), stream=None, params=None):
-        """params: abi.SsgiComposeParams (scene fog / isDebug) or None"""
+        """params: abi.SsgiComposeParams (scene fog / isDebug) or None.  With params.is_debug, gi is the debug view: any R32F, RGBA16F or
+        RGBA32F plane of any size (depth / scene are not read and may be None)"""
         self._chk(self.lib.rfx_ssgi_compose_launch(self.h, stream, C.byref(params) if params is not None else None, _r(depth), _r(gi), _r(scene), _r(out),
                                                    rows[0], rows[1]))
 
@@ -201,6 +202,10 @@ class Context:
 
     def motion_blur(self, p, velocity, inp, out, rows=(0, 0), stream=None):
         self._chk(self.lib.rfx_motion_blur_launch(self.h, stream, C.byref(p), _r(velocity), _r(inp), _r(out), rows[0], rows[1]))
+
+    def gbuffer_debug(self, mode, gbuffer, out, rows=(0, 0), stream=None):
+        """GBufferDebugPass: channel `mode` (abi.GBUFFER_DEBUG_MODES index; any other value shows emissive) of the packed G-buffer, RGBA32F"""
+        self._chk(self.lib.rfx_gbuffer_debug_launch(self.h, stream, int(mode), _r(gbuffer), _r(out), rows[0], rows[1]))
 
     def traa_compose(self, acc, out, rows=(0, 0), stream=None):
         self._chk(self.lib.rfx_traa_compose_launch(self.h, stream, _r(acc), _r(out), rows[0], rows[1]))
@@ -255,6 +260,10 @@ class SsgiChain:
             return
         self.traa = options if options is not None else abi.make_traa_tail_options()
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_enable_traa(self.h, C.byref(self.traa)))
+
+    def set_debug_view(self, view: int):
+        """the TRAA tail's K5 shows `view` (abi.DEBUG_VIEW_*; include/rfx.h: rfx_ssgi_chain_set_debug_view) instead of composed"""
+        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_set_debug_view(self.h, int(view)))
 
     @staticmethod
     def _frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved) -> abi.SsgiFrame:
