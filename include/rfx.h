@@ -174,6 +174,25 @@ typedef struct rfx_hbao_params {
                                 AOPass.js:79-83); {0, 0}: the out plane's size                                    */
 } rfx_hbao_params;
 
+/* K6h  horizon-march AO   an extension: the reference has no such draw (its hbao.frag takes cosine-hemisphere samples, SURVEY.md D1).
+ *      The per-sample horizon form of Bavoil, Sainz and Dimitrov, "Image-Space Horizon-Based Ambient Occlusion" (SIGGRAPH 2008): D
+ *      screen-space directions x S steps per pixel; same inputs and output layout as K6. */
+typedef struct rfx_hbao_horizon_params {
+  float projection[16];          /* camera.projectionMatrix: row 4 gives the clip w of the pixel, [5] the vertical scale          */
+  float projection_inverse[16];
+  float camera_matrix_world[16];
+  float view_matrix[16];         /* camera.matrixWorldInverse; used only with a normal plane                                      */
+  float resolution[2];           /* the AO target's UNROUNDED size (as rfx_hbao_params.resolution); {0, 0}: the out plane's size */
+  float distance;                /* world-space radius, > 0                                                                      */
+  float angle_bias;              /* subtracted from each tap's cosine, [0, 1)                                                    */
+  float intensity;               /* >= 0                                                                                          */
+  float max_radius_pixels;       /* the projected radius is clamped to this many texels, >= 1                                     */
+  int32_t directions;            /* 1..32                                                                                         */
+  int32_t steps;                 /* 1..64                                                                                         */
+  int32_t blue_noise_index;      /* != 0                                                                                          */
+  int32_t _pad[3];
+} rfx_hbao_horizon_params;
+
 /* K7  AO compose   src/ao/shader/ao_compose.frag:6-16 */
 typedef struct rfx_ao_compose_params {
   float power;
@@ -357,6 +376,20 @@ rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
 rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
                               const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
                               uint32_t row0, uint32_t row1);
+
+/* K6h. Horizon-march AO.  No reference draw exists for it: the reference's hbao.frag has no direction x step loop (SURVEY.md D1),
+ * so this pass is an extension, written to the definition in DESIGN.md §1 (K6h) and pinned by tests/horizon_oracle.cpp.
+ * Inputs and output are K6's: depth R32F; out RGBA16F (rgb = world normal, a = ao), no larger than depth, background pixels not
+ * written; normal NULL (rebuilt from 9 depth taps) or an RGBA8 view-space normal plane of depth's size.  Per pixel: D directions
+ * theta_d = 2 pi (d + blue.r / 255) / D, S steps of r / (S + 1) texels (r = the projected `distance`, clamped to max_radius_pixels)
+ * jittered by blue.g / 255, one NEAREST depth tap each; ao = clamp(1 - intensity * mean(term), 0, 1).
+ * RFX_ERR_BAD_FORMAT / RFX_ERR_SIZE_MISMATCH for the planes, RFX_ERR_INVALID_ARG for a parameter outside its documented range,
+ * RFX_ERR_UNSUPPORTED for blue_noise_index 0 (as K6). */
+rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_horizon_params* p,
+                                   const rfx_plane* depth, const rfx_plane* out, const rfx_plane* normal);
+/* K6h's direction table for `directions` (1..32), built on the host: out[2 * (d * 256 + b) + {0, 1}] = (cos, sin) of
+ * theta = 2 pi (d + b / 255) / directions, evaluated in double and rounded to float.  256 * directions pairs. */
+rfx_status rfx_hbao_horizon_directions(int32_t directions, float* out);
 
 /* K7. ao RGBA16F (.a; any size: sampled LINEAR by uv, e.g. a reduced-resolution AO target), input/out RGBA16F */
 rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p,

@@ -458,6 +458,59 @@ function checkAoScale(s) {
 HBAOEffect.DefaultOptions = defaultAOOptions
 
 // -------------------------------------------------------------------------------------------------------------------------
+// HorizonAOEffect: an extension (the reference has no horizon march, SURVEY.md D1).  AOEffect's keys that still mean something, plus
+// the march's own; spp, distancePower, bias and thickness are hbao.frag's and are not carried.
+export const defaultHorizonAOOptions = { resolutionScale: 1, distance: 2, power: 2, color: [0, 0, 0], useNormalPass: false, velocityDepthNormalPass: null,
+	normalTexture: null, directions: 8, steps: 32, angleBias: 0.1, intensity: 1, maxRadiusPixels: 64, ...defaultPoissonBlurOptions
+}
+
+const horizonRanges = {
+	directions: [v => Number.isInteger(v) && v >= 1 && v <= 32, "an integer in 1..32"],
+	steps: [v => Number.isInteger(v) && v >= 1 && v <= 64, "an integer in 1..64"],
+	distance: [v => Number.isFinite(v) && v > 0, "> 0"],
+	angleBias: [v => v >= 0 && v < 1, "in [0, 1)"],
+	intensity: [v => Number.isFinite(v) && v >= 0, ">= 0"],
+	maxRadiusPixels: [v => v >= 1, ">= 1"]
+}
+function checkHorizonOptions(o) {
+	checkAoScale(o.resolutionScale)
+	for (const [k, [ok, what]] of Object.entries(horizonRanges))
+		if (typeof o[k] !== "number" || !ok(o[k])) throw new RangeError(`HorizonAOEffect: ${k} must be ${what}, got ${o[k]}`)
+}
+
+export class HorizonAOEffect extends HBAOEffect {
+	// new HorizonAOEffect(composer, camera, scene, options): HBAOEffect with K6h, the horizon march (directions x steps depth taps per
+	// pixel), in place of hbao.frag; target sizing, normal plane, denoise and compose are HBAOEffect's.  Options are range-checked before
+	// any launch.
+	constructor(composer, camera, scene, options = defaultHorizonAOOptions) {
+		const opts = { ...defaultHorizonAOOptions, ...options }
+		checkHorizonOptions(opts)
+		super(composer, camera, scene, opts)
+		for (const k of ["spp", "distancePower", "bias", "thickness"]) if (!(k in opts)) delete this._options[k]
+	}
+	update(renderer, inputBuffer) {
+		checkHorizonOptions(this._options)
+		const cam = cameraBlock(this._camera)
+		const planes = this.planeSource.read(renderer, { depth: this.composer.depthRenderTarget, velocity: this.velocityDepthNormalPass?.renderTarget, directLight: inputBuffer })
+		if (this.normalPlane) {
+			renderer.readRenderTargetPixels(this.normalTarget, 0, 0, this.normalW, this.normalH, this.normalHost)
+			rfx.planeUpload(this.ctx, this.normalPlane, this.normalHost)
+		}
+		rfx.hbaoHorizon(this.ctx, { projection: f32(this._camera.projectionMatrix), projectionInverse: cam.projectionInverse, matrixWorld: cam.matrixWorld,
+			viewMatrix: f32(this._camera.matrixWorldInverse), resolution: this.resolution, distance: this.distance, angleBias: this.angleBias,
+			intensity: this.intensity, maxRadiusPixels: this.maxRadiusPixels, directions: this.directions, steps: this.steps,
+			blueNoiseIndex: this.index.value }, planes.depth, this.aoPlane, this.normalPlane ?? null)
+		this.denoise.depthPlane = planes.depth; this.denoise.gbufferPlane = planes.velocity; this.denoise.gbufferTexture = false
+		this.denoise.options.inputLinear = true
+		this.denoise.iterations = this._options.iterations
+		this.denoise.render()
+		rfx.aoCompose(this.ctx, { power: this.power, color: this.color }, planes.depth, this.texture, planes.directLight, this.outputPlane)   // ao_compose.frag:6-16
+		rfx.planeDownload(this.ctx, this.outputPlane, this.outputHost)
+	}
+}
+HorizonAOEffect.DefaultOptions = defaultHorizonAOOptions
+
+// -------------------------------------------------------------------------------------------------------------------------
 export class MotionBlurEffect {
 	// new MotionBlurEffect(velocityPass, options) — src/motion-blur/MotionBlurEffect.js:16-102
 	constructor(velocityPass, options = { intensity: 1, jitter: 1, samples: 16 }) {

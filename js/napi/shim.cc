@@ -326,6 +326,20 @@ napi_value Hbao(napi_env env, napi_callback_info info) {  // hbao(ctx, params, d
         "rfx_hbao_launch_ex");
   return undefined(env);
 }
+napi_value HbaoHorizon(napi_env env, napi_callback_info info) {  // hbaoHorizon(ctx, params, depth, out[, normal]); K6h, horizon-march AO
+  ARGS(5); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  Obj b{env, argv[1]};
+  rfx_hbao_horizon_params p{};
+  if (!b.f32("projection", p.projection, 16) || !b.f32("projectionInverse", p.projection_inverse, 16) || !b.f32("matrixWorld", p.camera_matrix_world, 16)) {
+    napi_throw_type_error(env, nullptr, "hbaoHorizon: projection / projectionInverse / matrixWorld"); return nullptr; }
+  p.distance = (float)b.num("distance", 2); p.angle_bias = (float)b.num("angleBias", 0.1); p.intensity = (float)b.num("intensity", 1);
+  p.max_radius_pixels = (float)b.num("maxRadiusPixels", 64);
+  p.directions = (int32_t)b.num("directions", 8); p.steps = (int32_t)b.num("steps", 32); p.blue_noise_index = (int32_t)b.num("blueNoiseIndex", 1);
+  b.floats("viewMatrix", p.view_matrix, 16); b.floats("resolution", p.resolution, 2);  // absent: unused / {0, 0} = the out plane's size
+  CHECK(c, rfx_hbao_horizon_launch(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), unwrap<rfx_plane>(env, argv[4])),
+        "rfx_hbao_horizon_launch");
+  return undefined(env);
+}
 napi_value AoCompose(napi_env env, napi_callback_info info) {  // aoCompose(ctx, {power, color}, depth, ao, input, out)
   ARGS(6); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
   Obj b{env, argv[1]};
@@ -453,7 +467,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("planeUpload", PlaneUpload), FN("planeDownload", PlaneDownload), FN("chainCreate", ChainCreate), FN("chainSetOptions", ChainSetOptions),
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
       FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
-      FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur),
+      FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur),
       FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),
       FN("groupDestroy", GroupDestroy), FN("chainRenderSharded", ChainRenderSharded),

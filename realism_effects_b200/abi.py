@@ -99,6 +99,12 @@ class HbaoParams(C.Structure):
                 ("view_matrix", F16), ("resolution", F2)]
 
 
+class HbaoHorizonParams(C.Structure):
+    _fields_ = [("projection", F16), ("projection_inverse", F16), ("camera_matrix_world", F16), ("view_matrix", F16), ("resolution", F2),
+                ("distance", C.c_float), ("angle_bias", C.c_float), ("intensity", C.c_float), ("max_radius_pixels", C.c_float),
+                ("directions", C.c_int32), ("steps", C.c_int32), ("blue_noise_index", C.c_int32), ("_pad", C.c_int32 * 3)]
+
+
 class AoComposeParams(C.Structure):
     _fields_ = [("power", C.c_float), ("color", F3)]
 
@@ -222,6 +228,8 @@ def _sig(lib):
     lib.rfx_ssgi_compose_launch.argtypes = [vp, vp, _P(SsgiComposeParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_hbao_launch.argtypes = [vp, vp, _P(HbaoParams), PP, PP, u32, u32]
     lib.rfx_hbao_launch_ex.argtypes = [vp, vp, _P(HbaoParams), PP, PP, PP, u32, u32]
+    lib.rfx_hbao_horizon_launch.argtypes = [vp, vp, _P(HbaoHorizonParams), PP, PP, PP]
+    lib.rfx_hbao_horizon_directions.argtypes = [C.c_int32, vp]
     lib.rfx_ao_compose_launch.argtypes = [vp, vp, _P(AoComposeParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_motion_blur_launch.argtypes = [vp, vp, _P(MotionBlurParams), PP, PP, PP, u32, u32]
     lib.rfx_traa_compose_launch.argtypes = [vp, vp, PP, PP, u32, u32]
@@ -274,7 +282,7 @@ EXPORTS = [
     "rfx_blue_noise_set", "rfx_env_set", "rfx_env_clear", "rfx_env_build", "rfx_env_tables_download", "rfx_plane_alloc", "rfx_plane_free", "rfx_plane_clear", "rfx_plane_upload",
     "rfx_plane_download", "rfx_host_alloc", "rfx_host_free", "rfx_format_bytes", "rfx_ssgi_trace_launch",
     "rfx_temporal_reproject_launch", "rfx_poisson_denoise_launch", "rfx_gi_compose_launch", "rfx_ssgi_compose_launch", "rfx_hbao_launch", "rfx_hbao_launch_ex",
-    "rfx_ao_compose_launch", "rfx_motion_blur_launch", "rfx_traa_compose_launch", "rfx_gbuffer_ingest_launch", "rfx_effects_launch", "rfx_taa_launch", "rfx_ssgi_chain_create", "rfx_ssgi_chain_destroy",
+    "rfx_hbao_horizon_launch", "rfx_hbao_horizon_directions", "rfx_ao_compose_launch", "rfx_motion_blur_launch", "rfx_traa_compose_launch", "rfx_gbuffer_ingest_launch", "rfx_effects_launch", "rfx_taa_launch", "rfx_ssgi_chain_create", "rfx_ssgi_chain_destroy",
     "rfx_ssgi_chain_reset", "rfx_ssgi_chain_render", "rfx_ssgi_chain_output", "rfx_ssgi_chain_enable_traa", "rfx_ssgi_chain_render_host",
     "rfx_ssgi_chain_submit_host", "rfx_ssgi_chain_wait_host",
     "rfx_ssgi_chain_set_profiling", "rfx_ssgi_chain_get_profile", "rfx_ssgi_chain_set_options",

@@ -1,4 +1,4 @@
-// k_post.cu — K6 HBAO, K7 AO compose, K8 motion blur, K9 TRAA compose, env mip downsample (sm_90a).
+// k_post.cu — K6 HBAO, K6h horizon-march AO, K7 AO compose, K8 motion blur, K9 TRAA compose, env mip downsample (sm_90a).
 //
 // K6 replaces reference src/ao/AOPass.js:108-109 running src/hbao/shader/hbao.frag:64-96 (+ hbao_utils.glsl,
 // whose stale line-1 include is dropped, SURVEY.md D3); K7 src/ao/shader/ao_compose.frag:6-16;
@@ -9,12 +9,36 @@
 
 namespace rfx {
 
-RFX_D v3 hbao_world_pos(const HbaoArgs& a, float depth, v2 coord) {  // hbao_utils.glsl:19-29
+// K6 and K6h share the world position and the world normal of hbao_utils.glsl (A: HbaoArgs or HbaoHorizonArgs; both carry
+// depth, normal, projection_inverse, camera_matrix_world and view_matrix).
+template <class A>
+RFX_D v3 hbao_world_pos(const A& a, float depth, v2 coord) {  // hbao_utils.glsl:19-29
   const float z = depth * 2.0f - 1.0f;
   const v4 clip = mk4(coord.x * 2.0f - 1.0f, coord.y * 2.0f - 1.0f, z, 1.0f);
   const v4 vs = mul(a.projection_inverse, clip);
   const v4 ws = mul(a.camera_matrix_world, vs);
   return xyz(ws) / ws.w;
+}
+// getWorldNormal (hbao_utils.glsl:46-79): from the normal plane when `use_normal_plane`, else rebuilt from 9 depth taps
+template <class A>
+RFX_D v3 hbao_world_normal(const A& a, v2 vUv, bool use_normal_plane) {
+  if (use_normal_plane) {  // useNormalTexture  hbao_utils.glsl:70-79: RGBA8 NEAREST, unpackRGBToNormal, (vec4(n, 1.) * viewMatrix).xyz
+    const uchar4 t = __ldg((const uchar4*)(a.normal.p + pv_off(a.normal, nearest_i(vUv.x, a.normal.w), nearest_i(vUv.y, a.normal.h), 4)));
+    const v3 n = mk3(2.0f * ((float)t.x / 255.0f) - 1.0f, 2.0f * ((float)t.y / 255.0f) - 1.0f, 2.0f * ((float)t.z / 255.0f) - 1.0f);
+    return normalize(xyz(mul(mk4(n, 1.0f), a.view_matrix)));
+  }
+  // computeWorldNormal  hbao_utils.glsl:46-68: in depth texels (textureSize(depthTexture)); texelFetch clamps at the border
+  const int DW = a.depth.w, DH = a.depth.h;
+  const float sx = (float)DW, sy = (float)DH;
+  const int ix = (int)(vUv.x * sx), iy = (int)(vUv.y * sy);
+  auto D = [&](int dx, int dy) { return ld_r32f(a.depth, clampi(ix + dx, DW), clampi(iy + dy, DH)); };
+  const float c0 = D(0, 0), l2 = D(-2, 0), l1 = D(-1, 0), r1 = D(1, 0), r2 = D(2, 0), b2 = D(0, -2), b1 = D(0, -1), t1 = D(0, 1), t2 = D(0, 2);
+  const float dl = fabsf((2.0f * l1 - l2) - c0), dr = fabsf((2.0f * r1 - r2) - c0);
+  const float db = fabsf((2.0f * b1 - b2) - c0), dt = fabsf((2.0f * t1 - t2) - c0);
+  const v3 ce = hbao_world_pos(a, c0, vUv);
+  const v3 dpdx = (dl < dr) ? ce - hbao_world_pos(a, l1, mk2(vUv.x - 1.0f / sx, vUv.y)) : -ce + hbao_world_pos(a, r1, mk2(vUv.x + 1.0f / sx, vUv.y));
+  const v3 dpdy = (db < dt) ? ce - hbao_world_pos(a, b1, mk2(vUv.x, vUv.y - 1.0f / sy)) : -ce + hbao_world_pos(a, t1, mk2(vUv.x, vUv.y + 1.0f / sy));
+  return normalize(cross(dpdx, dpdy));
 }
 
 // GENERAL = false: the target has the depth plane's size, `resolution` is that size and the normal is rebuilt from depth, so the
@@ -31,24 +55,7 @@ __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoA
   const v4 cp = mul(a.camera_matrix_world, mk4(0.0f, 0.0f, 0.0f, 1.0f));
   const v3 cameraPosition = xyz(cp);
   const v3 worldPos = hbao_world_pos(a, depth, vUv);
-  v3 worldNormal;
-  if (GENERAL && a.normal.p) {  // useNormalTexture  hbao_utils.glsl:70-79: RGBA8 NEAREST, unpackRGBToNormal, (vec4(n, 1.) * viewMatrix).xyz
-    const uchar4 t = __ldg((const uchar4*)(a.normal.p + pv_off(a.normal, nearest_i(vUv.x, a.normal.w), nearest_i(vUv.y, a.normal.h), 4)));
-    const v3 n = mk3(2.0f * ((float)t.x / 255.0f) - 1.0f, 2.0f * ((float)t.y / 255.0f) - 1.0f, 2.0f * ((float)t.z / 255.0f) - 1.0f);
-    worldNormal = normalize(xyz(mul(mk4(n, 1.0f), a.view_matrix)));
-  } else {  // computeWorldNormal  hbao_utils.glsl:46-68: in depth texels (textureSize(depthTexture)); texelFetch clamps at the border
-    const int DW = a.depth.w, DH = a.depth.h;
-    const float sx = (float)DW, sy = (float)DH;
-    const int ix = (int)(vUv.x * sx), iy = (int)(vUv.y * sy);
-    auto D = [&](int dx, int dy) { return ld_r32f(a.depth, clampi(ix + dx, DW), clampi(iy + dy, DH)); };
-    const float c0 = D(0, 0), l2 = D(-2, 0), l1 = D(-1, 0), r1 = D(1, 0), r2 = D(2, 0), b2 = D(0, -2), b1 = D(0, -1), t1 = D(0, 1), t2 = D(0, 2);
-    const float dl = fabsf((2.0f * l1 - l2) - c0), dr = fabsf((2.0f * r1 - r2) - c0);
-    const float db = fabsf((2.0f * b1 - b2) - c0), dt = fabsf((2.0f * t1 - t2) - c0);
-    const v3 ce = hbao_world_pos(a, c0, vUv);
-    const v3 dpdx = (dl < dr) ? ce - hbao_world_pos(a, l1, mk2(vUv.x - 1.0f / sx, vUv.y)) : -ce + hbao_world_pos(a, r1, mk2(vUv.x + 1.0f / sx, vUv.y));
-    const v3 dpdy = (db < dt) ? ce - hbao_world_pos(a, b1, mk2(vUv.x, vUv.y - 1.0f / sy)) : -ce + hbao_world_pos(a, t1, mk2(vUv.x, vUv.y + 1.0f / sy));
-    worldNormal = normalize(cross(dpdx, dpdy));
-  }
+  const v3 worldNormal = hbao_world_normal(a, vUv, GENERAL && a.normal.p);
   // getOcclusion: blueNoise() is re-evaluated with the same index for every sample (A9), so the
   // `spp` samples are identical; the loop is kept (it is what the shader executes) but the sample
   // itself is computed once.
@@ -91,6 +98,59 @@ cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
   if (a.general) hbao_kernel<true><<<grid, 256, 0, s>>>(a);
   else hbao_kernel<false><<<grid, 256, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
+// K6h: horizon-march AO (DESIGN.md §1 K6h; Bavoil, Sainz and Dimitrov 2008, per-sample form).  One thread per pixel walks its D x S
+// taps in order (direction-major), so the sum has the oracle's order.  Texel snapping, the projected radius and the step size are
+// IEEE in both variants; FAST puts the per-tap 1/sqrt(vv) and 1/distance^2 on the SFU.
+template <bool FAST>
+__global__ void __launch_bounds__(256) hbao_horizon_kernel(const __grid_constant__ HbaoHorizonArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.W || y >= a.H) return;
+  const v2 vUv = pixel_uv(x, y, a.W, a.H);
+  const float depth = tex_r32f_nearest(a.depth, vUv);
+  if (depth == 1.0f) return;  // background: the target keeps its texel
+  const v3 P = hbao_world_pos(a, depth, vUv);
+  const v3 N = hbao_world_normal(a, vUv, a.normal.p != nullptr);
+  // projected radius: distance * 0.5 * resolution.y * projection[5] / w_clip of the view position (perspective and orthographic)
+  const v4 vs = mul(a.projection_inverse, mk4(vUv.x * 2.0f - 1.0f, vUv.y * 2.0f - 1.0f, depth * 2.0f - 1.0f, 1.0f));
+  const v3 Pv = xyz(vs) / vs.w;
+  const float w_clip = mul(a.projection, mk4(Pv, 1.0f)).w;
+  const float r_px = a.distance * 0.5f * a.res_y * a.projection.m[5] / w_clip;
+  float ao = 1.0f;
+  if (r_px >= 1.0f) {
+    const float delta = fminf(r_px, a.max_radius_pixels) / (float)(a.steps + 1);
+    const int bx = (int)(vUv.x * a.res_x), by = (int)(vUv.y * a.res_y);  // ivec2(vUv * resolution), K6's blue-noise texel
+    const uchar4 bn = __ldg(a.blue.tex + ((by + a.blue.shift.sy) % a.blue.size) * a.blue.size + ((bx + a.blue.shift.sx) % a.blue.size));
+    const float j = (float)bn.y / 255.0f;
+    const float2* dirs = a.dirs + bn.x;
+    float sum = 0.0f;
+    for (int d = 0; d < a.directions; d++) {
+      const float2 dir = __ldg(dirs + d * 256);
+#pragma unroll 4
+      for (int k = 0; k < a.steps; k++) {
+        const float t = 1.0f + ((float)k + j) * delta;
+        const float ox = floorf(dir.x * t + 0.5f), oy = floorf(dir.y * t + 0.5f);
+        const v2 uv = mk2(vUv.x + ox / a.res_x, vUv.y + oy / a.res_y);
+        const float sd = tex_r32f_nearest(a.depth, uv);
+        const v3 V = hbao_world_pos(a, sd, uv) - P;
+        const float vv = dot(V, V);
+        if (vv > 0.0f) {
+          const float c = (FAST ? dot(N, V) * fx_rsqrt(vv) : dot(N, V) / sqrtf(vv)) - a.angle_bias;
+          const float f = 1.0f - (FAST ? vv * a.inv_dist2 : vv / a.dist2);
+          sum += clampf(c, 0.0f, 1.0f) * clampf(f, 0.0f, 1.0f);
+        }
+      }
+    }
+    ao = clampf(1.0f - a.intensity * sum / (float)(a.directions * a.steps), 0.0f, 1.0f);
+  }
+  st_h4(a.out.p, a.out.pitch, x, y, mk4(N, ao));
+}
+cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s) {
+  dim3 grid((a.W + 31) / 32, (a.H + 7) / 8);
+  if (a.fast) hbao_horizon_kernel<true><<<grid, 256, 0, s>>>(a);
+  else hbao_horizon_kernel<false><<<grid, 256, 0, s>>>(a);
   return cudaGetLastError();
 }
 

@@ -29,6 +29,7 @@ struct rfx_ctx {
   float2* rot_table = nullptr;  // [256]
   float* step_table = nullptr;  // [steps-1][256]
   int step_table_steps = 0;
+  float2* horizon_dirs[33] = {};  // K6h direction table per `directions` value, built on first use and kept (never rewritten)
   // env
   bool env_set = false;
   double env_total = 0.0;  // totalSumValue of the device-built tables (rfx_env_build)
@@ -117,6 +118,7 @@ void rfx_ctx_destroy(rfx_ctx* ctx) {
   cudaFree(ctx->blue);
   cudaFree(ctx->rot_table);
   cudaFree(ctx->step_table);
+  for (float2* t : ctx->horizon_dirs) cudaFree(t);
   cudaFree(ctx->nrd);
   cudaFree(ctx->viewz);
   cudaStreamDestroy(ctx->stream);
@@ -697,6 +699,72 @@ rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p,
   rfx_hbao_params q{};  // the fields before view_matrix only: callers built against the shorter struct pass no more than those
   memcpy(&q, p, offsetof(rfx_hbao_params, view_matrix));
   return rfx_hbao_launch_ex(ctx, stream, &q, depth, nullptr, out, row0, row1);
+}
+
+rfx_status rfx_hbao_horizon_directions(int32_t directions, float* out) {
+  if (directions < 1 || directions > 32 || !out) return RFX_ERR_INVALID_ARG;
+  for (int d = 0; d < directions; d++)
+    for (int b = 0; b < 256; b++) {
+      const double theta = 2.0 * 3.14159265358979323846 * ((double)d + (double)b / 255.0) / (double)directions;
+      out[2 * (d * 256 + b)] = (float)std::cos(theta);
+      out[2 * (d * 256 + b) + 1] = (float)std::sin(theta);
+    }
+  return RFX_OK;
+}
+
+// K6h: horizon-march AO (an extension; no reference draw exists, SURVEY.md D1)
+rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_horizon_params* p, const rfx_plane* depth, const rfx_plane* out,
+                                   const rfx_plane* normal) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: null argument");
+  HbaoHorizonArgs a{};
+  if (!pv(depth, RFX_FMT_R32F, a.depth) || !ov(out, RFX_FMT_RGBA16F, a.out))
+    return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao_horizon: depth R32F, out RGBA16F required");
+  if (normal && !pv(normal, RFX_FMT_RGBA8, a.normal)) return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao_horizon: the normal plane must be RGBA8");
+  a.W = (int)out->width; a.H = (int)out->height;
+  if (a.W > a.depth.w || a.H > a.depth.h)
+    return fail(ctx, RFX_ERR_SIZE_MISMATCH, "hbao_horizon: the output may be smaller than the depth plane, not larger");
+  if (a.normal.p && (a.normal.w != a.depth.w || a.normal.h != a.depth.h))
+    return fail(ctx, RFX_ERR_SIZE_MISMATCH, "hbao_horizon: the normal plane must have the depth plane's size");
+  if (p->directions < 1 || p->directions > 32) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: directions must lie in 1..32");
+  if (p->steps < 1 || p->steps > 64) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: steps must lie in 1..64");
+  if (!(p->distance > 0.0f) || !std::isfinite(p->distance)) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: distance must be > 0");
+  if (!(p->max_radius_pixels >= 1.0f)) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: max_radius_pixels must be >= 1");
+  if (!(p->intensity >= 0.0f) || !std::isfinite(p->intensity)) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: intensity must be >= 0");
+  if (!(p->angle_bias >= 0.0f && p->angle_bias < 1.0f)) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: angle_bias must lie in [0, 1)");
+  const bool res_default = p->resolution[0] == 0.0f && p->resolution[1] == 0.0f;
+  if (!res_default && !(p->resolution[0] > 0.0f && p->resolution[1] > 0.0f))
+    return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: resolution must be positive or {0, 0}");
+  a.res_x = res_default ? (float)a.W : p->resolution[0];
+  a.res_y = res_default ? (float)a.H : p->resolution[1];
+  memcpy(a.projection.m, p->projection, 64);
+  memcpy(a.projection_inverse.m, p->projection_inverse, 64);
+  memcpy(a.camera_matrix_world.m, p->camera_matrix_world, 64);
+  memcpy(a.view_matrix.m, p->view_matrix, 64);
+  a.distance = p->distance;
+  a.dist2 = p->distance * p->distance;
+  a.inv_dist2 = 1.0f / a.dist2;
+  a.angle_bias = p->angle_bias; a.intensity = p->intensity; a.max_radius_pixels = p->max_radius_pixels;
+  a.directions = p->directions; a.steps = p->steps;
+  a.fast = ctx->fast_math;
+  if (p->blue_noise_index == 0) return fail(ctx, RFX_ERR_UNSUPPORTED, "hbao_horizon: blue_noise_index 0 is not used by this pass");
+  rfx_status st = blue_for(ctx, p->blue_noise_index, a.blue);
+  if (st != RFX_OK) return st;
+  float2*& dirs = ctx->horizon_dirs[p->directions];
+  if (!dirs) {  // a fresh allocation no launch has read yet, filled synchronously; kept only once filled
+    std::vector<float> host((size_t)p->directions * 512);
+    rfx_hbao_horizon_directions(p->directions, host.data());
+    float2* t = nullptr;
+    CU(cudaMalloc(&t, host.size() * sizeof(float)));
+    const cudaError_t e = cudaMemcpy(t, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaFree(t);
+      return fail(ctx, RFX_ERR_CUDA, "hbao_horizon: direction table upload failed: %s", cudaGetErrorString(e));
+    }
+    dirs = t;
+  }
+  a.dirs = dirs;
+  LAUNCHED(launch_hbao_horizon(a, pick(ctx, stream)));
+  return RFX_OK;
 }
 
 rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p, const rfx_plane* depth, const rfx_plane* ao,

@@ -243,6 +243,23 @@ struct HbaoArgs {
 };
 cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s);
 
+// K6h: horizon-march AO (an extension; DESIGN.md §1)
+struct HbaoHorizonArgs {
+  PV depth;
+  PV normal;  // RGBA8 view-space normal (NormalPass layout) or p == nullptr: rebuilt from depth
+  OutV out;
+  int W, H;
+  M4 projection, projection_inverse, camera_matrix_world;
+  M4 view_matrix;       // normal texture only
+  float res_x, res_y;   // the target's unrounded size
+  float distance, dist2, inv_dist2, angle_bias, intensity, max_radius_pixels;
+  int directions, steps;
+  int fast;             // SFU sqrt / reciprocal for the per-tap values
+  BlueD blue;
+  const float2* dirs;   // [directions][256] (cos, sin)
+};
+cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s);
+
 struct AoComposeArgs {
   PV depth, ao, input;
   OutV out;

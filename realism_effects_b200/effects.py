@@ -627,6 +627,72 @@ def _check_ao_scale(s):
 
 
 # ---------------------------------------------------------------------------------------------------
+# HorizonAOEffect: AOEffect's keys that still mean something for a horizon march, plus the march's own; spp, distancePower, bias and
+# thickness (read only by hbao.frag's hemisphere samples) are not carried.
+defaultHorizonAOOptions = dict(
+    resolutionScale=1, distance=2, power=2, color=(0.0, 0.0, 0.0), useNormalPass=False, velocityDepthNormalPass=None, normalTexture=None,
+    directions=8, steps=32, angleBias=0.1, intensity=1, maxRadiusPixels=64, **defaultPoissonBlurOptions)
+
+_HORIZON_RANGES = {  # key: (test, what the error says)
+    "directions": (lambda v: isinstance(v, int) and 1 <= v <= 32, "an integer in 1..32"),
+    "steps": (lambda v: isinstance(v, int) and 1 <= v <= 64, "an integer in 1..64"),
+    "distance": (lambda v: math.isfinite(v) and v > 0, "> 0"),
+    "angleBias": (lambda v: 0 <= v < 1, "in [0, 1)"),
+    "intensity": (lambda v: math.isfinite(v) and v >= 0, ">= 0"),
+    "maxRadiusPixels": (lambda v: v >= 1, ">= 1"),
+}
+
+
+def check_horizon_ao_options(o: dict) -> None:
+    """HorizonAOEffect's option ranges (those rfx_hbao_horizon_launch enforces, and resolutionScale in (0, 1]); raises abi.RfxError"""
+    _check_ao_scale(o["resolutionScale"])
+    for k, (ok, what) in _HORIZON_RANGES.items():
+        v = o[k]
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not ok(v):
+            raise abi.RfxError(f"HorizonAOEffect: {k} must be {what}, got {v!r}")
+
+
+class HorizonAOEffect(HBAOEffect):
+    """new HorizonAOEffect(composer, camera, scene, options): HBAOEffect with K6h, the horizon march (directions x steps depth taps per
+    pixel; DESIGN.md §1 K6h), in place of hbao.frag.  An extension: the reference has no such effect (SURVEY.md D1).  The AO target and
+    its resolutionScale, the normal plane (useNormalPass / normalTexture), the one-plane Poisson denoise and ao_compose are HBAOEffect's.
+    Options are reactive and range-checked before any launch."""
+
+    DefaultOptions = defaultHorizonAOOptions
+
+    def __init__(self, composer, camera, scene, options=None):
+        o = {**defaultHorizonAOOptions, **(options or {})}
+        check_horizon_ao_options(o)
+        super().__init__(composer, camera, scene, o)
+        for k in ("spp", "distancePower", "bias", "thickness"):  # HBAOEffect's hemisphere-sample keys: not options of this effect
+            if k not in o:
+                del self._options[k]
+
+    def __setattr__(self, k, v):
+        o = self.__dict__.get("_options")
+        if o is not None and k in _HORIZON_RANGES:
+            check_horizon_ao_options({**o, k: v})
+        super().__setattr__(k, v)
+
+    def update(self, renderer=None, inputBuffer=None, deltaTime=None):
+        o, cam_u = self._options, self._camera.uniforms()
+        p = abi.HbaoHorizonParams()
+        for k in ("projection", "projection_inverse", "camera_matrix_world", "view_matrix"):
+            abi.set_f16(getattr(p, k), cam_u[k])
+        p.resolution[:] = [float(self._resolution[0]), float(self._resolution[1])]
+        p.distance, p.angle_bias, p.intensity, p.max_radius_pixels = o["distance"], o["angleBias"], o["intensity"], o["maxRadiusPixels"]
+        p.directions, p.steps, p.blue_noise_index = int(o["directions"]), int(o["steps"]), self.blueNoiseIndex.value
+        self.ctx.hbao_horizon(p, self._scene.depth, self.aoTarget, normal=self._normal)
+        self.PoissonDenoisePass.setGBufferPass(self._scene.velocity, self._scene.depth, is_gbuffer=False)
+        self.PoissonDenoisePass.render(renderer)
+        if inputBuffer is not None and getattr(self.composer, "outputBuffer", None) is not None:
+            c = abi.AoComposeParams()
+            c.power = o["power"]
+            c.color[:] = [float(x) for x in o["color"]]
+            self.ctx.ao_compose(c, self._scene.depth, self.texture, inputBuffer, self.composer.outputBuffer)
+
+
+# ---------------------------------------------------------------------------------------------------
 class MotionBlurEffect(_Reactive):
     """new MotionBlurEffect(velocityPass, options)  (src/motion-blur/MotionBlurEffect.js:16-102)"""
 

@@ -197,6 +197,11 @@ class Context:
         normal: RGBA8 view-space normal plane (NormalPass layout, p.view_matrix turns it to world space) or None"""
         self._chk(self.lib.rfx_hbao_launch_ex(self.h, stream, C.byref(p), _r(depth), _r(normal), _r(out), rows[0], rows[1]))
 
+    def hbao_horizon(self, p, depth, out, normal=None, stream=None):
+        """K6h, horizon-march AO (abi.HbaoHorizonParams): K6's planes and output layout; normal: RGBA8 view-space normal plane of depth's
+        size or None"""
+        self._chk(self.lib.rfx_hbao_horizon_launch(self.h, stream, C.byref(p), _r(depth), _r(out), _r(normal)))
+
     def ao_compose(self, p, depth, ao, inp, out, rows=(0, 0), stream=None):
         self._chk(self.lib.rfx_ao_compose_launch(self.h, stream, C.byref(p), _r(depth), _r(ao), _r(inp), _r(out), rows[0], rows[1]))
 
