@@ -612,6 +612,72 @@ rfx_status rfx_shard_ranges(uint32_t width, uint32_t height, uint32_t own0, uint
                             int32_t ssgi_mode, uint32_t* ranges, uint32_t n_launches);
 rfx_status rfx_shard_rebalance(const uint32_t* bounds, const uint32_t* measured_bounds, const float* costs, int32_t n, uint32_t* out);
 
+/* ---- AO chain (native mirror of HBAOEffect.update / HorizonAOEffect.update, src/ao/AOEffect.js:148-178): K6 or K6h into the AO
+ *      target -> 2 * iterations Poisson passes (one plane, velocity-layout normals) -> K7 ao_compose, in one call.  Owns the AO target
+ *      and the Poisson targets A / B, and the two blue-noise counters (the AO pass's and the denoiser's, each advanced on every read
+ *      in that order).  The launches and their bytes are exactly those of the per-pass effect classes. -------------------------- */
+typedef struct rfx_ao_chain rfx_ao_chain;
+#define RFX_AO_HBAO 0     /* K6: hbao.frag's spp-sample form */
+#define RFX_AO_HORIZON 1  /* K6h: the horizon march (directions x steps) */
+typedef struct rfx_ao_chain_options {
+  uint32_t width, height;         /* output size = depth / velocity / input / output planes                                    */
+  int32_t algorithm;              /* RFX_AO_*; constructor-time                                                                 */
+  float resolution_scale;         /* (0, 1], 0 = 1: the AO target is (int)(width*s) x (int)(height*s), its `resolution` the
+                                     unrounded product (AOEffect.setSize); constructor-time                                     */
+  int32_t use_normal_plane;       /* 1: frame->normal (RGBA8 view-space normals) replaces the normal rebuilt from depth         */
+  /* K6 (RFX_AO_HBAO) */
+  int32_t spp;
+  float distance;                 /* K6's aoDistance and K6h's world-space radius                                               */
+  float distance_power, bias, thickness;
+  /* K6h (RFX_AO_HORIZON): ranges of rfx_hbao_horizon_params */
+  int32_t directions, steps;
+  float angle_bias, intensity, max_radius_pixels;
+  /* Poisson denoise (PoissonDenoisePass with AOEffect's options) */
+  int32_t iterations;             /* >= 0; 0: K7 composes the AO target                                                         */
+  float radius, phi, luma_phi, depth_phi, normal_phi;
+  /* K7 */
+  float power, color[3];
+  int32_t blue_noise_start;       /* the AO pass's BlueNoiseIndex start                                                         */
+  int32_t denoise_blue_noise_start; /* the denoiser's (PoissonDenoisePass's) start                                              */
+  int32_t _pad;
+} rfx_ao_chain_options;
+typedef struct rfx_ao_frame {
+  float projection[16], projection_inverse[16], camera_matrix_world[16], view_matrix[16];
+  const rfx_plane* depth;         /* R32F, width x height                                                                       */
+  const rfx_plane* velocity;      /* RGBA32F VelocityDepthNormalPass layout: the Poisson taps' normals and depths               */
+  const rfx_plane* normal;        /* RGBA8 view-space normals when use_normal_plane, else ignored                               */
+  const rfx_plane* input;         /* RGBA16F scene colour K7 darkens                                                            */
+  const rfx_plane* output;        /* RGBA16F; NULL skips K7 (and `input` is not read)                                            */
+} rfx_ao_frame;
+rfx_status rfx_ao_chain_create(rfx_ctx* ctx, const rfx_ao_chain_options* opt, rfx_ao_chain** out);
+void rfx_ao_chain_destroy(rfx_ao_chain* chain);
+/* Replaces the per-frame options.  luma_phi / depth_phi / normal_phi that differ from the current option are clamped to >= 1e-4, as
+ * HBAOEffect's setters do (AOEffect.js:106-110); values given at creation are taken as they are.  width, height and resolution_scale
+ * (a size change): RFX_ERR_SIZE_MISMATCH; algorithm: RFX_ERR_UNSUPPORTED (create a new chain). */
+rfx_status rfx_ao_chain_set_options(rfx_ao_chain* chain, const rfx_ao_chain_options* opt);
+/* Back to the state of a new chain: the kept planes are cleared and both blue-noise counters restart (every rank of a group together). */
+rfx_status rfx_ao_chain_reset(rfx_ao_chain* chain);
+rfx_status rfx_ao_chain_render(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);
+/* which: 0 the AO target (RGBA16F, the scaled size), 1 the denoised plane K7 composes (Poisson target B; the AO target with
+ * iterations 0), of the latest frame */
+rfx_status rfx_ao_chain_output(rfx_ao_chain* chain, int32_t which, rfx_plane* out);
+/* Row-sharded AO.  A group takes an AO chain or an SSGI chain, never both (RFX_ERR_INVALID_ARG).  No AO pass reads a produced plane at
+ * an arbitrary uv: K6 / K6h read the caller's depth, the Poisson taps and K7 are bounded stencils, recomputed on widened ranges
+ * (rfx_ao_shard_ranges).  In a group of n > 1 the AO target and Poisson targets A / B are double-buffered by frame parity and
+ * peer-mapped at attach time, and a discarded (background) pixel of K6 / K6h / K3 carries last frame's texel from the rank that owns the
+ * row.  Both algorithms, every iteration count, with or without a normal plane, fast_math on or off.  resolution_scale < 1 (the rows
+ * of a smaller AO target do not map 1:1 onto output rows) and fewer than 64 rows per rank: RFX_ERR_UNSUPPORTED; members whose
+ * algorithm or iterations differ: RFX_ERR_INVALID_ARG.  Results are bit-identical to one rfx_ao_chain. */
+rfx_status rfx_group_attach_ao_chain(rfx_group* group, rfx_ao_chain* chain);  /* collective */
+rfx_status rfx_group_attach_ao_chains_inprocess(rfx_group* const* groups, rfx_ao_chain* const* chains, int32_t world);
+rfx_status rfx_ao_chain_render_sharded(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);  /* collective */
+/* pure host arithmetic: rows [ranges[2k], ranges[2k+1]) of launch k (K6 / K6h, Poisson pass 0 .. 2*iterations-1, K7) for the band
+ * [own0, own1); n_launches = 2 + 2 * iterations.  K7 runs on the band, the last Poisson pass on the band +- 1 row (K7's LINEAR fetch at
+ * the pixel centre; with iterations 0 K6 gets those rows), and every earlier launch on the next one's range widened by the Poisson halo
+ * ceil(|radius| * max(1, height / width)) + 1. */
+rfx_status rfx_ao_shard_ranges(uint32_t width, uint32_t height, uint32_t own0, uint32_t own1, int32_t iterations, float radius,
+                               uint32_t* ranges, uint32_t n_launches);
+
 /* Per-pass device timing (CUDA events recorded on the launching stream around every kernel of
  * the chain).  Slots: 0 K1 trace, 1 K2 temporal, 2 K3 pass 0, 3 K3 passes >= 1, 4 K4 compose.
  * get_profile synchronises the stream, adds the elapsed milliseconds / launch counts of all

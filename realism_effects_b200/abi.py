@@ -168,6 +168,24 @@ class SsgiHostFrame(C.Structure):
                 ("camera_pos", F3), ("camera_moved", C.c_int32), ("out_composed", C.c_void_p)]
 
 
+AO_HBAO, AO_HORIZON = 0, 1  # rfx_ao_chain_options.algorithm: K6 (HBAOEffect) or K6h (HorizonAOEffect)
+
+
+class AoChainOptions(C.Structure):
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("algorithm", C.c_int32), ("resolution_scale", C.c_float),
+                ("use_normal_plane", C.c_int32), ("spp", C.c_int32), ("distance", C.c_float), ("distance_power", C.c_float), ("bias", C.c_float),
+                ("thickness", C.c_float), ("directions", C.c_int32), ("steps", C.c_int32), ("angle_bias", C.c_float), ("intensity", C.c_float),
+                ("max_radius_pixels", C.c_float), ("iterations", C.c_int32), ("radius", C.c_float), ("phi", C.c_float), ("luma_phi", C.c_float),
+                ("depth_phi", C.c_float), ("normal_phi", C.c_float), ("power", C.c_float), ("color", F3), ("blue_noise_start", C.c_int32),
+                ("denoise_blue_noise_start", C.c_int32), ("_pad", C.c_int32)]
+
+
+class AoFrame(C.Structure):
+    _fields_ = [("projection", F16), ("projection_inverse", F16), ("camera_matrix_world", F16), ("view_matrix", F16),
+                ("depth", C.POINTER(Plane)), ("velocity", C.POINTER(Plane)), ("normal", C.POINTER(Plane)), ("input", C.POINTER(Plane)),
+                ("output", C.POINTER(Plane))]
+
+
 def make_camera(u: dict, perspective: "bool | None" = None) -> CameraS:
     """u: dict from synth.Camera.uniforms() (float32 column-major arrays); perspective: camera.isPerspectiveCamera (default: u["perspective"], else True)."""
     if perspective is None:
@@ -274,6 +292,18 @@ def _sig(lib):
     lib.rfx_ssgi_chain_render_sharded.argtypes = [vp, vp, _P(SsgiFrame)]
     lib.rfx_shard_ranges.argtypes = [u32, u32, u32, u32, C.c_int32, C.c_float, C.c_int32, U32P, u32]
     lib.rfx_shard_rebalance.argtypes = [U32P, U32P, _P(C.c_float), C.c_int32, U32P]
+    # AO chain
+    lib.rfx_ao_chain_create.argtypes = [vp, _P(AoChainOptions), _P(vp)]
+    lib.rfx_ao_chain_destroy.argtypes = [vp]
+    lib.rfx_ao_chain_destroy.restype = None
+    lib.rfx_ao_chain_set_options.argtypes = [vp, _P(AoChainOptions)]
+    lib.rfx_ao_chain_reset.argtypes = [vp]
+    lib.rfx_ao_chain_render.argtypes = [vp, vp, _P(AoFrame)]
+    lib.rfx_ao_chain_output.argtypes = [vp, C.c_int32, PP]
+    lib.rfx_group_attach_ao_chain.argtypes = [vp, vp]
+    lib.rfx_group_attach_ao_chains_inprocess.argtypes = [_P(vp), _P(vp), C.c_int32]
+    lib.rfx_ao_chain_render_sharded.argtypes = [vp, vp, _P(AoFrame)]
+    lib.rfx_ao_shard_ranges.argtypes = [u32, u32, u32, u32, C.c_int32, C.c_float, U32P, u32]
 
 
 EXPORTS = [
@@ -290,6 +320,8 @@ EXPORTS = [
     "rfx_group_attach_chain", "rfx_group_get_bounds", "rfx_group_set_bounds", "rfx_group_set_rebalance", "rfx_group_last_costs",
     "rfx_group_begin_frame", "rfx_group_get_last_bounds", "rfx_group_allgather_rows", "rfx_ssgi_chain_render_sharded", "rfx_shard_ranges",
     "rfx_shard_rebalance", "rfx_gbuffer_debug_launch", "rfx_ssgi_chain_set_debug_view",
+    "rfx_ao_chain_create", "rfx_ao_chain_destroy", "rfx_ao_chain_set_options", "rfx_ao_chain_reset", "rfx_ao_chain_render", "rfx_ao_chain_output",
+    "rfx_group_attach_ao_chain", "rfx_group_attach_ao_chains_inprocess", "rfx_ao_chain_render_sharded", "rfx_ao_shard_ranges",
 ]
 
 

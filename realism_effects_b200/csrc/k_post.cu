@@ -45,13 +45,17 @@ RFX_D v3 hbao_world_normal(const A& a, v2 vUv, bool use_normal_plane) {
 // pixel itself addresses the depth texel and the blue noise.  GENERAL = true: the target may be smaller than the depth plane
 // (AOEffect.setSize scales the AO pass by resolutionScale, src/ao/AOEffect.js:126-146) and `resolution` may be fractional; the
 // depth is fetched NEAREST by uv, the blue-noise pixel is ivec2(vUv * resolution) and the normal may come from a normal texture.
-template <bool GENERAL>
-__global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoArgs a) {
+// CARRY (row-sharded AO chain): `out` is double-buffered and a discarded pixel copies last frame's texel from its owner (`c`)
+template <bool GENERAL, bool CARRY>
+__global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoArgs a, const __grid_constant__ PeerPV c) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.W || y >= a.row1) return;
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
   const float depth = GENERAL ? tex_r32f_nearest(a.depth, vUv) : ld_r32f(a.depth, x, y);
-  if (depth == 1.0f) return;  // discard: target keeps its texel
+  if (depth == 1.0f) {  // discard: target keeps its texel
+    if (CARRY) carry_texel<8>(c, a.out, x, y);
+    return;
+  }
   const v4 cp = mul(a.camera_matrix_world, mk4(0.0f, 0.0f, 0.0f, 1.0f));
   const v3 cameraPosition = xyz(cp);
   const v3 worldPos = hbao_world_pos(a, depth, vUv);
@@ -94,23 +98,28 @@ __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoA
   ao = clampf(1.0f - ao, 0.0f, 1.0f);
   st_h4(a.out.p, a.out.pitch, x, y, mk4(worldNormal, ao));
 }
-cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s) {
+cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s, const PeerPV* carry) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
-  if (a.general) hbao_kernel<true><<<grid, 256, 0, s>>>(a);
-  else hbao_kernel<false><<<grid, 256, 0, s>>>(a);
+  const PeerPV c = carry ? *carry : PeerPV{};
+  if (a.general) { if (carry) hbao_kernel<true, true><<<grid, 256, 0, s>>>(a, c); else hbao_kernel<true, false><<<grid, 256, 0, s>>>(a, c); }
+  else { if (carry) hbao_kernel<false, true><<<grid, 256, 0, s>>>(a, c); else hbao_kernel<false, false><<<grid, 256, 0, s>>>(a, c); }
   return cudaGetLastError();
 }
 
 // K6h: horizon-march AO (DESIGN.md §1 K6h; Bavoil, Sainz and Dimitrov 2008, per-sample form).  One thread per pixel walks its D x S
 // taps in order (direction-major), so the sum has the oracle's order.  Texel snapping, the projected radius and the step size are
 // IEEE in both variants; FAST puts the per-tap 1/sqrt(vv) and 1/distance^2 on the SFU.
-template <bool FAST>
-__global__ void __launch_bounds__(256) hbao_horizon_kernel(const __grid_constant__ HbaoHorizonArgs a) {
-  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= a.W || y >= a.H) return;
+// CARRY: as hbao_kernel's
+template <bool FAST, bool CARRY>
+__global__ void __launch_bounds__(256) hbao_horizon_kernel(const __grid_constant__ HbaoHorizonArgs a, const __grid_constant__ PeerPV c) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.W || y >= a.row1) return;
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
   const float depth = tex_r32f_nearest(a.depth, vUv);
-  if (depth == 1.0f) return;  // background: the target keeps its texel
+  if (depth == 1.0f) {  // background: the target keeps its texel
+    if (CARRY) carry_texel<8>(c, a.out, x, y);
+    return;
+  }
   const v3 P = hbao_world_pos(a, depth, vUv);
   const v3 N = hbao_world_normal(a, vUv, a.normal.p != nullptr);
   // projected radius: distance * 0.5 * resolution.y * projection[5] / w_clip of the view position (perspective and orthographic)
@@ -147,10 +156,11 @@ __global__ void __launch_bounds__(256) hbao_horizon_kernel(const __grid_constant
   }
   st_h4(a.out.p, a.out.pitch, x, y, mk4(N, ao));
 }
-cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s) {
-  dim3 grid((a.W + 31) / 32, (a.H + 7) / 8);
-  if (a.fast) hbao_horizon_kernel<true><<<grid, 256, 0, s>>>(a);
-  else hbao_horizon_kernel<false><<<grid, 256, 0, s>>>(a);
+cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s, const PeerPV* carry) {
+  dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
+  const PeerPV c = carry ? *carry : PeerPV{};
+  if (a.fast) { if (carry) hbao_horizon_kernel<true, true><<<grid, 256, 0, s>>>(a, c); else hbao_horizon_kernel<true, false><<<grid, 256, 0, s>>>(a, c); }
+  else { if (carry) hbao_horizon_kernel<false, true><<<grid, 256, 0, s>>>(a, c); else hbao_horizon_kernel<false, false><<<grid, 256, 0, s>>>(a, c); }
   return cudaGetLastError();
 }
 

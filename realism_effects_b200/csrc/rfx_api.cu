@@ -665,9 +665,11 @@ rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_co
   return RFX_OK;
 }
 
-rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
-                              uint32_t row0, uint32_t row1) {
-  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: null argument");
+}  // extern "C"
+
+// K6 over output rows [r0, r1); carry: as poisson_denoise's, `out` (the AO chain in a row-sharded group)
+static rfx_status hbao(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
+                       uint32_t row0, uint32_t row1, const PeerPV* carry = nullptr) {
   HbaoArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !ov(out, RFX_FMT_RGBA16F, a.out)) return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao: depth R32F, out RGBA16F required");
   if (normal && !pv(normal, RFX_FMT_RGBA8, a.normal)) return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao: the normal plane must be RGBA8");
@@ -690,8 +692,16 @@ rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params*
   if (st != RFX_OK) return st;
   if (p->blue_noise_index == 0) return fail(ctx, RFX_ERR_UNSUPPORTED, "hbao: blue_noise_index 0 is not used by this pass");
   a.rot_table = ctx->rot_table;
-  LAUNCHED(launch_hbao(a, pick(ctx, stream)));
+  LAUNCHED(launch_hbao(a, pick(ctx, stream), carry));
   return RFX_OK;
+}
+
+extern "C" {
+
+rfx_status rfx_hbao_launch_ex(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* normal, const rfx_plane* out,
+                              uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao: null argument");
+  return hbao(ctx, stream, p, depth, normal, out, row0, row1);
 }
 
 rfx_status rfx_hbao_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_params* p, const rfx_plane* depth, const rfx_plane* out, uint32_t row0, uint32_t row1) {
@@ -712,10 +722,11 @@ rfx_status rfx_hbao_horizon_directions(int32_t directions, float* out) {
   return RFX_OK;
 }
 
-// K6h: horizon-march AO (an extension; no reference draw exists, SURVEY.md D1)
-rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_horizon_params* p, const rfx_plane* depth, const rfx_plane* out,
-                                   const rfx_plane* normal) {
-  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: null argument");
+}  // extern "C"
+
+// K6h: horizon-march AO (an extension; no reference draw exists, SURVEY.md D1) over output rows [r0, r1) (0, 0: all); carry: as hbao's
+static rfx_status hbao_horizon(rfx_ctx* ctx, void* stream, const rfx_hbao_horizon_params* p, const rfx_plane* depth, const rfx_plane* out,
+                               const rfx_plane* normal, uint32_t row0, uint32_t row1, const PeerPV* carry = nullptr) {
   HbaoHorizonArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !ov(out, RFX_FMT_RGBA16F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "hbao_horizon: depth R32F, out RGBA16F required");
@@ -745,6 +756,7 @@ rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_ho
   a.inv_dist2 = 1.0f / a.dist2;
   a.angle_bias = p->angle_bias; a.intensity = p->intensity; a.max_radius_pixels = p->max_radius_pixels;
   a.directions = p->directions; a.steps = p->steps;
+  rows(row0, row1, out->height, a.row0, a.row1);
   a.fast = ctx->fast_math;
   if (p->blue_noise_index == 0) return fail(ctx, RFX_ERR_UNSUPPORTED, "hbao_horizon: blue_noise_index 0 is not used by this pass");
   rfx_status st = blue_for(ctx, p->blue_noise_index, a.blue);
@@ -763,13 +775,13 @@ rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_ho
     dirs = t;
   }
   a.dirs = dirs;
-  LAUNCHED(launch_hbao_horizon(a, pick(ctx, stream)));
+  LAUNCHED(launch_hbao_horizon(a, pick(ctx, stream), carry));
   return RFX_OK;
 }
 
-rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p, const rfx_plane* depth, const rfx_plane* ao,
-                                 const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1) {
-  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_compose: null argument");
+// K7 over output rows [r0, r1) (0, 0: all)
+static rfx_status ao_compose(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p, const rfx_plane* depth, const rfx_plane* ao,
+                             const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1) {
   AoComposeArgs a{};
   if (!pv(depth, RFX_FMT_R32F, a.depth) || !pv(ao, RFX_FMT_RGBA16F, a.ao) || !pv(input, RFX_FMT_RGBA16F, a.input) || !ov(out, RFX_FMT_RGBA16F, a.out))
     return fail(ctx, RFX_ERR_BAD_FORMAT, "ao_compose: depth R32F, ao/input/out RGBA16F required");
@@ -781,6 +793,20 @@ rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compos
   memcpy(a.color, p->color, 12);
   LAUNCHED(launch_ao_compose(a, pick(ctx, stream)));
   return RFX_OK;
+}
+
+extern "C" {
+
+rfx_status rfx_hbao_horizon_launch(rfx_ctx* ctx, void* stream, const rfx_hbao_horizon_params* p, const rfx_plane* depth, const rfx_plane* out,
+                                   const rfx_plane* normal) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "hbao_horizon: null argument");
+  return hbao_horizon(ctx, stream, p, depth, out, normal, 0, 0);
+}
+
+rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compose_params* p, const rfx_plane* depth, const rfx_plane* ao,
+                                 const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_compose: null argument");
+  return ao_compose(ctx, stream, p, depth, ao, input, out, row0, row1);
 }
 
 rfx_status rfx_motion_blur_launch(rfx_ctx* ctx, void* stream, const rfx_motion_blur_params* p, const rfx_plane* velocity, const rfx_plane* input,
@@ -1717,5 +1743,186 @@ rfx_status rfx_ssgi_chain_render_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
 }
 
 }  // extern "C"
+
+// ==========================================================================================
+// native AO chain: HBAOEffect.update / HorizonAOEffect.update (K6 or K6h -> K3 x 2*iterations -> K7) in one call
+// ==========================================================================================
+struct rfx_ao_chain {
+  rfx_ctx* ctx;
+  rfx_ao_chain_options opt;
+  float luma_phi, depth_phi, normal_phi;  // the denoiser's values: opt's, clamped where a setter changed them (AOEffect.js:106-110)
+  // the planes a frame leaves for the next (a discarded pixel keeps its texel): alone single-buffered (buffer 0, rendered in place);
+  // buffer 1 is added by a group of n > 1 (group_alloc_history)
+  HistPlane target, dnA, dnB;
+  int32_t bn_ao = 0, bn_dn = 0;  // the AO pass's and the denoiser's BlueNoiseIndex
+  struct rfx_group* group = nullptr;
+  bool group_peer = false;  // attached to a group of n > 1: double-buffered planes, carry instantiations
+};
+static int pass_latest(const rfx_ao_chain* ch);  // the buffer of every plane that holds the latest frame (rfx_group.inl)
+
+static void ao_target_size(const rfx_ao_chain_options& o, uint32_t& w, uint32_t& h, float& rx, float& ry) {
+  const double s = o.resolution_scale == 0.0f ? 1.0 : (double)o.resolution_scale;
+  const double fw = (double)o.width * s, fh = (double)o.height * s;  // AOEffect.setSize: setSize(width * scale, height * scale)
+  w = (uint32_t)fw; h = (uint32_t)fh;
+  rx = (float)fw; ry = (float)fh;  // uniform `resolution`: the unrounded product
+}
+
+extern "C" {
+
+rfx_status rfx_ao_chain_create(rfx_ctx* ctx, const rfx_ao_chain_options* opt, rfx_ao_chain** out) {
+  if (!ctx || !opt || !out || opt->width == 0 || opt->height == 0 || opt->iterations < 0) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_create: bad arguments");
+  if (opt->algorithm != RFX_AO_HBAO && opt->algorithm != RFX_AO_HORIZON) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_create: algorithm must be RFX_AO_HBAO or RFX_AO_HORIZON");
+  if (opt->resolution_scale != 0.0f && !(opt->resolution_scale > 0.0f && opt->resolution_scale <= 1.0f))
+    return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_create: resolution_scale must be in (0, 1]");
+  uint32_t tw, th;
+  float rx, ry;
+  ao_target_size(*opt, tw, th, rx, ry);
+  if (tw == 0 || th == 0) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_create: resolution_scale leaves an empty AO target");
+  CU(cudaSetDevice(ctx->device));
+  rfx_ao_chain* ch = new rfx_ao_chain();
+  ch->ctx = ctx;
+  ch->opt = *opt;
+  ch->luma_phi = opt->luma_phi; ch->depth_phi = opt->depth_phi; ch->normal_phi = opt->normal_phi;
+  rfx_status st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, tw, th, &ch->target.buf[0]);
+  for (HistPlane* h : {&ch->dnA, &ch->dnB})
+    if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, opt->width, opt->height, &h->buf[0]);
+  if (st != RFX_OK) { rfx_ao_chain_destroy(ch); return st; }
+  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB}) local_views(*h);
+  *out = ch;
+  return RFX_OK;
+}
+
+void rfx_ao_chain_destroy(rfx_ao_chain* ch) {
+  if (!ch) return;
+  cudaStreamSynchronize(ch->ctx->stream);
+  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
+    for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ch->ctx, &p);
+  delete ch;
+}
+
+rfx_status rfx_ao_chain_set_options(rfx_ao_chain* ch, const rfx_ao_chain_options* opt) {
+  if (!ch || !opt) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (opt->width != ch->opt.width || opt->height != ch->opt.height || opt->resolution_scale != ch->opt.resolution_scale)
+    return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ao_chain_set_options: width, height and resolution_scale size the planes: create a new chain");
+  if (opt->algorithm != ch->opt.algorithm) return fail(ctx, RFX_ERR_UNSUPPORTED, "ao_chain_set_options: the algorithm is a constructor option: create a new chain");
+  if (opt->iterations < 0) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_set_options: iterations < 0");
+  if (opt->luma_phi != ch->opt.luma_phi) ch->luma_phi = std::max(opt->luma_phi, 0.0001f);
+  if (opt->depth_phi != ch->opt.depth_phi) ch->depth_phi = std::max(opt->depth_phi, 0.0001f);
+  if (opt->normal_phi != ch->opt.normal_phi) ch->normal_phi = std::max(opt->normal_phi, 0.0001f);
+  const int32_t s0 = ch->opt.blue_noise_start, s1 = ch->opt.denoise_blue_noise_start;
+  ch->opt = *opt;
+  ch->opt.blue_noise_start = s0;  // the counters keep their start index for the life of the effect
+  ch->opt.denoise_blue_noise_start = s1;
+  return RFX_OK;
+}
+
+rfx_status rfx_ao_chain_reset(rfx_ao_chain* ch) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
+    for (const rfx_plane& p : h->buf)
+      if (p.ptr) CU(cudaMemset2DAsync(p.ptr, p.pitch, 0, (size_t)p.width * 8, p.height, ctx->stream));
+  ch->bn_ao = ch->bn_dn = 0;
+  ch->luma_phi = ch->opt.luma_phi; ch->depth_phi = ch->opt.depth_phi; ch->normal_phi = ch->opt.normal_phi;
+  return RFX_OK;
+}
+
+rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) {
+  if (!ch || !out) return RFX_ERR_INVALID_ARG;
+  if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1");
+  const HistPlane& h = which == 1 && ch->opt.iterations > 0 ? ch->dnB : ch->target;  // AOEffect's `texture`
+  *out = h.buf[h.buf[1].ptr ? pass_latest(ch) : 0];
+  return RFX_OK;
+}
+
+}  // extern "C"
+
+// One frame of the AO chain.  `ranges` == nullptr: whole planes.  Otherwise ranges[2k], ranges[2k+1] = output rows [a,b) of launch k
+// (K6 / K6h, K3 pass 0..2*iterations-1, K7) of this rank's band, widened by the halos the next launches recompute (rfx_ao_shard_ranges).
+static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f, const uint32_t* ranges) {
+  rfx_ctx* ctx = ch->ctx;
+  const rfx_ao_chain_options& o = ch->opt;
+  if (!f->depth || !f->velocity) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: depth and velocity are required");
+  if (o.use_normal_plane && !f->normal) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: use_normal_plane needs frame->normal (RGBA8 view-space normals)");
+  if (f->output && !f->input) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: K7 composes over frame->input: it may not be NULL with an output");
+  if (f->depth->width != o.width || f->depth->height != o.height) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ao_chain: the depth plane must have the chain's size");
+  const rfx_plane* normal = o.use_normal_plane ? f->normal : nullptr;
+  // Alone the chain renders in place.  In a row-sharded group of n > 1 (rfx_group.inl) it writes buffer `wr` and a discarded pixel
+  // carries last frame's texel (buffer `rd`) from the rank that owns the row.
+  const bool peer = ch->group_peer;
+  const int rd = pass_latest(ch), wr = peer ? rd ^ 1 : rd;
+  uint32_t k = 0;
+  rfx_status st;
+  {  // ---- K6 / K6h  AOPass.render (src/ao/AOPass.js:86-110)
+    uint32_t tw, th;
+    float rx, ry;
+    ao_target_size(o, tw, th, rx, ry);
+    const Rows kr = launch_rows(ranges, k, (int)th);
+    const PeerPV* carry = peer ? &ch->target.view[rd] : nullptr;
+    if (o.algorithm == RFX_AO_HBAO) {
+      rfx_hbao_params p{};
+      for (int c = 0; c < 4; c++)  // projectionMatrix * matrixWorldInverse in float64, rounded to fp32 (AOPass.js:93-96)
+        for (int r = 0; r < 4; r++) {
+          double acc = 0.0;
+          for (int i = 0; i < 4; i++) acc += (double)f->projection[i * 4 + r] * (double)f->view_matrix[c * 4 + i];
+          p.projection_view[c * 4 + r] = (float)acc;
+        }
+      memcpy(p.projection_inverse, f->projection_inverse, 64);
+      memcpy(p.camera_matrix_world, f->camera_matrix_world, 64);
+      memcpy(p.view_matrix, f->view_matrix, 64);
+      p.resolution[0] = rx; p.resolution[1] = ry;
+      p.ao_distance = o.distance; p.distance_power = o.distance_power; p.bias = o.bias; p.thickness = o.thickness; p.spp = o.spp;
+      p.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_ao);
+      st = hbao(ctx, stream, &p, f->depth, normal, &ch->target.buf[wr], (uint32_t)kr.r0, (uint32_t)kr.r1, carry);
+    } else {
+      rfx_hbao_horizon_params p{};
+      memcpy(p.projection, f->projection, 64);
+      memcpy(p.projection_inverse, f->projection_inverse, 64);
+      memcpy(p.camera_matrix_world, f->camera_matrix_world, 64);
+      memcpy(p.view_matrix, f->view_matrix, 64);
+      p.resolution[0] = rx; p.resolution[1] = ry;
+      p.distance = o.distance; p.angle_bias = o.angle_bias; p.intensity = o.intensity; p.max_radius_pixels = o.max_radius_pixels;
+      p.directions = o.directions; p.steps = o.steps;
+      p.blue_noise_index = next_blue(o.blue_noise_start, ch->bn_ao);
+      st = hbao_horizon(ctx, stream, &p, f->depth, &ch->target.buf[wr], normal, (uint32_t)kr.r0, (uint32_t)kr.r1, carry);
+    }
+    if (st != RFX_OK) return st;
+  }
+  k++;
+  // ---- K3  PoissonDenoisePass.render with AOEffect's options: one plane, velocity-layout normals, LINEAR input (the RGBA16F AO target)
+  rfx_poisson_params pp{};
+  pp.radius = o.radius; pp.phi = o.phi; pp.luma_phi = ch->luma_phi; pp.depth_phi = ch->depth_phi; pp.normal_phi = ch->normal_phi;
+  pp.texture_count = 1; pp.gbuffer_texture = 0; pp.input_linear = 1;
+  bool decoded = false;
+  for (int i = 0; i < 2 * o.iterations; i++, k++) {
+    const bool horizontal = (i % 2) == 0;
+    HistPlane& inp = i == 0 ? ch->target : (horizontal ? ch->dnB : ch->dnA);
+    HistPlane& outp = horizontal ? ch->dnA : ch->dnB;
+    pp.blue_noise_index = next_blue(o.denoise_blue_noise_start, ch->bn_dn);
+    const Rows kr = launch_rows(ranges, k, (int)o.height);
+    PeerCarry pc{};
+    pc.p[0] = outp.view[rd];  // the target's plane of last frame
+    st = poisson_denoise(ctx, stream, &pp, f->depth, f->velocity, &inp.buf[wr], nullptr, &outp.buf[wr], nullptr, kr.r0, kr.r1, decoded, peer ? &pc : nullptr);
+    if (st != RFX_OK) return st;
+    decoded = true;  // the velocity plane does not change within a frame; the first pass's rows are the widest
+  }
+  // ---- K7  ao_compose.frag over AOEffect's `texture`
+  if (f->output) {
+    rfx_ao_compose_params cp{};
+    cp.power = o.power;
+    memcpy(cp.color, o.color, 12);
+    const Rows kr = launch_rows(ranges, k, (int)o.height);
+    const HistPlane& tex = o.iterations > 0 ? ch->dnB : ch->target;
+    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    if (st != RFX_OK) return st;
+  }
+  return RFX_OK;
+}
+
+extern "C" rfx_status rfx_ao_chain_render(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f) {
+  if (!ch || !f) return RFX_ERR_INVALID_ARG;
+  return ao_render_impl(ch, stream, f, nullptr);
+}
 
 #include "rfx_group.inl"

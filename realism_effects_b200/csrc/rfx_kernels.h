@@ -241,14 +241,14 @@ struct HbaoArgs {
   BlueD blue;
   const float2* rot_table;
 };
-cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s);
+cudaError_t launch_hbao(const HbaoArgs& a, cudaStream_t s, const PeerPV* carry = nullptr);  // carry: as launch_poisson's, `out`
 
 // K6h: horizon-march AO (an extension; DESIGN.md §1)
 struct HbaoHorizonArgs {
   PV depth;
   PV normal;  // RGBA8 view-space normal (NormalPass layout) or p == nullptr: rebuilt from depth
   OutV out;
-  int W, H;
+  int W, H, row0, row1;
   M4 projection, projection_inverse, camera_matrix_world;
   M4 view_matrix;       // normal texture only
   float res_x, res_y;   // the target's unrounded size
@@ -258,7 +258,7 @@ struct HbaoHorizonArgs {
   BlueD blue;
   const float2* dirs;   // [directions][256] (cos, sin)
 };
-cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s);
+cudaError_t launch_hbao_horizon(const HbaoHorizonArgs& a, cudaStream_t s, const PeerPV* carry = nullptr);  // carry: as launch_hbao's
 
 struct AoComposeArgs {
   PV depth, ao, input;

@@ -322,3 +322,82 @@ class SsgiChain:
 
     def wait_host(self, max_in_flight: int = 0):
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_wait_host(self.h, int(max_in_flight)))
+
+
+def ao_chain_options(width: int, height: int, options: dict | None = None, horizon: bool = False) -> abi.AoChainOptions:
+    """rfx_ao_chain_options from HBAOEffect's option table (effects.defaultAOOptions), or HorizonAOEffect's with horizon=True
+    (effects.defaultHorizonAOOptions); missing keys take those defaults.  `blueNoiseStart` is the AO pass's start (the effect's option),
+    `denoiseBlueNoiseStart` the denoiser's (PoissonDenoisePass's, 1234567)."""
+    from . import effects
+
+    o = {**(effects.defaultHorizonAOOptions if horizon else effects.defaultAOOptions), **(options or {})}
+    if horizon:
+        effects.check_horizon_ao_options(o)
+    c = abi.AoChainOptions()
+    c.width, c.height = int(width), int(height)
+    c.algorithm = abi.AO_HORIZON if horizon else abi.AO_HBAO
+    c.resolution_scale = float(o["resolutionScale"])
+    c.use_normal_plane = int(bool(o.get("useNormalPass") or o.get("normalTexture") is not None))
+    c.spp, c.distance = int(o.get("spp", 0)), float(o["distance"])
+    c.distance_power, c.bias, c.thickness = float(o.get("distancePower", 0.0)), float(o.get("bias", 0.0)), float(o.get("thickness", 0.0))
+    c.directions, c.steps = int(o.get("directions", 1)), int(o.get("steps", 1))
+    c.angle_bias, c.intensity, c.max_radius_pixels = float(o.get("angleBias", 0.0)), float(o.get("intensity", 1.0)), float(o.get("maxRadiusPixels", 1.0))
+    c.iterations, c.radius, c.phi = int(o["iterations"]), float(o["radius"]), float(o["phi"])
+    c.luma_phi, c.depth_phi, c.normal_phi = float(o["lumaPhi"]), float(o["depthPhi"]), float(o["normalPhi"])
+    c.power = float(o["power"])
+    c.color[:] = [float(x) for x in o["color"]]
+    c.blue_noise_start = int(o.get("blueNoiseStart", 1234567))
+    c.denoise_blue_noise_start = int(o.get("denoiseBlueNoiseStart", 1234567))
+    return c
+
+
+class AoChain:
+    """Native AO chain (rfx_ao_chain): K6 or K6h -> K3 x 2*iterations -> K7 in one call, the launches of HBAOEffect.update /
+    HorizonAOEffect.update.  Options: ao_chain_options(...)."""
+
+    def __init__(self, ctx: Context, opt: abi.AoChainOptions):
+        self.ctx, self.opt = ctx, opt
+        h = C.c_void_p()
+        ctx._chk(ctx.lib.rfx_ao_chain_create(ctx.h, C.byref(opt), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if self.h:
+            self.ctx.lib.rfx_ao_chain_destroy(self.h)
+            self.h = None
+
+    def reset(self):
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_reset(self.h))
+
+    def set_options(self, opt: abi.AoChainOptions):
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_set_options(self.h, C.byref(opt)))
+        self.opt = opt
+
+    @staticmethod
+    def _frame(cam_u: dict, depth, velocity, normal=None, inp=None, out=None) -> abi.AoFrame:
+        """cam_u: camera uniforms (synth.Camera.uniforms()); planes: DevPlane (or objects with `.p`), normal / inp / out may be None"""
+        f = abi.AoFrame()
+        for k in ("projection", "projection_inverse", "camera_matrix_world", "view_matrix"):
+            abi.set_f16(getattr(f, k), cam_u[k])
+        ptr = lambda p: None if p is None else C.pointer(p.p)  # noqa: E731
+        f.depth, f.velocity, f.normal, f.input, f.output = ptr(depth), ptr(velocity), ptr(normal), ptr(inp), ptr(out)
+        return f
+
+    def render(self, cam_u: dict, depth, velocity, normal=None, inp=None, out=None, stream=None):
+        """one frame; out=None skips K7"""
+        f = self._frame(cam_u, depth, velocity, normal, inp, out)
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_render(self.h, stream, C.byref(f)))
+
+    def output(self, which: int = 1) -> Plane:
+        """0 the AO target, 1 the denoised plane K7 composes (the AO target with iterations 0)"""
+        p = Plane()
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_output(self.h, which, C.byref(p)))
+        return p
+
+    def download(self, which: int = 1) -> np.ndarray:
+        p = self.output(which)
+        out = np.empty((p.height, p.width, 4), np.float16)
+        self.ctx.sync()
+        self.ctx._chk(self.ctx.lib.rfx_plane_download(self.ctx.h, None, C.byref(p), out.ctypes.data_as(C.c_void_p), 0))
+        self.ctx.sync()
+        return out

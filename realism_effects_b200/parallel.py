@@ -1,4 +1,4 @@
-"""Row-band sharding of the SSGI chain across N GPUs (one process per GPU).
+"""Row-band sharding of the SSGI chain and the AO chain across N GPUs (one process per GPU).
 
 The product path is native: `rfx_group_*` / `rfx_ssgi_chain_render_sharded` in csrc/rfx_group.inl (C ABI, include/rfx.h).
 This module is the Python host binding of that API (`ShardedSsgiChain`) plus a pure-Python mirror of its host arithmetic
@@ -161,6 +161,40 @@ class ShardPlan:
         return (0, 4, 5) if self.ssgi_mode else (4,)
 
 
+@dataclass
+class AoShardPlan:
+    """Row ranges [a, b) per launch of one AO chain frame for the band `own`, in chain order: K6 / K6h, K3 pass 0..2*iterations-1, K7
+    (mirror of rfx_ao_shard_ranges).  No AO pass reads a produced plane at an arbitrary uv, so the only cross-row reads are K7's LINEAR
+    fetch at the pixel centre (1 row) and the Poisson taps (the halo of ShardPlan)."""
+
+    width: int
+    height: int
+    own: tuple
+    iterations: int
+    radius: float
+
+    K7_INPUT_ROWS = 1
+
+    @property
+    def poisson_halo(self) -> int:
+        return int(math.ceil(abs(self.radius) * max(1.0, self.height / self.width))) + 1
+
+    @property
+    def n_launches(self) -> int:
+        return 2 + 2 * self.iterations
+
+    @property
+    def ranges(self) -> list:
+        expand = lambda r, rows: (max(0, r[0] - rows), min(self.height, r[1] + rows))  # noqa: E731
+        out = [tuple(self.own)]
+        r = expand(out[0], self.K7_INPUT_ROWS)
+        for _ in range(2 * self.iterations):
+            out.append(r)
+            r = expand(r, self.poisson_halo)
+        out.append(r)
+        return out[::-1]
+
+
 def rebalance(bounds, costs, measured_bounds=None, align: int = 16, min_rows: int = 64, max_share: float = 4.0, damping: float = 0.6):
     """New band borders from per-rank costs (any unit) measured with `measured_bounds` (default: `bounds`).
 
@@ -210,6 +244,27 @@ def _raw_plane(abi, ptr: int, width: int, height: int, pitch: int, fmt: int):
     return p
 
 
+def _group_unique_id(ctx, rank, world, unique_id, dist_group):
+    """(rank, world, 128-byte NCCL unique id): as given, or from torch.distributed (rank 0 makes the id and broadcasts it)"""
+    import ctypes as C
+
+    from . import abi
+
+    if rank is not None and world is not None and unique_id is not None:
+        return rank, world, unique_id
+    import torch.distributed as dist
+
+    rank, world = dist.get_rank(dist_group), dist.get_world_size(dist_group)
+    box = [None]
+    if rank == 0:
+        buf = C.create_string_buffer(abi.GROUP_ID_BYTES)
+        ctx._chk(ctx.lib.rfx_group_get_unique_id(buf))
+        box[0] = bytes(buf.raw)
+    src = dist.get_global_rank(dist_group, 0) if dist_group is not None else 0
+    dist.broadcast_object_list(box, src=src, group=dist_group)
+    return rank, world, box[0]
+
+
 class ShardedSsgiChain:
     """This rank's member of a row-sharded SSGI chain: Python binding of rfx_group_* + rfx_ssgi_chain_render_sharded.
 
@@ -226,18 +281,7 @@ class ShardedSsgiChain:
         from . import abi, engine
 
         self._abi, self.ctx, self.lib, self._C = abi, ctx, ctx.lib, C
-        if rank is None or world is None or unique_id is None:
-            import torch.distributed as dist
-
-            rank, world = dist.get_rank(dist_group), dist.get_world_size(dist_group)
-            box = [None]
-            if rank == 0:
-                buf = C.create_string_buffer(abi.GROUP_ID_BYTES)
-                ctx._chk(self.lib.rfx_group_get_unique_id(buf))
-                box[0] = bytes(buf.raw)
-            src = dist.get_global_rank(dist_group, 0) if dist_group is not None else 0
-            dist.broadcast_object_list(box, src=src, group=dist_group)
-            unique_id = box[0]
+        rank, world, unique_id = _group_unique_id(ctx, rank, world, unique_id, dist_group)
         self.rank, self.world = rank, world
         self.chain = engine.SsgiChain(ctx, chain_options)
         if traa is not None:  # before the attach: the group maps the tail's history plane then
@@ -480,3 +524,71 @@ class InProcessGroup:
             self.lib.rfx_group_destroy(g)
         for ch in self.chains:
             ch.close()
+
+
+class ShardedAoChain(ShardedSsgiChain):
+    """This rank's member of a row-sharded AO chain: rfx_group_* + rfx_ao_chain_render_sharded.  Bands, rebalancing and the unique-id
+    exchange are ShardedSsgiChain's; the host-buffer path is not (out of scope for AO)."""
+
+    def __init__(self, ctx, ao_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
+                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None):
+        import ctypes as C
+
+        from . import abi, engine
+
+        self._abi, self.ctx, self.lib, self._C = abi, ctx, ctx.lib, C
+        self.rank, self.world, unique_id = _group_unique_id(ctx, rank, world, unique_id, dist_group)
+        self.chain = engine.AoChain(ctx, ao_options)
+        g = C.c_void_p()
+        ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, self.rank, self.world, C.byref(g)))
+        self.g = g
+        ctx._chk(self.lib.rfx_group_attach_ao_chain(g, self.chain.h))
+        ctx._chk(self.lib.rfx_group_set_rebalance(g, int(rebalance_every), int(rebalance_lag)))
+        self.rebalance_every = rebalance_every
+        self._host = None
+
+    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, stream=None):
+        """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective."""
+        f = self.chain._frame(cam_u, depth, velocity, normal, inp, out)
+        self.ctx._chk(self.lib.rfx_ao_chain_render_sharded(self.chain.h, stream, self._C.byref(f)))
+
+    def download_band(self, which: int = 1):
+        """this rank's rows of AoChain output `which` of the last frame (numpy)"""
+        b0, b1 = self.band_of_last_frame
+        return self.chain.download(which)[b0:b1]
+
+    def submit_host(self, *a, **k):
+        raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the AO chain has no host-buffer path")
+
+
+class InProcessAoGroup(InProcessGroup):
+    """InProcessGroup for the AO chain (rfx_group_attach_ao_chains_inprocess): every member owns an AoChain with the same options."""
+
+    def __init__(self, ctxs, ao_options, world: int):
+        import ctypes as C
+
+        from . import engine
+
+        self._C, self.world = C, world
+        self.ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs] * world
+        assert len(self.ctxs) == world
+        self.lib = self.ctxs[0].lib
+        self.chains = [engine.AoChain(c, ao_options) for c in self.ctxs]
+        self.groups = []
+        for r, c in enumerate(self.ctxs):
+            g = C.c_void_p()
+            c._chk(self.lib.rfx_group_create_inprocess(c.h, r, world, C.byref(g)))
+            self.groups.append(g)
+        ga = (C.c_void_p * world)(*[g.value for g in self.groups])
+        ca = (C.c_void_p * world)(*[ch.h.value for ch in self.chains])
+        self.ctxs[0]._chk(self.lib.rfx_group_attach_ao_chains_inprocess(ga, ca, world))
+
+    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, wait: bool = True):
+        """one frame: every member renders its band (its rows of `out` too); all of them finish before the next frame starts"""
+        self._last_bounds = self.bounds
+        for c, ch in zip(self.ctxs, self.chains):
+            f = ch._frame(cam_u, depth, velocity, normal, inp, out)
+            c._chk(self.lib.rfx_ao_chain_render_sharded(ch.h, None, self._C.byref(f)))
+        if wait or len(set(self.ctxs)) > 1:
+            for c in set(self.ctxs):
+                c.sync()
