@@ -121,7 +121,7 @@ RFX_D float atan2_poly(float y, float x) {
 
 template <bool AP, bool POLY = false>
 RFX_D v2 equirectDirectionToUv(v3 d) {  // ssgi_utils.frag:64-74
-  v2 uv = POLY ? mk2(atan2_poly(d.z, d.x), acos_poly(d.y)) : mk2(atan2f(d.z, d.x), acosf(d.y));
+  v2 uv = POLY ? mk2(atan2_poly(d.z, d.x), acos_poly(d.y)) : mk2(atan2cr(d.z, d.x), acoscr(d.y));
   uv = mk2(div_<AP>(uv.x, 2.0f * PI_F), div_<AP>(uv.y, PI_F));
   uv.x += 0.5f;
   uv.y = 1.0f - uv.y;
@@ -139,13 +139,13 @@ RFX_D v3 equirectUvToDirection(v2 uv) {  // :77-86
     __sincosf(phi, &sp, &cp);
     return mk3(sp * ct, cp, sp * st);
   }
-  const float sinPhi = sinf(phi);
-  return mk3(sinPhi * cosf(theta), cosf(phi), sinPhi * sinf(theta));
+  const float sinPhi = sincr(phi);
+  return mk3(sinPhi * coscr(theta), coscr(phi), sinPhi * sincr(theta));
 }
 template <bool FAST>
 RFX_D float pow5(float x) {
   if (FAST) { const float x2 = x * x; return x2 * x2 * x; }
-  return powf(x, 5.0f);
+  return powcr(x, 5.0f);
 }
 template <bool FAST>
 RFX_D float F_Schlick1(float f0, float f90, float theta) { return f0 + (f90 - f0) * pow5<FAST>(1.0f - theta); }
@@ -340,7 +340,7 @@ __global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_kernel(const
     const v2 sz = mk2(a.env.size_x, a.env.size_y);
     const v2 ddx = (ux - cdfUv) * sz, ddy = (uy - cdfUv) * sz;
     const float rho = fmaxf(length(ddx), length(ddy));
-    lambda = rho > 0.0f ? (FAST ? lg2a_(rho) : log2f(rho)) : -1000.0f;
+    lambda = rho > 0.0f ? (FAST ? lg2a_(rho) : log2cr(rho)) : -1000.0f;
   }
   if (!active) return;
 
@@ -535,9 +535,9 @@ RFX_D v2 march_fast(const SsgiArgs& a, v3& dir, v3& hitPos, int noiseB, bool& hi
       }
     }
   }
-  if (!hit) {
+  if (!hit) {  // the shader returns the uv of the last step tested; with steps = 1 none is, and its uv keeps (0, 0)
     hitPos = mk3(10.0e9f);
-    return view_to_screen<SPARSE, true>(a, p);
+    return a.steps > 1 ? view_to_screen<SPARSE, true>(a, p) : mk2(0.0f, 0.0f);
   }
   if (a.refine_steps > 0) {
     dir = dir * 0.5f;

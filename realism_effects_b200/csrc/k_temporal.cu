@@ -34,16 +34,16 @@ template <bool LOG, bool FAST>
 RFX_D v3 transformColor(v3 c) {  // reproject.frag:42
   if (!LOG) return c;
   if (FAST) return mk3(t_lg2a(c.x + 1.0f) * T_LN2, t_lg2a(c.y + 1.0f) * T_LN2, t_lg2a(c.z + 1.0f) * T_LN2);
-  return vlog1p_(c);
+  return mk3(logcr(c.x + 1.0f), logcr(c.y + 1.0f), logcr(c.z + 1.0f));
 }
 template <bool LOG, bool FAST>
 RFX_D v3 undoColorTransform(v3 c) {  // :43
   if (!LOG) return c;
   if (FAST) return mk3(t_ex2a(c.x * T_LOG2E) - 1.0f, t_ex2a(c.y * T_LOG2E) - 1.0f, t_ex2a(c.z * T_LOG2E) - 1.0f);
-  return vexpm1_(c);
+  return mk3(expcr(c.x) - 1.0f, expcr(c.y) - 1.0f, expcr(c.z) - 1.0f);
 }
 template <bool FAST>
-RFX_D float tpow(float x, float p) { return FAST ? t_ex2a(p * t_lg2a(x)) : powf(x, p); }
+RFX_D float tpow(float x, float p) { return FAST ? t_ex2a(p * t_lg2a(x)) : powcr(x, p); }
 
 RFX_D float getViewZ(const TemporalArgs& a, float d) {
   return a.cam.perspective ? perspectiveDepthToViewZ(d, a.cam.near_plane, a.cam.far_plane) : orthographicDepthToViewZ(d, a.cam.near_plane, a.cam.far_plane);

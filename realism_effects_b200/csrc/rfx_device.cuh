@@ -8,9 +8,12 @@
 //   cross        fma(a.y, b.z, -(b.y*a.z)) ...
 //   normalize    a * (1/sqrt(dot(a,a)))      (IEEE sqrt + IEEE reciprocal)
 //   division / sqrt: IEEE (-prec-div=true -prec-sqrt=true are nvcc defaults)
-// These are the rules the parity oracle states in oracle/glsl.h; keeping them identical makes
-// every non-transcendental value bit-identical, so parity differences come only from the
-// 1-2 ulp of the device libm (sinf/cosf/expf/logf/powf/atan2f/acosf).
+//   transcendentals of the exact K1 and K2: evaluated in double and rounded once to fp32 (the *cr
+//   functions below), as the oracle does.  The fp32 device libm (sinf/cosf/expf/logf/powf/atan2f/
+//   acosf/log2f) is 1-2 ulp off the correctly rounded value, and one such ulp that crosses an fp16
+//   rounding boundary of K1's packed output changes the output's bits.
+// These are the rules the parity oracle states in oracle/glsl.h; keeping them identical makes the
+// exact K1 and K2 bit-identical to the oracle; elsewhere parity differences come only from the device libm.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -77,6 +80,16 @@ RFX_D float smoothstepf(float e0, float e1, float x) {
 RFX_D v3 vmin(v3 a, v3 b) { return mk3(fminf(a.x, b.x), fminf(a.y, b.y), fminf(a.z, b.z)); }
 RFX_D v3 vmax(v3 a, v3 b) { return mk3(fmaxf(a.x, b.x), fmaxf(a.y, b.y), fmaxf(a.z, b.z)); }
 RFX_D v3 vabs(v3 a) { return mk3(fabsf(a.x), fabsf(a.y), fabsf(a.z)); }
+// correctly rounded fp32 transcendentals (oracle/glsl.h): the double result is within 1-2 double ulps, so rounding it to fp32
+// gives the correctly rounded value except where that value sits within ~1e-16 relative of an fp32 rounding midpoint
+RFX_D float sincr(float x) { return (float)sin((double)x); }
+RFX_D float coscr(float x) { return (float)cos((double)x); }
+RFX_D float expcr(float x) { return (float)exp((double)x); }
+RFX_D float logcr(float x) { return (float)log((double)x); }
+RFX_D float log2cr(float x) { return (float)log2((double)x); }
+RFX_D float powcr(float x, float y) { return (float)pow((double)x, (double)y); }
+RFX_D float atan2cr(float y, float x) { return (float)atan2((double)y, (double)x); }
+RFX_D float acoscr(float x) { return (float)acos((double)x); }
 RFX_D v3 vlog1p_(v3 a) { return mk3(logf(a.x + 1.0f), logf(a.y + 1.0f), logf(a.z + 1.0f)); }   // log(c + 1.)
 RFX_D v3 vexpm1_(v3 a) { return mk3(expf(a.x) - 1.0f, expf(a.y) - 1.0f, expf(a.z) - 1.0f); }   // exp(c) - 1.
 

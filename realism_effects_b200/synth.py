@@ -269,16 +269,21 @@ class Frame:
 
 
 def render_frame(width: int, height: int, t: int = 0, *, device="cpu", cam_step=(0.02, 0.0, 0.0), static=False, fov: float = 40.0,
-                 aspect: float | None = None) -> Frame:
+                 aspect: float | None = None, view_offset=None) -> Frame:
     """Ray-cast frame `t`.  The camera translates by `cam_step` per frame (SURVEY.md §8d); with
     `static=True` it does not move (exercises fullAccumulate).  `fov` = vertical field of view in degrees; `aspect`
-    overrides width/height (non-square pixels: the same view sampled with more rows, used for weak scaling)."""
+    overrides width/height (non-square pixels: the same view sampled with more rows, used for weak scaling).
+    `view_offset(camera, k)`, if given, is called on the camera of frame k (this frame's and the previous one) before anything is
+    projected: a three.js setViewOffset, such as TRAA's sub-pixel jitter or a sub-rectangle of a larger frame (an off-axis frustum)."""
     aspect = width / height if aspect is None else aspect
     step = (0.0, 0.0, 0.0) if static else cam_step
 
     def cam_at(k):
         off = tuple(s * k for s in step)
-        return Camera(fov=fov, aspect=aspect, position=(0.0 + off[0], 8.75 + off[1], 25.0 + off[2]), target=(0.0 + off[0], 8.75 + off[1], 0.0 + off[2]))
+        c = Camera(fov=fov, aspect=aspect, position=(0.0 + off[0], 8.75 + off[1], 25.0 + off[2]), target=(0.0 + off[0], 8.75 + off[1], 0.0 + off[2]))
+        if view_offset is not None:
+            view_offset(c, k)
+        return c
 
     cam, prev = cam_at(t), cam_at(max(t - 1, 0))
     dev = torch.device(device)

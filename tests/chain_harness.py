@@ -79,14 +79,17 @@ class Inputs:
 
 
 def make_inputs(width: int, height: int, n_frames: int, *, static=False, env_size=(128, 64), device="cpu", reference_env=False, fov: float = 40.0,
-                cam_step=(0.02, 0.0, 0.0), orthographic: bool = False) -> Inputs:
+                cam_step=(0.02, 0.0, 0.0), orthographic: bool = False, view_offset=None, blue_size: int = 128) -> Inputs:
     """reference_env: use the reference demo's environment map (synth.load_reference_env, SURVEY.md §8d) instead of the small analytic sky.
     orthographic: the same planes seen through a three.js OrthographicCamera (the shaders' #else branches of PERSPECTIVE_CAMERA): the projection
     matrices are replaced (Matrix4.makeOrthographic), the depth plane is re-encoded so that the view-space z of every texel is kept, and the
-    camera dict carries perspective=False (abi.make_camera reads it)."""
+    camera dict carries perspective=False (abi.make_camera reads it).
+    view_offset: a perspective camera's setViewOffset, called per frame (synth.render_frame), e.g. r2_jitter() or off_axis().
+    blue_size: the blue-noise texture is the top-left blue_size x blue_size crop of the 128 x 128 asset (not a power of two: the
+    kernels' `%` addressing)."""
     frames = []
     for t in range(n_frames):
-        fr = synth.render_frame(width, height, t, device=device, static=static, fov=fov, cam_step=cam_step)
+        fr = synth.render_frame(width, height, t, device=device, static=static, fov=fov, cam_step=cam_step, view_offset=view_offset)
         u = fr.cam.uniforms()
         moved = (t > 0) and not static
         if orthographic:
@@ -99,7 +102,21 @@ def make_inputs(width: int, height: int, n_frames: int, *, static=False, env_siz
     else:
         env = synth.synthetic_env(*env_size)
         marg, cond, total = synth.build_env_cdf(env.astype(np.float32), flip_y=False)
-    return Inputs(width, height, frames, env, marg, cond, total, synth.load_blue_noise())
+    return Inputs(width, height, frames, env, marg, cond, total, np.ascontiguousarray(synth.load_blue_noise()[:blue_size, :blue_size]))
+
+
+def r2_jitter(width: int, height: int):
+    """TRAA's sub-pixel jitter (effects.jitter: the R2 sequence, frame k's offset) as a make_inputs view_offset: projection[8] and [9]
+    become small and non-zero"""
+    from realism_effects_b200 import effects
+
+    return lambda cam, k: effects.jitter(width, height, cam, k)
+
+
+def off_axis(width: int, height: int):
+    """the top-right width x height sub-rectangle of a 1.5x larger frame (setViewOffset, as a tiled or multi-monitor render takes it):
+    projection[8] = 0.5 and projection[9] = 0.5, a strongly off-axis frustum"""
+    return lambda cam, k: cam.setViewOffset(1.5 * width, 1.5 * height, 0.5 * width, 0.0, width, height)
 
 
 def _to_orthographic(u: dict, depth, aspect: float, half_height: float = 11.0):

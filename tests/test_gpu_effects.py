@@ -139,14 +139,17 @@ def test_hbao_effect_traa_effect_motion_blur_effect(built):
         ctx.close()
 
 
-@pytest.mark.parametrize("flip_y", [False, True])
-def test_env_cdf_tables_built_on_device_are_bit_identical(built, flip_y):
+@pytest.mark.parametrize("flip_y,size", [pytest.param(f, (w, h), id=str(f) if (w, h) == (256, 128) else f"{f}-{w}x{h}")
+                                         for w, h in ((256, 128), (100, 50), (37, 19)) for f in (False, True)])
+def test_env_cdf_tables_built_on_device_are_bit_identical(built, flip_y, size):
     """rfx_env_build (SURVEY.md §8f row 1): the device-built marginal / conditional inverse-CDF tables and totalSum equal the
     restatement of `gatherData` (EquirectHdrInfoUniform.js:149-245, synth.build_env_cdf) bit for bit, including the reference's
-    mirroring "un-flip" for flipY textures (A4); and K1 gives the same bytes with either set of tables."""
-    env = synth.synthetic_env(256, 128)
-    env[40:60, 100:140, :3] = 0  # a black patch: flat CDF stretches (ties in the binary search)
-    env[7] = 0                   # an all-black row: cumulativeRowWeight == 0 branch
+    mirroring "un-flip" for flipY textures (A4); and K1 gives the same bytes with either set of tables.  Odd sizes: the flipY mirror
+    has a middle row, and the env map's mip chain has levels of odd size (K1's trilinear fetches)."""
+    w, h = size
+    env = synth.synthetic_env(w, h)
+    env[h * 40 // 128:h * 60 // 128, w * 100 // 256:w * 140 // 256, :3] = 0  # a black patch: flat CDF stretches (ties in the binary search)
+    env[h * 7 // 128] = 0                                                    # an all-black row: cumulativeRowWeight == 0 branch
     marg, cond, total = synth.build_env_cdf(env.astype(np.float32), flip_y=flip_y)
     inp = ch.make_inputs(96, 54, 1)
     ctx = engine.Context(0, inp.blue)
@@ -157,7 +160,7 @@ def test_env_cdf_tables_built_on_device_are_bit_identical(built, flip_y):
         assert np.array_equal(gm.view(np.uint32), marg.view(np.uint32))
         assert np.array_equal(gc.view(np.uint32), cond.view(np.uint32))
         fr = inp.frames[0]
-        p = ch.ssgi_params(ch.Opts(), abi.make_camera(fr["cam"]), 4242, (256, 128))
+        p = ch.ssgi_params(ch.Opts(), abi.make_camera(fr["cam"]), 4242, (w, h))
         planes = [ctx.upload(fr[k]) for k in ("depth", "gbuffer", "direct")]
         out_dev = ctx.alloc(abi.FMT_RGBA32F, 96, 54)
         ctx.ssgi_trace(p, planes[0], planes[1], None, planes[2], None, out_dev)
