@@ -285,7 +285,10 @@ cudaError_t launch_ctemporal(const CTemporalArgs& a, cudaStream_t s) {
 // ------------------------------------------------------------------------------------------------------------------
 // The arithmetic is the exact K4's IEEE division / sqrt (k_denoise.cu: gi_compose_kernel): the two fp16 inputs already sit up to
 // one fp16 ulp (9.8e-4) from the oracle's, so composed pixels crowd the 1e-3 line, and SFU reciprocals were measured to more than
-// double the pixels outside it (DESIGN.md §2).  The pixel-centre fetch is the centre texel and pow(x, 5) is multiplies.
+// double the pixels outside it (DESIGN.md §2).  The perspective viewZ divides once, as perspectiveDepthToViewZ: near depth 1 the
+// denominator cancels, and the reciprocal's second rounding moved composed pixels by up to 70 %.  The pixel-centre fetch is the centre
+// texel (the literal LINEAR fetch would need the neighbours' dn texels, which other blocks of the fused last Poisson pass write; on
+// 3840-wide frames it puts up to 8.8e-4 of the pixels outside 1e-3, tests/test_gpu_compose_options.py) and pow(x, 5) is multiplies.
 RFX_D float4 c_compose(const CamD& cam, int x, int y, int W, int H, float4 g, float rough0, float depth, v3 dgi, v3 sgi) {
   const v2 vUv = pixel_uv(x, y, W, H);
   const v3 diffuse = xyz(floatToVec4(g.x));
@@ -295,8 +298,7 @@ RFX_D float4 c_compose(const CamD& cam, int x, int y, int W, int H, float4 g, fl
   const float fexp = e.w * 255.0f - 128.0f;
   const v3 emissive = xyz(e) * exp2f(fexp);  // decodeRGBE8
   const v3 viewNormal = mul_dir_left(wn, cam.camera_matrix_world);
-  const float gz = cam.perspective ? (cam.near_plane * cam.far_plane) * (1.0f / ((cam.far_plane - cam.near_plane) * depth - cam.far_plane))
-                                   : orthographicDepthToViewZ(depth, cam.near_plane, cam.far_plane);
+  const float gz = cam.perspective ? perspectiveDepthToViewZ(depth, cam.near_plane, cam.far_plane) : orthographicDepthToViewZ(depth, cam.near_plane, cam.far_plane);
   const float viewZ = -gz;
   const float clipW = cam.projection.m[2 * 4 + 3] * viewZ + cam.projection.m[3 * 4 + 3];
   v4 clip = mk4((vUv.x - 0.5f) * 2.0f, (vUv.y - 0.5f) * 2.0f, (viewZ - 0.5f) * 2.0f, 1.0f);

@@ -338,7 +338,8 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
   const v3 diffuse = xyz(floatToVec4(g.x));
   const v3 wn = unpackNormal(g.y);
   const float rough0 = gb_roughness(g.z), metalness = gb_metalness(g.z);
-  const v3 emissive = decodeRGBE8(floatToVec4(g.w));
+  const v4 rgbe = floatToVec4(g.w);
+  const v3 emissive = a.fast ? decodeRGBE8(rgbe) : decodeRGBE8<true>(rgbe);
 
   const v3 viewNormal = mul_dir_left(wn, a.cam.camera_matrix_world);
   const float gz = a.cam.perspective ? perspectiveDepthToViewZ(depth, a.cam.near_plane, a.cam.far_plane)
@@ -351,13 +352,13 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
   v3 viewPos = xyz(mul(a.cam.projection_inverse, clip));
   viewPos.z = -viewZ;
   const v3 viewDir = normalize(viewPos);
-  // pixel-centre fetch of the LINEAR Poisson targets (literal bilinear, like the GL sampler)
-  // exact variant: the literal bilinear fetch a GL sampler performs at the pixel centre; fast variant: the centre texel itself
-  // (the literal weights are (1,0,0,0) up to one ulp of u*W, i.e. the two differ by <= 1.2e-4 x the neighbour contrast)
+  // pixel-centre fetch of the LINEAR Poisson targets: the literal bilinear fetch a GL sampler performs, in both variants.  Its weights
+  // are (1,0,0,0) only up to a few ulps of u*W - 0.5, so the centre texel alone is off by up to ~1e-3 x the neighbour contrast on
+  // wide frames (3840 columns), which GI planes with 64x contrast between neighbours push past the 1e-3 bar.
   // a texture the inputType does not bind is a null sampler: (0,0,0,1)  (DenoiserComposePass.js:23-33)
   const v4 nul = mk4(0.0f, 0.0f, 0.0f, 1.0f);
-  const v4 dgi = !a.diffuse.p ? nul : (a.gi_f32 ? f4v(ld_f4(a.diffuse, x, y)) : (a.fast ? ld_h4(a.diffuse, x, y) : tex_h4_linear(a.diffuse, vUv)));
-  const v4 sgi = !a.specular.p ? nul : (a.gi_f32 ? f4v(ld_f4(a.specular, x, y)) : (a.fast ? ld_h4(a.specular, x, y) : tex_h4_linear(a.specular, vUv)));
+  const v4 dgi = !a.diffuse.p ? nul : (a.gi_f32 ? f4v(ld_f4(a.diffuse, x, y)) : tex_h4_linear(a.diffuse, vUv));
+  const v4 sgi = !a.specular.p ? nul : (a.gi_f32 ? f4v(ld_f4(a.specular, x, y)) : tex_h4_linear(a.specular, vUv));
 
   // constructGlobalIllumination :53-107
   const float roughness = rough0 * rough0;
@@ -384,7 +385,7 @@ __global__ void __launch_bounds__(kThreads) gi_compose_kernel(const __grid_const
   const float VoH = fmaxf(1e-6f, dot(v, h));
   const v3 f0 = mix(mk3(0.04f), diffuse, metalness);
   const float omv = 1.0f - VoH, omv2 = omv * omv;
-  const v3 F = f0 + (mk3(1.0f) - f0) * (a.fast ? omv2 * omv2 * omv : powf(omv, 5.0f));
+  const v3 F = f0 + (mk3(1.0f) - f0) * (a.fast ? omv2 * omv2 * omv : powcr(omv, 5.0f));
   // TYPE_SPECULAR (SSR): the diffuse component is the scene colour (composer input buffer, LINEAR)  denoiser_compose_functions.glsl:97-101
   const v3 diffuseComponent = a.input_type != RFX_INPUT_SPECULAR ? diffuse * (1.0f - metalness) * (mk3(1.0f) - F) * xyz(dgi)
                                                                  : (a.scene.p ? xyz(tex_h4_linear(a.scene, vUv)) : mk3(0.0f));

@@ -136,7 +136,7 @@ RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
     if (a.use_fog) {  // :34-41 + three.js <fog_fragment>
       const float gz = a.perspective ? perspectiveDepthToViewZ(depth, a.camera_near, a.camera_far) : orthographicDepthToViewZ(depth, a.camera_near, a.camera_far);
       const float vFogDepth = -(gz * 0.4f);
-      const float fogFactor = a.fog_exp2 ? 1.0f - expf(-a.fog_density * a.fog_density * vFogDepth * vFogDepth) : smoothstepf(a.fog_near, a.fog_far, vFogDepth);
+      const float fogFactor = a.fog_exp2 ? 1.0f - expcr(-a.fog_density * a.fog_density * vFogDepth * vFogDepth) : smoothstepf(a.fog_near, a.fog_far, vFogDepth);
       c = mix(c, mk3(a.fog_color[0], a.fog_color[1], a.fog_color[2]), fogFactor);
     }
   }

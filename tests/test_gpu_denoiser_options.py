@@ -194,8 +194,9 @@ def test_per_pass_poisson_kernels_match_the_oracle(ctxs, case):
 # (700 W): 0 passes 0; 1 iteration 3.5e-4; 3 iterations 7.9e-4; 5 iterations 9.2e-4 apart from the case below.  Each pass alone is
 # within the per-pass bar (0 pixels out, test above); what grows with the passes is that a pass's output is the next one's input, so
 # a last-bit difference of the fast kernels' SFU lg2 / ex2 from the oracle's libm that flips one fp16 rounding is carried and can
-# flip the next.  (Two residues are not traced to the pixel: 4 pixels of frame 0's `composed` on 120x200, 1.2e-3 off with identical
-# dn inputs, and up to 9 pixels of dn0 on 80x320 at radius 11 with all weights 0.)
+# flip the next.  (Up to 9 pixels of dn0 on 80x320 at radius 11 with all weights 0 are not traced to the pixel.  Frame 0's `composed`
+# on 120x200 had 4 pixels 1.2e-3 off in 15 cases while c_compose formed the perspective viewZ with a reciprocal; with one division, as
+# perspectiveDepthToViewZ, those 15 cases have none, H100 80GB HBM3, 700 W.)
 CHAIN_BAR = {0: PER_PASS_BAR, 1: 5e-4, 3: 1e-3, 5: 1e-3}
 # Measured 1.37e-3 (33 pixels of dn1, frame 0).  18 of them are flat pixels whose every tap weight is cut (w < 0.0001) by the large
 # weights, so each pass writes fp16(1.0003 * c) (the centre's factor, poisson_denoise.frag); near c = 1.6276 that product is half an fp16

@@ -11,6 +11,8 @@ import torch
 
 import chain_harness as ch
 from realism_effects_b200 import abi
+from test_compose_options_cpu import K5_CASES
+from test_march_options_cpu import make_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -26,30 +28,24 @@ def _options(fog, cam_u):
     return abi.make_traa_tail_options(compose=ch.fog_params(cam_u, exp2=False) if fog else None)
 
 
-@pytest.mark.parametrize("size", [(320, 192), (3840, 2160)])
-@pytest.mark.parametrize("fog", [False, True])
-def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
-    """4 frames with history and a reset before frame 2: the fast chain's fused tail (outputs 6 / 7) == ssgi_compose -> temporal_reproject
-    (TRAA form, RGBA16F history, LINEAR) -> traa_compose launched one by one on the chain's own `composed`, byte for byte, every frame.
-    At the small size a chain without the tail runs alongside: outputs 0..5 are byte-identical with and without it."""
+def _tail_equals_per_pass_sequence(ctx, inp, o, topt, name, reset_at=None, with_plain=False):
+    """Renders inp.frames with the fast chain's fused tail; every frame, outputs 6 / 7 == ssgi_compose -> temporal_reproject (TRAA form,
+    RGBA16F history, LINEAR) -> traa_compose launched one by one on the chain's own `composed`, byte for byte.  reset_at: the frame
+    before which the chain is reset.  with_plain: a chain without the tail runs alongside, and outputs 0..5 must be byte-identical.
+    Returns the last frame's output 6."""
     from realism_effects_b200 import engine
 
-    W, H = size
-    o = ch.Opts(denoise_iterations=1 if W > 1000 else 2)
-    inp = ch.make_inputs(W, H, 4, device="cuda" if W > 1000 else "cpu")
-    ctx = engine.Context(0, inp.blue)
+    W, H = inp.width, inp.height
+    copt = ch.chain_options(inp, o)
+    chain = engine.SsgiChain(ctx, copt)
+    plain = engine.SsgiChain(ctx, copt) if with_plain else None
+    k5, out = ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)
+    acc = [ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)]
     try:
-        ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
-        copt = ch.chain_options(inp, o)
-        chain = engine.SsgiChain(ctx, copt)
-        topt = _options(fog, inp.frames[0]["cam"])
         chain.enable_traa(topt)
-        plain = engine.SsgiChain(ctx, copt) if W < 1000 else None
-        k5, out = ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)
-        acc = [ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)]
         keep, prev = 0.0, None
         for t, fr in enumerate(inp.frames):
-            if t == 2:
+            if t == reset_at:
                 chain.reset()
                 if plain is not None:
                     plain.reset()
@@ -64,19 +60,55 @@ def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
             ctx.traa_compose(acc[t & 1], out)
             keep, prev = 1.0, fr["cam"]
             got6, got7 = chain.download(6), chain.download(7)
-            assert got7.tobytes() == acc[t & 1].download().tobytes(), (t, "TRAA accumulated plane")
-            assert got6.tobytes() == out.download().tobytes(), (t, "K9 output")
+            assert got7.tobytes() == acc[t & 1].download().tobytes(), (name, t, "TRAA accumulated plane")
+            assert got6.tobytes() == out.download().tobytes(), (name, t, "K9 output")
             assert np.isfinite(got6).all() and (got6[..., 3] == 1).all()
             if plain is not None:
                 plain.render(cam, *planes, fr["cam"]["position"], fr["moved"])
                 for which in range(6):
-                    assert chain.download(which).tobytes() == plain.download(which).tobytes(), (t, which)
+                    assert chain.download(which).tobytes() == plain.download(which).tobytes(), (name, t, which)
             for p in planes:
                 p.free()
-        assert np.abs(got6[..., :3].astype(np.float32)).max() > 0.05
+        return got6
+    finally:
         chain.close()
         if plain is not None:
             plain.close()
+        for q in [k5, out] + acc:
+            q.free()
+
+
+@pytest.mark.parametrize("size", [(320, 192), (3840, 2160)])
+@pytest.mark.parametrize("fog", [False, True])
+def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
+    """4 frames with history and a reset before frame 2: the fused tail writes the bytes of the per-pass sequence every frame.  At the
+    small size a chain without the tail runs alongside: outputs 0..5 are byte-identical with and without it."""
+    from realism_effects_b200 import engine
+
+    W, H = size
+    inp = ch.make_inputs(W, H, 4, device="cuda" if W > 1000 else "cpu")
+    ctx = engine.Context(0, inp.blue)
+    try:
+        ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
+        got6 = _tail_equals_per_pass_sequence(ctx, inp, ch.Opts(denoise_iterations=1 if W > 1000 else 2), _options(fog, inp.frames[0]["cam"]),
+                                              f"{size} fog={fog}", reset_at=2, with_plain=W < 1000)
+        assert np.abs(got6[..., :3].astype(np.float32)).max() > 0.05
+    finally:
+        ctx.close()
+
+
+@pytest.mark.parametrize("case", K5_CASES, ids=str)
+def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence_across_k5_options(built, case):
+    """3 frames at each point of the SSGI compose grid (tests/test_compose_options_cpu.py: no fog, linear fog and FogExp2 with
+    perspective and orthographic cameras, isDebug, odd sizes and a 3840x16 strip) as the tail's compose options: the fused tail
+    (ctraa_kernel, which shares ssgi_compose_px with ssgi_compose_kernel) writes the bytes of the per-pass sequence every frame"""
+    from realism_effects_b200 import engine
+
+    inp = make_inputs(case.W, case.H, case.camera, frames=3)
+    ctx = engine.Context(0, inp.blue)
+    try:
+        ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
+        _tail_equals_per_pass_sequence(ctx, inp, ch.Opts(), abi.make_traa_tail_options(compose=case.params(inp.frames[0]["cam"])), str(case))
     finally:
         ctx.close()
 

@@ -257,9 +257,10 @@ def np_normalize(a):
     return a / np.linalg.norm(a, axis=-1, keepdims=True)
 
 
-def np_gi_compose(cam: dict, depth, gbuffer, dgi, sgi, prev):
+def np_gi_compose(cam: dict, depth, gbuffer, dgi, sgi, prev, flips: list | None = None):
     """DenoiserComposePass.js:58-85 + constructGlobalIllumination (denoiser_compose_functions.glsl:53-107), inputType DIFFUSE_SPECULAR.
-    cam: synth camera uniforms (column-major 4x4 arrays)."""
+    cam: synth camera uniforms (column-major 4x4 arrays).  flips: if a list, the mask of the composed pixels that take the
+    `dot(viewNormal, l) < 0` flip is appended to it."""
     H, W = depth.shape
     M = lambda k: np.asarray(cam[k], np.float64).reshape(4, 4).T  # noqa: E731  column-major -> numpy row-major
     P, Pinv, Mw, V = M("projection"), M("projection_inverse"), M("camera_matrix_world"), M("view_matrix")
@@ -306,7 +307,10 @@ def np_gi_compose(cam: dict, depth, gbuffer, dgi, sgi, prev):
     l = np_normalize(inc - 2.0 * (Hh * inc).sum(-1, keepdims=True) * Hh)   # reflect(-V, H)
     l = l[..., 0:1] * T + l[..., 1:2] * B + l[..., 2:3] * N
     l = np_normalize(rot_left(l, Mw))  # (vec4(l, 1.) * cameraMatrixWorld).xyz: the translation row only feeds .w
-    l = np.where(((view_normal * l).sum(-1) < 0.0)[..., None], -l, l)
+    flip = (view_normal * l).sum(-1) < 0.0
+    if flips is not None:
+        flips.append(flip & ~discard)
+    l = np.where(flip[..., None], -l, l)
     h = np_normalize(vv + l)
     # GLSL max(x, y) = (x < y) ? y : x.  With roughness 0 on a back-facing texel H = normalize(0) is NaN, the comparison with
     # NaN is false and max(EPSILON, NaN) returns EPSILON - the shader's output there is finite (F ~ 1), and so is the oracle's.
