@@ -5,10 +5,11 @@
 // the colour is handed from one mainImage() to the next.  effects_kernel is that merged shader, selected at run time: up to four
 // effects in caller order, one read of the frame, one write — instead of one full-frame round trip per effect.  HBM traffic is
 // 8 B/px in + 8 B/px out (+ 4 depth / + 16 velocity when used); the 3x3 and bilinear taps of the input are L1 / L2 hits.
-// Arithmetic is IEEE fp32 with libm transcendentals, except where the shader itself amplifies the last bit: the hash of SparkleEffect
-// (fract(sin(x) * 43758.5)) and pow(noise, 500 * spread) turn a one-ulp difference of sin() into a different sparkle pattern, so those two
-// are evaluated in double and rounded once (what "correctly rounded" means for the parity oracle); TAAPass re-evaluates its sRGB curve in
-// double only for the ~0.4 % of texels whose 8-bit rounding is within 2e-3 of a tie.
+// Arithmetic is IEEE fp32, and every transcendental of the effects is evaluated in double and rounded once (rfx_device.cuh's sincr /
+// expcr / powcr, what "correctly rounded" means for the parity oracle), so effects_kernel is bit-equal to the oracle.  A libm fp32 call
+// 1-2 ulp off would not stay small here: the hash of SparkleEffect (fract(sin(x) * 43758.5)) and pow(noise, 500 * spread) turn a one-ulp
+// difference of sin() into a different sparkle pattern.  TAAPass takes its sRGB curve on the SFU and re-evaluates it in double only for
+// the ~0.4 % of texels whose 8-bit rounding is within 2e-3 of a tie.
 #include "rfx_device.cuh"
 #include "rfx_kernels.h"
 
@@ -16,9 +17,9 @@ namespace rfx {
 
 namespace {
 
-RFX_D float sincr(float x) { return (float)sin((double)x); }
-RFX_D float powcr(float x, float y) { return (float)pow((double)x, (double)y); }
 RFX_D v4 add4(v4 a, v4 b) { return mk4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+// powcr(x, 4.) without the double pow: x * x is exact in double, so d * d is x^4 rounded once to double, as pow returns it
+RFX_D float pow4cr(float x) { const double d = (double)x * (double)x; return (float)(d * d); }
 
 // SharpnessEffect.js:8-29
 RFX_D v4 fx_sharpness(const PV& in, v4 inputColor, v2 uv, v2 ts, float sharp) {
@@ -68,7 +69,12 @@ RFX_D v4 fx_gradual_background(const EffectsArgs& a, v4 inputColor, int x, int y
   const v3 viewPos = view_position(a.cam, uv, view_z(a.cam, a.cam.perspective != 0, depth));
   const v3 worldPos = xyz(mul(a.cam.camera_matrix_world, mk4(viewPos, 1.0f)));
   const float distToCenter = length(mk2(worldPos.x, worldPos.z)) + fmaxf(0.0f, -worldPos.y);
-  const float fade = clampf(powf(distToCenter, 0.1f) * 15.0f - a.max_distance, 0.0f, 1.0f);  // libm fp32 (<= 2 ulp): not amplified
+  // pow(distToCenter, 0.1) is taken in double (powcr) only where the clamp may not saturate: elsewhere the fp32 powf (a few ulps, far
+  // inside the 1e-5 margin) already puts the fade at 0 or 1, and so would the exact value
+  const float p15 = powf(distToCenter, 0.1f) * 15.0f, margin = 1e-5f * (p15 + fabsf(a.max_distance));
+  float g = p15 - a.max_distance;
+  if (g > -margin && g < 1.0f + margin) g = powcr(distToCenter, 0.1f) * 15.0f - a.max_distance;
+  const float fade = clampf(g, 0.0f, 1.0f);
   const v3 c = mix(xyz(inputColor), mk3(a.bg[0], a.bg[1], a.bg[2]), fade);
   return mk4(c, 1.0f);
 }
@@ -97,9 +103,9 @@ RFX_D v4 fx_sparkle(const EffectsArgs& a, v4 inputColor, int x, int y, v2 uv) {
   if (worldPos.y < 0.01f) return inputColor;
   const v3 cameraPos = xyz(mul(a.cam.camera_matrix_world, mk4(0.0f, 0.0f, 0.0f, 1.0f)));
   const float dist = length(worldPos - cameraPos);
-  const float distFactor = expf(-dist * 0.005f);
+  const float distFactor = expcr(-dist * 0.005f);
   float facing = fmaxf(dot(-viewDir, viewNormal), 0.0f);
-  facing = powf(facing, 4.0f);
+  facing = pow4cr(facing);
   const v3 nw = normalize(worldPos);
   const v2 offset = mk2(nw.x, nw.z) * 1000.0f + mk2(normal.x, normal.z) * 500.0f;
   float noise = nn(offset);
@@ -108,7 +114,7 @@ RFX_D v4 fx_sparkle(const EffectsArgs& a, v4 inputColor, int x, int y, v2 uv) {
   lum = smoothstepf(0.15f, 1.0f, lum);
   const float sparkleFactor = noise * lum * facing * distFactor * 5000.0f * a.intensity;
   const v3 c = xyz(inputColor);
-  const v3 color = c + mk3(powf(c.x, 4.0f), powf(c.y, 4.0f), powf(c.z, 4.0f)) * sparkleFactor;
+  const v3 color = c + mk3(pow4cr(c.x), pow4cr(c.y), pow4cr(c.z)) * sparkleFactor;
   return mk4(color, 1.0f);
 }
 
@@ -131,10 +137,12 @@ __global__ void __launch_bounds__(256) effects_kernel(const __grid_constant__ Ef
 
 // three r151 LinearTosRGB (encodings_pars_fragment)
 // EXACT = false: v^0.41666 on the SFU (ex2(0.41666 * lg2(v)), relative error ~1e-6, i.e. < 3e-4 of an 8-bit step — two orders inside the
-// tie window that triggers the exact re-evaluation below)
+// tie window that triggers the exact re-evaluation below).  As pow, it is NaN for a negative v (lg2 of a negative number is NaN) and 0
+// for +-0 (lg2 gives -inf, ex2 of it 0); mix() carries the NaN even where v <= 0.0031308 selects the linear segment, so a negative
+// channel ends at 0 after the clamp whatever the history holds.
 template <bool EXACT>
 RFX_D float linear_to_srgb(float v) {
-  const float pw = EXACT ? powcr(v, 0.41666f) : (v > 0.0f ? fx_ex2(0.41666f * fx_lg2(v)) : 0.0f);
+  const float pw = EXACT ? powcr(v, 0.41666f) : fx_ex2(0.41666f * fx_lg2(v));
   const float hi = pw * 1.055f - 0.055f, lo = v * 12.92f;
   return mixf(hi, lo, v <= 0.0031308f ? 1.0f : 0.0f);
 }

@@ -74,7 +74,10 @@ __global__ void __launch_bounds__(256) hbao_kernel(const __grid_constant__ HbaoA
     const v3 t = cross(b, worldNormal);
     sampleWorldDir = normalize(r * sc.x * b + sqrtf(1.0f - ux) * worldNormal + r * sc.y * t);
   }
-  const v3 sampleWorldPos = worldPos + a.ao_distance * powf(bz, a.distance_power + 1.0f) * sampleWorldDir;
+  // pow(blueNoise.z, distancePower + 1.): at the default distancePower = 1, bz * bz is powcr(bz, 2) bit for bit (the square of an fp32
+  // value is exact in double, so both round it to fp32 once) without the double pow
+  const float dp = a.distance_power + 1.0f;
+  const v3 sampleWorldPos = worldPos + a.ao_distance * (dp == 2.0f ? bz * bz : powcr(bz, dp)) * sampleWorldDir;
   const v4 suv4 = mul(a.projection_view, mk4(sampleWorldPos, 1.0f));
   const v2 sq = mk2(suv4.x, suv4.y) / suv4.w;
   const v2 suv = mk2(sq.x * 0.5f + 0.5f, sq.y * 0.5f + 0.5f);
@@ -170,7 +173,7 @@ __global__ void __launch_bounds__(256) ao_compose_kernel(const __grid_constant__
   const v2 uv = pixel_uv(x, y, a.W, a.H);
   const float unpackedDepth = ld_r32f(a.depth, x, y);
   float ao = unpackedDepth > 0.9999f ? 1.0f : tex_h4_linear(a.ao, uv).w;
-  ao = powf(ao, a.power);
+  ao = a.power == 2.0f ? ao * ao : powcr(ao, a.power);  // the default power 2: ao * ao is powcr(ao, 2) bit for bit, as in hbao_kernel
   const v3 aoColor = mix(mk3(a.color[0], a.color[1], a.color[2]), mk3(1.0f), ao);
   const v4 in = tex_h4_linear(a.input, uv);
   st_h4(a.out.p, a.out.pitch, x, y, mk4(aoColor * xyz(in), in.w));

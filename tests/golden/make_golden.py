@@ -10,7 +10,7 @@ the CUDA engine against them.  Inputs are stored with the outputs so the fixture
   chain_ssr_64x36.npz  SSR chain (mode "ssr": 1-plane K2/K3, TYPE_SPECULAR compose), 3 frames
   reference_pins.json  every reference-shader call of the pinning tests (tests/test_reference_glsl.py, tests/test_ingest_cpu.py,
                        tests/test_denoiser_options_cpu.py, tests/test_march_options_cpu.py,
-                       tests/test_compose_options_cpu.py), in
+                       tests/test_compose_options_cpu.py, tests/test_post_options_cpu.py), in
                        call order (tests/refpins.py); minting runs those tests against the live shaders, so it also checks them
   reference_js_tables.json  the option tables and the export list of the reference's JS (tests/test_host_logic.py)
 """
@@ -87,6 +87,7 @@ def mint_pins():
     import test_host_logic
     import test_ingest_cpu
     import test_march_options_cpu
+    import test_post_options_cpu
     import test_reference_glsl as t
 
     refpins.MINT = True
@@ -99,6 +100,7 @@ def mint_pins():
     test_denoiser_options_cpu.test_oracle_equals_reference_shaders_denoiser_option_space()
     test_march_options_cpu.test_oracle_equals_reference_shaders_march_options()
     test_compose_options_cpu.test_oracle_equals_reference_shaders_compose_options()
+    test_post_options_cpu.test_oracle_equals_reference_shaders_post_options()
     test_ingest_cpu.test_oracle_ingest_equals_the_reference_packgbuffer_glsl()
     path = refpins.save()
     print("wrote", path, os.path.getsize(path), "bytes")

@@ -7,6 +7,7 @@ same call runs on the oracle (tests/orc.py, same signatures) and its outputs mus
 reference, bit for bit, on any machine.
 
     R = refpins.ref("tag")        # stands in for the refglsl module: R.hbao(...), ch.run_oracle_chain(..., impl=R)
+    R.arrays(ours, reference)     # a call through another harness: ours() on the oracle, reference() on the shaders when minting
     refpins.done(R)               # exactly the recorded calls were made
 """
 from __future__ import annotations
@@ -63,6 +64,20 @@ class _Ref:
             return r
 
         return call
+
+    def arrays(self, ours, reference):
+        """one call through a harness other than tests/orc.py (e.g. tests/ao_harness.py), recorded like a pass call: `ours()` runs the
+        oracle; in minting `reference()` runs the reference's shaders and must give the same bytes"""
+        i = len(self.calls)
+        r = ours()
+        got = ["arrays", digest(r)]
+        if MINT:
+            assert digest(reference()) == got[1], f"{self.tag}: call {i} differs from the reference's shaders"
+        self.calls.append(got)
+        if not MINT:
+            want = _load().get(self.tag, [])
+            assert i < len(want) and got == want[i], f"{self.tag}: call {i} differs from the reference's shaders: {got} != {want[i] if i < len(want) else None}"
+        return r
 
 
 def ref(tag: str) -> _Ref:

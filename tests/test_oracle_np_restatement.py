@@ -788,8 +788,9 @@ def test_motion_blur_oracle_matches_numpy_restatement(frame, res):
     assert _agree(want, got, 2e-3, 1e-4, 2e-3) < 2e-3 and (got[:8, :8] == col[:8, :8].astype(np.float64)).all()
 
 
-def np_hbao(p: abi.HbaoParams, depth, blue, prev):
-    """hbao.frag:21-96 + hbao_utils.glsl (normal from depth, the spp-sample form: blueNoise() returns the same texel for every sample)"""
+def np_hbao(p: abi.HbaoParams, depth, blue, prev, paths: dict | None = None):
+    """hbao.frag:21-96 + hbao_utils.glsl (normal from depth, the spp-sample form: blueNoise() returns the same texel for every sample).
+    paths: filled with the foreground pixels' `deltaDepth < th` ("near") and sample weight theta ("theta")"""
     H, W = depth.shape
     M = lambda arr: np.asarray(list(arr), np.float64).reshape(4, 4).T  # noqa: E731
     PV, Pinv, Mw = M(p.projection_view), M(p.projection_inverse), M(p.camera_matrix_world)
@@ -825,6 +826,9 @@ def np_hbao(p: abi.HbaoParams, depth, blue, prev):
     theta = _dot(n, sdir)
     occ = np.sqrt(10.0 * np.maximum(0.0, sdepth + delta * p.bias * 1000.0 - d) * theta * np.maximum(0.0, 1.0 - delta / th) / dist)
     occ = np.where(delta < th, occ, 0.0)
+    if paths is not None:
+        fg = depth != 1.0
+        paths.update(near=(delta < th)[fg], theta=theta[fg], blue_x=np.round(bn[..., 0] * 255.0)[fg])
     total = p.spp * theta
     ao = p.spp * occ
     ao = np.where(total > 0.0, ao / np.where(total == 0.0, 1.0, total), ao)
