@@ -9,7 +9,7 @@
 namespace rfx {
 
 // luminance() of poisson_denoise.frag:28
-RFX_D float lum_p(v3 a) { return powf(dot(mk3(0.2125f, 0.7154f, 0.0721f), a), 0.125f); }
+RFX_D float lum_p(v3 a) { return powcr(dot(mk3(0.2125f, 0.7154f, 0.0721f), a), 0.125f); }
 
 template <bool LINEAR, bool HALF>
 RFX_D v4 fetch_in(const PV& t, v2 uv) {
@@ -50,13 +50,13 @@ __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant
   for (int i = 0; i < TC; i++) {  // :138-164
     const PV& tex = spec[i] ? *ins[1] : a.in0;
     v4 t = fetch_in<LINEAR, HALF>(tex, vUv);
-    age[i] = 1.0f / powf(t.w + 1.0f, 1.2f * a.phi);
+    age[i] = 1.0f / powcr(t.w + 1.0f, 1.2f * a.phi);
     v3 c = xyz(t) * 1.0003f;
-    c = vlog1p_(c);
+    c = mk3(logcr(c.x + 1.0f), logcr(c.y + 1.0f), logcr(c.z + 1.0f));  // log(c + 1.)
     rgb[i] = c; alpha[i] = t.w; lumc[i] = lum_p(c); tw[i] = 1.0f;
   }
   const float glossiness = fmaxf(0.0f, 4.0f * (1.0f - roughness / 0.25f));
-  const float specularFactor = expf(-glossiness * a.specular_phi);
+  const float specularFactor = expcr(-glossiness * a.specular_phi);
   float flatness = 1.0f - fminf(fwn, 1.0f);
   flatness = flatness * flatness * 0.75f + 0.25f;  // pow(flatness, 2.) * 0.75 + 0.25
 
@@ -85,9 +85,9 @@ __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant
       const float depthDiff = 10000.0f * fabsf(depth - ndepth);
       if (GB) {
         const float roughnessDiff = fabsf(roughness - gb_roughness(g.z));
-        wBasic = expf(-normalDiff * a.normal_phi - depthDiff * a.depth_phi - roughnessDiff * a.roughness_phi);
+        wBasic = expcr(-normalDiff * a.normal_phi - depthDiff * a.depth_phi - roughnessDiff * a.roughness_phi);
       } else {
-        wBasic = expf(-normalDiff * a.normal_phi - depthDiff * a.depth_phi);
+        wBasic = expcr(-normalDiff * a.normal_phi - depthDiff * a.depth_phi);
       }
     }
 #pragma unroll
@@ -96,11 +96,11 @@ __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant
       const PV& tex = spec[j] ? *ins[1] : a.in0;
       if (spec[j]) w *= specularFactor;
       v4 t = fetch_in<LINEAR, HALF>(tex, nuv);
-      v3 c = vlog1p_(xyz(t));
-      const float disocclW = powf(w, 0.1f);
+      const v3 c = mk3(logcr(t.x + 1.0f), logcr(t.y + 1.0f), logcr(t.z + 1.0f));
+      const float disocclW = powcr(w, 0.1f);
       float lumaDiff = fabsf(lumc[j] - lum_p(c));
       lumaDiff = fminf(lumaDiff, 0.5f);
-      const float lumaFactor = expf(-lumaDiff * a.luma_phi);
+      const float lumaFactor = expcr(-lumaDiff * a.luma_phi);
       w = mixf(w * lumaFactor, disocclW, age[j]) * age[j];
       w *= (w < 0.0001f) ? 0.0f : 1.0f;  // step(0.0001, w)
       rgb[j] = rgb[j] + w * c;
@@ -109,7 +109,8 @@ __global__ void __launch_bounds__(kThreads) poisson_kernel(const __grid_constant
   }
 #pragma unroll
   for (int j = 0; j < TC; j++) {  // outputTexel :94-100
-    v3 c = vexpm1_(rgb[j] / tw[j]);
+    const v3 m = rgb[j] / tw[j];
+    const v3 c = mk3(expcr(m.x) - 1.0f, expcr(m.y) - 1.0f, expcr(m.z) - 1.0f);  // exp(c) - 1.
     const OutV& o = j == 0 ? a.out0 : a.out1;
     st_h4(o.p, o.pitch, x, y, mk4(c, alpha[j]));
   }
@@ -150,7 +151,9 @@ cudaError_t launch_gbuffer_decode(PV gb, OutV nrd, int W, int H, int gbuffer_tex
 //   w * lumaFactor = exp(A [+ S] - lumaDiff*lumaPhi)     (one ex2 each, no pow)
 //   age = ex2(-1.2*phi*lg2(a + 1)),  exp(x) - 1 -> ex2(x*log2e) - 1
 // The approximate lg2/ex2 have ~2^-22 relative error, far inside the 1e-3 parity budget (the outputs are
-// rounded to fp16 anyway); the exact variant above stays available (rfx_ctx_set_fast_math(ctx, 0)).
+// rounded to fp16 anyway).  The exact variant above (rfx_ctx_set_fast_math(ctx, 0), and every fp16 NEAREST input) takes every
+// transcendental in double and rounds once (logcr / expcr / powcr, as the oracle does), so it is bit-equal to the oracle; at
+// 3840x2160 that costs it ~2.5x the time of the fp32 device libm (H100 80GB HBM3, 700 W).
 // ------------------------------------------------------------------------------------------
 RFX_D float lg2a(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 RFX_D float ex2a(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }

@@ -90,8 +90,6 @@ RFX_D float log2cr(float x) { return (float)log2((double)x); }
 RFX_D float powcr(float x, float y) { return (float)pow((double)x, (double)y); }
 RFX_D float atan2cr(float y, float x) { return (float)atan2((double)y, (double)x); }
 RFX_D float acoscr(float x) { return (float)acos((double)x); }
-RFX_D v3 vlog1p_(v3 a) { return mk3(logf(a.x + 1.0f), logf(a.y + 1.0f), logf(a.z + 1.0f)); }   // log(c + 1.)
-RFX_D v3 vexpm1_(v3 a) { return mk3(expf(a.x) - 1.0f, expf(a.y) - 1.0f, expf(a.z) - 1.0f); }   // exp(c) - 1.
 
 // ---- mat4 (column-major float[16]; M[col*4+row]) ----------------------------------------
 struct M4 { float m[16]; };

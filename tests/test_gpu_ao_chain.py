@@ -49,16 +49,81 @@ def _diff(name, a, b):
         raise AssertionError(f"{name}: rows {rows[0]}..{rows[-1]} differ ({len(rows)} rows)")
 
 
+class OracleAo:
+    """HBAOEffect / HorizonAOEffect.update on the oracle, frame after frame: the AO pass on the (scaled) target with the effect's blue-noise
+    counter, 2 * iterations full-size one-plane Poisson passes with the denoiser's counter, ao_compose.  Like the effect's planes, the AO
+    target and the two Poisson targets carry their texels from frame to frame (background texels keep them)."""
+
+    def __init__(self, W, H, opts, horizon):
+        self.o = {**(effects.defaultHorizonAOOptions if horizon else effects.defaultAOOptions), **opts}
+        self.horizon, self.W, self.H = horizon, W, H
+        self.size, self.res = ao.ao_target_size(W, H, self.o["resolutionScale"])
+        self.ao_index, self.dn_index = effects.BlueNoiseIndex(self.o["blueNoiseStart"]), effects.BlueNoiseIndex(1234567)
+        self.target = np.zeros((self.size[1], self.size[0], 4), np.float16)
+        self.tA, self.tB = np.zeros((H, W, 4), np.float16), np.zeros((H, W, 4), np.float16)
+
+    def frame(self, fr, blue, normal, inp_color):
+        import horizon_harness as hz
+
+        o, cam = self.o, fr["cam"]
+        if self.horizon:
+            p = hz.horizon_params(cam, self.ao_index.value, int(o["directions"]), int(o["steps"]), self.res, distance=o["distance"],
+                                  angle_bias=o["angleBias"], intensity=o["intensity"], max_radius_pixels=o["maxRadiusPixels"])
+            self.target = hz.oracle_hbao_horizon(p, fr["depth"], blue, self.target, normal=normal)
+        else:
+            p = abi.HbaoParams()
+            P = np.asarray(cam["projection"], np.float64).reshape(4, 4).T
+            V = np.asarray(cam["view_matrix"], np.float64).reshape(4, 4).T
+            abi.set_f16(p.projection_view, np.ascontiguousarray((P @ V).T.reshape(16)).astype(np.float32))
+            for k in ("projection_inverse", "camera_matrix_world", "view_matrix"):
+                abi.set_f16(getattr(p, k), cam[k])
+            p.resolution[:] = [float(self.res[0]), float(self.res[1])]
+            p.ao_distance, p.distance_power, p.bias, p.thickness = o["distance"], o["distancePower"], o["bias"], o["thickness"]
+            p.spp, p.blue_noise_index = int(o["spp"]), self.ao_index.value
+            self.target = ao.oracle.hbao(p, fr["depth"], blue, self.target, out_size=self.size, normal=normal, resolution=self.res)
+        for i in range(2 * o["iterations"]):
+            q = abi.PoissonParams()
+            q.radius, q.phi, q.luma_phi, q.depth_phi, q.normal_phi = o["radius"], o["phi"], o["lumaPhi"], o["depthPhi"], o["normalPhi"]
+            q.texture_count, q.gbuffer_texture, q.input_linear, q.blue_noise_index = 1, 0, 1, self.dn_index.value
+            q.is_texture_specular[:] = [0, 0]
+            src = self.target if i == 0 else (self.tB if i % 2 == 0 else self.tA)
+            if i % 2 == 0:
+                self.tA, _ = ao.oracle.poisson_denoise(q, fr["depth"], fr["velocity"], src, None, blue, self.tA, None)
+            else:
+                self.tB, _ = ao.oracle.poisson_denoise(q, fr["depth"], fr["velocity"], src, None, blue, self.tB, None)
+        tex = self.tB if o["iterations"] > 0 else self.target
+        c = abi.AoComposeParams()
+        c.power = o["power"]
+        c.color[:] = [float(x) for x in o["color"]]
+        return self.target, tex, ao.oracle.ao_compose(c, fr["depth"], tex, inp_color)
+
+
 @pytest.mark.parametrize("fast", [True, False], ids=["fast", "exact"])
 @pytest.mark.parametrize("scale", [1.0, 0.5])
 @pytest.mark.parametrize("use_normal", [False, True], ids=["depth-normal", "normal-plane"])
 @pytest.mark.parametrize("iterations", [0, 1, 2])
 @pytest.mark.parametrize("horizon", [False, True], ids=["hbao", "horizon"])
 def test_ao_chain_equals_the_effect(built, horizon, iterations, use_normal, scale, fast):
-    """AO target, denoised plane and composed output of AoChain equal HBAOEffect / HorizonAOEffect byte for byte over 5 moving frames"""
+    """AO target, denoised plane and composed output of AoChain equal HBAOEffect / HorizonAOEffect byte for byte over 5 moving frames.
+    With fast_math off every kernel of the chain is bit-equal to the oracle, so the three planes also equal an oracle AO chain's."""
+    ao_chain_against_effect_and_oracle(horizon, iterations, use_normal, scale, fast, {})
+
+
+@pytest.mark.parametrize("fast", [True, False], ids=["fast", "exact"])
+@pytest.mark.parametrize("scale", [1.0, 0.5])
+@pytest.mark.parametrize("iterations", [0, 1])
+@pytest.mark.parametrize("horizon", [False, True], ids=["hbao", "horizon"])
+def test_ao_chain_with_a_tinted_compose_equals_the_effect(built, horizon, iterations, scale, fast):
+    """as above with power 1.5 and a non-black colour: ao_compose's powcr path (power 2 takes the exact square)"""
+    ao_chain_against_effect_and_oracle(horizon, iterations, False, scale, fast, {"power": 1.5, "color": (0.25, 0.5, 0.125)})
+
+
+def ao_chain_against_effect_and_oracle(horizon, iterations, use_normal, scale, fast, compose: dict):
     W, H = 96, 64
     inp = ch.make_inputs(W, H, 5)
-    opts = {"blueNoiseStart": 777, "resolutionScale": scale, "useNormalPass": use_normal, "iterations": iterations, **(HORIZON_SMALL if horizon else {})}
+    opts = {"blueNoiseStart": 777, "resolutionScale": scale, "useNormalPass": use_normal, "iterations": iterations, **(HORIZON_SMALL if horizon else {}),
+            **compose}
+    orc_ao = None if fast else OracleAo(W, H, opts, horizon)
     ctx = engine.Context(0, inp.blue)
     try:
         ctx.set_fast_math(fast)
@@ -78,9 +143,14 @@ def test_ao_chain_equals_the_effect(built, horizon, iterations, use_normal, scal
             comp.inputBuffer.upload(fr["direct"])
             fx.update(None, comp.inputBuffer)
             chain.render(fr["cam"], sc.depth, sc.velocity, sc.normal, comp.inputBuffer, out)
-            _diff(f"frame {t} AO target", fx.aoTarget.download(), chain.download(0))
-            _diff(f"frame {t} denoised", fx.texture.download(), chain.download(1))
-            _diff(f"frame {t} composed", comp.outputBuffer.download(), out.download())
+            got = chain.download(0), chain.download(1), out.download()
+            _diff(f"frame {t} AO target", fx.aoTarget.download(), got[0])
+            _diff(f"frame {t} denoised", fx.texture.download(), got[1])
+            _diff(f"frame {t} composed", comp.outputBuffer.download(), got[2])
+            if orc_ao is not None:
+                want = orc_ao.frame(fr, inp.blue, normals[t], fr["direct"].astype(np.float16))
+                for name, w, g in zip(("AO target", "denoised", "composed"), want, got):
+                    assert not ch.byte_report("", w, g), ch.byte_report(f"frame {t} {name}", w, g)
         chain.close()
         fx.dispose()
     finally:

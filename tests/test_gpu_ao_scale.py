@@ -71,7 +71,11 @@ def test_poisson_upsamples_a_smaller_linear_input(scene, fast):
         ctx.set_fast_math(fast)
         out = ctx.upload(z)
         ctx.poisson_denoise(p, ctx.upload(f1["depth"]), ctx.upload(f1["velocity"]), ctx.upload(small), None, out, None)
-        check(f"K3 from {tw}x{th} fast={fast}", want, out.download())
+        got = out.download()
+        if fast:
+            check(f"K3 from {tw}x{th} fast={fast}", want, got)
+        else:  # the exact kernel is bit-equal to the oracle
+            assert not ch.byte_report("", want, got), ch.byte_report(f"K3 from {tw}x{th} exact", want, got)
     finally:
         ctx.close()
 

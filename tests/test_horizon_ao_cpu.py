@@ -121,8 +121,9 @@ def directions_table(D: int) -> np.ndarray:
     return out
 
 
-def numpy_horizon(p: abi.HbaoHorizonParams, depth, blue, out_prev, normal=None):
-    """DESIGN.md §1 K6h, restated; returns the RGBA16F target"""
+def numpy_horizon(p: abi.HbaoHorizonParams, depth, blue, out_prev, normal=None, branches: dict | None = None):
+    """DESIGN.md §1 K6h, restated; returns the RGBA16F target.  `branches`, if given, receives per-pixel masks of the branches the
+    pixel takes: foreground, r_px < 1, the max_radius_pixels clamp binding, and the final clamp saturating at 0 and at 1."""
     H, W = out_prev.shape[:2]
     M = {k: np.asarray(getattr(p, k)[:], f32) for k in ("projection", "projection_inverse", "camera_matrix_world", "view_matrix")}
     Proj, Pinv, Cmw, View = M["projection"], M["projection_inverse"], M["camera_matrix_world"], M["view_matrix"]
@@ -161,12 +162,92 @@ def numpy_horizon(p: abi.HbaoHorizonParams, depth, blue, out_prev, normal=None):
             c = np.clip((dot3(N, V) / np.sqrt(safe)).astype(f32) - f32(p.angle_bias), 0, 1).astype(f32)
             f = np.clip(f32(1) - (safe / dist2).astype(f32), 0, 1).astype(f32)
             s = (s + np.where(pos, (c * f).astype(f32), f32(0))).astype(f32)
-    ao = np.clip(f32(1) - ((f32(p.intensity) * s).astype(f32) / f32(p.directions * p.steps)).astype(f32), 0, 1).astype(f32)
-    ao = np.where(r_px >= f32(1), ao, f32(1))
+    ao_raw = (f32(1) - ((f32(p.intensity) * s).astype(f32) / f32(p.directions * p.steps)).astype(f32)).astype(f32)
+    ao = np.where(r_px >= f32(1), np.clip(ao_raw, 0, 1).astype(f32), f32(1))
     out = np.array(out_prev, np.float16, copy=True)
     fg = d0 != f32(1)
+    if branches is not None:
+        marched = fg & (r_px >= f32(1))
+        branches.update(fg=fg, radius_under_one=fg & (r_px < f32(1)), clamp_binds=marched & (r_px > f32(p.max_radius_pixels)),
+                        clamp_free=marched & (r_px <= f32(p.max_radius_pixels)), saturate_0=marched & (ao_raw <= 0), saturate_1=marched & (ao_raw >= 1))
     out[fg] = np.stack(N + [ao], -1)[fg].astype(np.float16)
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------ option grid
+# The scenes of tests/test_gpu_horizon_ao.py: (width, height, orthographic, resolutionScale).  201 x 121 at 0.5 has the fractional
+# `resolution` (100.5, 60.5) over a 100 x 60 target.
+HZ_SCENES = ((200, 120, False, 1.0), (201, 121, False, 0.5), (200, 120, True, 1.0))
+# a distance at which some foreground pixels have r_px < 1 and the others march (perspective); the orthographic r_px is one value for the
+# whole frame, so there it is under 1 everywhere
+SMALL_DISTANCE = {(200, 120, False, 1.0): 0.15, (201, 121, False, 0.5): 0.3, (200, 120, True, 1.0): 0.15}
+LARGE_DISTANCE = 50.0  # the max_radius_pixels clamp binds on most pixels
+
+
+class HzCase:
+    def __init__(self, scene, distance=2.0, max_radius_pixels=64.0, angle_bias=0.1, intensity=1.0):
+        self.scene, self.distance, self.max_radius_pixels, self.angle_bias, self.intensity = scene, distance, max_radius_pixels, angle_bias, intensity
+
+    def __str__(self):
+        W, H, ortho, scale = self.scene
+        return (f"{W}x{H}{'-ortho' if ortho else ''}-s{scale}-d{self.distance:g}-mr{self.max_radius_pixels:g}-ab{self.angle_bias:g}"
+                f"-i{self.intensity:g}")
+
+    def params(self, cam_u: dict, res, index: int = 4711) -> abi.HbaoHorizonParams:
+        return hz.horizon_params(cam_u, index, 8, 32, res, distance=self.distance, angle_bias=self.angle_bias, intensity=self.intensity,
+                                 max_radius_pixels=self.max_radius_pixels)
+
+
+def _hz_grid() -> list:
+    out = []
+    for sc in HZ_SCENES:
+        small = SMALL_DISTANCE[sc]
+        out += [HzCase(sc), HzCase(sc, distance=small), HzCase(sc, distance=LARGE_DISTANCE), HzCase(sc, max_radius_pixels=1.0),
+                HzCase(sc, max_radius_pixels=7.5), HzCase(sc, angle_bias=0.0), HzCase(sc, angle_bias=0.9), HzCase(sc, intensity=0.0),
+                HzCase(sc, intensity=16.0), HzCase(sc, LARGE_DISTANCE, 7.5, 0.0, 16.0), HzCase(sc, small, 1.0, 0.9, 16.0)]
+    return out
+
+
+HZ_CASES = _hz_grid()
+
+
+def hz_inputs(scene, cache: dict = {}):  # noqa: B006  (one set of frames per scene for the whole session)
+    if scene not in cache:
+        W, H, ortho, _ = scene
+        cache[scene] = ch.make_inputs(W, H, 2, orthographic=ortho)
+    return cache[scene]
+
+
+def hz_call(case: HzCase):
+    """(params, depth, blue noise, target filled with a sentinel) of `case` on frame 1 of its scene"""
+    W, H, _, scale = case.scene
+    inp = hz_inputs(case.scene)
+    f1 = inp.frames[1]
+    (tw, th), res = ao.ao_target_size(W, H, scale)
+    return case.params(f1["cam"], res), f1["depth"], inp.blue, np.full((th, tw, 4), -3.0, np.float16)
+
+
+def test_option_grid_reaches_every_branch():
+    """the K6h option grid of tests/test_gpu_horizon_ao.py, counted with the numpy restatement: on each perspective scene one case has
+    pixels with r_px < 1 (AO 1) beside pixels that march; on each scene the max_radius_pixels clamp binds on most pixels of one case and
+    on none of another; the final clamp saturates at 0 and at 1"""
+    for sc in HZ_SCENES:
+        counts = []
+        for case in (c for c in HZ_CASES if c.scene == sc):
+            p, depth, blue, prev = hz_call(case)
+            b = {}
+            numpy_horizon(p, depth, blue, prev, branches=b)
+            counts.append((case, {k: float(v.sum() / b["fg"].sum()) for k, v in b.items() if k != "fg"}))
+        name = str(counts[0][0])
+        if sc[2]:
+            assert any(c["radius_under_one"] == 1.0 for _, c in counts), name
+        else:
+            assert any(0.05 < c["radius_under_one"] < 0.95 for _, c in counts), (name, counts)
+        assert any(c["clamp_binds"] > 0.5 for case, c in counts if case.distance == LARGE_DISTANCE), name
+        assert any(c["clamp_binds"] == 0.0 and c["clamp_free"] > 0.9 for _, c in counts), name
+        assert any(c["clamp_binds"] > 0.9 for case, c in counts if case.max_radius_pixels == 7.5), name
+        assert any(c["saturate_0"] > 0 for _, c in counts), name
+        assert any(0 < c["saturate_1"] < 1 for _, c in counts) and any(c["saturate_1"] == 1.0 for case, c in counts if case.intensity == 0), name
 
 
 # ------------------------------------------------------------------------------------------------------------------ fixtures
