@@ -657,9 +657,32 @@ void rfx_ao_chain_destroy(rfx_ao_chain* chain);
 rfx_status rfx_ao_chain_set_options(rfx_ao_chain* chain, const rfx_ao_chain_options* opt);
 /* Back to the state of a new chain: the kept planes are cleared and both blue-noise counters restart (every rank of a group together). */
 rfx_status rfx_ao_chain_reset(rfx_ao_chain* chain);
+/* With the TRAA tail on: RFX_ERR_INVALID_ARG (the tail needs the camera: rfx_ao_chain_render_traa). */
 rfx_status rfx_ao_chain_render(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);
+/* TRAA frame tail: the frame an AOEffect user runs, whose update looks for an enabled TRAAEffect in the composer
+ * (src/ao/AOEffect.js:156-169): the AO EffectPass (K6 / K6h -> Poisson -> K7) into a chain-owned composer buffer, then the TRAA
+ * EffectPass (K2 in its TRAA form: temporal_reproject.frag with textureCount 1, inputType "diffuse", RGBA16F history sampled LINEAR;
+ * src/traa/TRAAEffect.js:21-31) and K9 traa_compose into frame->output.  The same per-pass launches as the SSGI chain's tail without its
+ * K5; the AO bytes do not change (AOEffect defines animatedNoise under TRAA, but hbao.frag never reads the seed it computes).
+ * Options: rfx_traa_tail_options with `compose` all zero (the AO tail has no K5; anything else is RFX_ERR_INVALID_ARG).  Allocates the
+ * tail's planes (the K7 output RGBA16F; the TRAA accumulated plane RGBA16F x 2 by tail-frame parity) and renders the tail from the next
+ * frame on; on a chain whose tail is on it replaces the options and resets the TRAA history (keepData 0 on the next frame).  The first
+ * frame after enabling renders with keepData 0 too.  opt == NULL turns the tail off and frees its planes.  A chain attached to a group
+ * of n > 1 cannot change its tail: RFX_ERR_UNSUPPORTED. */
+rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* chain, const rfx_traa_tail_options* opt);
+/* What the TRAA pass needs and rfx_ao_frame lacks: near / far, the perspective flag and the position of the UN-jittered camera (jittering
+ * the rasteriser, TAAUtils.js, stays the host's job), and didCameraMove (src/utils/SceneUtils.js:17-27) for fullAccumulate.  The chain
+ * keeps the previous frame's camera; on the first frame and after rfx_ao_chain_reset the previous camera is the current one. */
+typedef struct rfx_ao_traa_frame {
+  rfx_camera cam;
+  float camera_pos[3];
+  int32_t camera_moved;
+} rfx_ao_traa_frame;
+/* One frame with the tail (frame->input and frame->output required: RFX_ERR_INVALID_ARG).  Tail off: RFX_ERR_NOT_READY. */
+rfx_status rfx_ao_chain_render_traa(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame, const rfx_ao_traa_frame* traa);
 /* which: 0 the AO target (RGBA16F, the scaled size), 1 the denoised plane K7 composes (Poisson target B; the AO target with
- * iterations 0), of the latest frame */
+ * iterations 0), of the latest frame; with the TRAA tail on, 2 the K7 output and 3 the TRAA accumulated plane (next frame's history).
+ * 2 / 3 with the tail off: RFX_ERR_INVALID_ARG. */
 rfx_status rfx_ao_chain_output(rfx_ao_chain* chain, int32_t which, rfx_plane* out);
 /* Row-sharded AO.  A group takes an AO chain or an SSGI chain, never both (RFX_ERR_INVALID_ARG).  No AO pass reads a produced plane at
  * an arbitrary uv: K6 / K6h read the caller's depth, the Poisson taps and K7 are bounded stencils, recomputed on widened ranges
@@ -667,14 +690,22 @@ rfx_status rfx_ao_chain_output(rfx_ao_chain* chain, int32_t which, rfx_plane* ou
  * peer-mapped at attach time, and a discarded (background) pixel of K6 / K6h / K3 carries last frame's texel from the rank that owns the
  * row.  Both algorithms, every iteration count, with or without a normal plane, fast_math on or off.  resolution_scale < 1 (the rows
  * of a smaller AO target do not map 1:1 onto output rows) and fewer than 64 rows per rank: RFX_ERR_UNSUPPORTED; members whose
- * algorithm or iterations differ: RFX_ERR_INVALID_ARG.  Results are bit-identical to one rfx_ao_chain. */
+ * algorithm or iterations differ: RFX_ERR_INVALID_ARG.  Results are bit-identical to one rfx_ao_chain.
+ * With the TRAA tail on (rfx_ao_chain_enable_traa before the attach), the TRAA accumulated plane is one more kept plane: the TRAA pass
+ * reads last frame's at reprojected uvs anywhere on screen, on the rank that owns each row (or replicated, RFX_GROUP_EXCHANGE=allgather).
+ * Members whose tail is on and off: RFX_ERR_INVALID_ARG. */
 rfx_status rfx_group_attach_ao_chain(rfx_group* group, rfx_ao_chain* chain);  /* collective */
 rfx_status rfx_group_attach_ao_chains_inprocess(rfx_group* const* groups, rfx_ao_chain* const* chains, int32_t world);
-rfx_status rfx_ao_chain_render_sharded(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);  /* collective */
+/* collective.  With the TRAA tail on: RFX_ERR_INVALID_ARG (rfx_ao_chain_render_sharded_traa). */
+rfx_status rfx_ao_chain_render_sharded(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);
+/* collective: rfx_ao_chain_render_traa in a group.  Tail off: RFX_ERR_NOT_READY. */
+rfx_status rfx_ao_chain_render_sharded_traa(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame, const rfx_ao_traa_frame* traa);
 /* pure host arithmetic: rows [ranges[2k], ranges[2k+1]) of launch k (K6 / K6h, Poisson pass 0 .. 2*iterations-1, K7) for the band
  * [own0, own1); n_launches = 2 + 2 * iterations.  K7 runs on the band, the last Poisson pass on the band +- 1 row (K7's LINEAR fetch at
  * the pixel centre; with iterations 0 K6 gets those rows), and every earlier launch on the next one's range widened by the Poisson halo
- * ceil(|radius| * max(1, height / width)) + 1. */
+ * ceil(|radius| * max(1, height / width)) + 1.
+ * n_launches = 3 + 2 * iterations: the same with the TRAA tail as the last launch; it runs on the band and K7 on the band widened by
+ * RFX_TRAA_TAIL_ROWS (every earlier launch widens from K7's range as above). */
 rfx_status rfx_ao_shard_ranges(uint32_t width, uint32_t height, uint32_t own0, uint32_t own1, int32_t iterations, float radius,
                                uint32_t* ranges, uint32_t n_launches);
 

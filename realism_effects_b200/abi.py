@@ -186,6 +186,11 @@ class AoFrame(C.Structure):
                 ("output", C.POINTER(Plane))]
 
 
+class AoTraaFrame(C.Structure):
+    """rfx_ao_traa_frame: the TRAA tail's un-jittered camera, its position and didCameraMove"""
+    _fields_ = [("cam", CameraS), ("camera_pos", F3), ("camera_moved", C.c_int32)]
+
+
 def make_camera(u: dict, perspective: "bool | None" = None) -> CameraS:
     """u: dict from synth.Camera.uniforms() (float32 column-major arrays); perspective: camera.isPerspectiveCamera (default: u["perspective"], else True)."""
     if perspective is None:
@@ -300,6 +305,9 @@ def _sig(lib):
     lib.rfx_ao_chain_reset.argtypes = [vp]
     lib.rfx_ao_chain_render.argtypes = [vp, vp, _P(AoFrame)]
     lib.rfx_ao_chain_output.argtypes = [vp, C.c_int32, PP]
+    lib.rfx_ao_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
+    lib.rfx_ao_chain_render_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
+    lib.rfx_ao_chain_render_sharded_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
     lib.rfx_group_attach_ao_chain.argtypes = [vp, vp]
     lib.rfx_group_attach_ao_chains_inprocess.argtypes = [_P(vp), _P(vp), C.c_int32]
     lib.rfx_ao_chain_render_sharded.argtypes = [vp, vp, _P(AoFrame)]
@@ -322,6 +330,7 @@ EXPORTS = [
     "rfx_shard_rebalance", "rfx_gbuffer_debug_launch", "rfx_ssgi_chain_set_debug_view",
     "rfx_ao_chain_create", "rfx_ao_chain_destroy", "rfx_ao_chain_set_options", "rfx_ao_chain_reset", "rfx_ao_chain_render", "rfx_ao_chain_output",
     "rfx_group_attach_ao_chain", "rfx_group_attach_ao_chains_inprocess", "rfx_ao_chain_render_sharded", "rfx_ao_shard_ranges",
+    "rfx_ao_chain_enable_traa", "rfx_ao_chain_render_traa", "rfx_ao_chain_render_sharded_traa",
 ]
 
 

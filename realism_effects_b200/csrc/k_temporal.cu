@@ -321,12 +321,13 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_kernel(c
 
 // K2 with the history read on the owners and the carry of discarded pixels (TemporalPeer).  temporal_px returns without a store
 // exactly where the shader discards, so a pixel whose planes were not stored copies last frame's texels of out0 / out1.
+// FAST = false exists for the TRAA form only (TC 1, DIFFUSE): the AO chain's TRAA tail in a group with fast_math off.
 struct StoreSeen {
   PlaneStore s;
   bool* seen;
   RFX_D void operator()(int i, v4 v) const { *seen = true; s(i, v); }
 };
-template <int TC, int ITYPE, bool LOG>
+template <int TC, int ITYPE, bool LOG, bool FAST = true>
 __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_peer_kernel(const __grid_constant__ TemporalArgs a, const __grid_constant__ TemporalPeer p) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
@@ -337,7 +338,7 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_peer_ker
   s.curvature = length(fwidth_3(s.worldNormal));
   if (!active) return;
   bool seen = false;
-  temporal_px<TC, ITYPE, LOG, true, true>(a, PlaneH4{a.input}, PeerHist{p.hist0}, PeerHist{p.hist1}, s, fwd, x, y, StoreSeen{PlaneStore{a, x, y}, &seen});
+  temporal_px<TC, ITYPE, LOG, true, FAST>(a, PlaneH4{a.input}, PeerHist{p.hist0}, PeerHist{p.hist1}, s, fwd, x, y, StoreSeen{PlaneStore{a, x, y}, &seen});
   if (ITYPE != RFX_INPUT_DIFFUSE && !seen) {
     if (a.out_half) { carry_texel<8>(p.carry.p[0], a.out0, x, y); if (TC == 2) carry_texel<8>(p.carry.p[1], a.out1, x, y); }
     else { carry_texel<16>(p.carry.p[0], a.out0, x, y); if (TC == 2) carry_texel<16>(p.carry.p[1], a.out1, x, y); }
@@ -345,8 +346,14 @@ __global__ void __launch_bounds__(kThreads, RFX_K2_MIN_BLOCKS) temporal_peer_ker
 }
 
 cudaError_t launch_temporal_peer(const TemporalArgs& a, const TemporalPeer& p, cudaStream_t s) {
-  if (!a.history_linear || !a.fast || a.in_scaled) return cudaErrorNotSupported;
+  if (!a.history_linear || a.in_scaled) return cudaErrorNotSupported;
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
+  if (!a.fast) {
+    if (a.input_type != RFX_INPUT_DIFFUSE || a.texture_count != 1) return cudaErrorNotSupported;
+    if (a.log_transform) temporal_peer_kernel<1, RFX_INPUT_DIFFUSE, true, false><<<grid, kThreads, 0, s>>>(a, p);
+    else temporal_peer_kernel<1, RFX_INPUT_DIFFUSE, false, false><<<grid, kThreads, 0, s>>>(a, p);
+    return cudaGetLastError();
+  }
 #define RFX_LTP(TC, IT) do { if (a.log_transform) temporal_peer_kernel<TC, IT, true><<<grid, kThreads, 0, s>>>(a, p); else temporal_peer_kernel<TC, IT, false><<<grid, kThreads, 0, s>>>(a, p); } while (0)
   if (a.input_type == RFX_INPUT_DIFFUSE_SPECULAR && a.texture_count == 2) RFX_LTP(2, RFX_INPUT_DIFFUSE_SPECULAR);
   else if (a.input_type == RFX_INPUT_DIFFUSE && a.texture_count == 1) RFX_LTP(1, RFX_INPUT_DIFFUSE);

@@ -1315,6 +1315,32 @@ static rfx_status debug_view_plane(rfx_ssgi_chain* ch, void* stream, const rfx_s
   return RFX_OK;
 }
 
+// The TRAA pass of a chain's frame tail (TRAAEffect, shared by the SSGI and AO chains).  traa_params: K2's uniforms, TRAAEffect's forced
+// options (TRAAEffect.js:21-31) over the TemporalReprojectPass defaults, on cam_tp's camera and previous-frame matrices.
+static rfx_temporal_params traa_params(const rfx_temporal_params& cam_tp, const rfx_traa_tail_options& o, float keep, int32_t camera_moved) {
+  rfx_temporal_params tp = cam_tp;
+  tp.max_blend = o.max_blend; tp.neighborhood_clamp_intensity = o.neighborhood_clamp_intensity;
+  tp.confidence_power = o.confidence_power; tp.log_transform = o.log_transform ? 1 : 0;
+  tp.keep_data = keep;
+  tp.full_accumulate = o.full_accumulate && !camera_moved ? 1 : 0;
+  tp.texture_count = 1; tp.input_type = RFX_INPUT_DIFFUSE; tp.history_linear = 1;
+  tp.reproject_specular[0] = tp.reproject_specular[1] = 0;
+  return tp;
+}
+// K2 in its TRAA form over `input` on the output rows kr +- 1 (K9's LINEAR fetch) into buffer `cur` of the accumulated plane, reading last
+// frame's buffer cur ^ 1 (in a row-sharded group of n > 1, `peer`: on the rank that owns each row), then K9 from it into `out` on kr.
+// `input` must hold rows kr +- RFX_TRAA_TAIL_ROWS.
+static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_params& tp, const rfx_plane* input, const rfx_plane* velocity,
+                                HistPlane& acc, int cur, bool peer, const rfx_plane* out, Rows kr) {
+  const int H = (int)acc.buf[cur].height;
+  TemporalPeer tpeer{};
+  tpeer.hist0 = tpeer.hist1 = acc.view[cur ^ 1];
+  rfx_status st = temporal_reproject(ctx, stream, &tp, input, velocity, &acc.buf[cur ^ 1], nullptr, &acc.buf[cur], nullptr, std::max(0, kr.r0 - 1),
+                                     std::min(H, kr.r1 + 1), peer ? &tpeer : nullptr);
+  if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+  return st;
+}
+
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
 // rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
 // K2 on them +- 1).
@@ -1323,13 +1349,7 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   const int W = (int)ch->opt.width, H = (int)ch->opt.height;
   const Rows kr = launch_rows(ranges, k, H);
   const int cur = (int)(ch->traa_frames & 1), prev = cur ^ 1;
-  rfx_temporal_params tp = ch->traa_tp;  // TRAAEffect's forced options over the TemporalReprojectPass defaults (TRAAEffect.js:21-31)
-  tp.max_blend = ch->traa.max_blend; tp.neighborhood_clamp_intensity = ch->traa.neighborhood_clamp_intensity;
-  tp.confidence_power = ch->traa.confidence_power; tp.log_transform = ch->traa.log_transform ? 1 : 0;
-  tp.keep_data = ch->traa_keep;
-  tp.full_accumulate = ch->traa.full_accumulate && !f->camera_moved ? 1 : 0;
-  tp.texture_count = 1; tp.input_type = RFX_INPUT_DIFFUSE; tp.history_linear = 1;
-  tp.reproject_specular[0] = tp.reproject_specular[1] = 0;
+  const rfx_temporal_params tp = traa_params(ch->traa_tp, ch->traa, ch->traa_keep, f->camera_moved);
   const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
   if (ch->fastpath && !debug) {
     CTraaArgs a{};
@@ -1363,12 +1383,7 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     if (st == RFX_OK)
       st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &ch->traa_k5, (uint32_t)std::max(0, kr.r0 - halo),
                                    (uint32_t)std::min(H, kr.r1 + halo));
-    TemporalPeer tpeer{};  // in a row-sharded group of n > 1 the TRAA history is read on the rank that owns each row
-    tpeer.hist0 = tpeer.hist1 = ch->traa_acc.view[prev];
-    if (st == RFX_OK)
-      st = temporal_reproject(ctx, stream, &tp, &ch->traa_k5, f->velocity, &ch->traa_acc.buf[prev], nullptr, &ch->traa_acc.buf[cur], nullptr,
-                              std::max(0, kr.r0 - 1), std::min(H, kr.r1 + 1), ch->group_peer ? &tpeer : nullptr);
-    if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &ch->traa_acc.buf[cur], &ch->traa_out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, &ch->traa_k5, f->velocity, ch->traa_acc, cur, ch->group_peer, &ch->traa_out, kr);
     if (st != RFX_OK) return st;
   }
   ch->traa_keep = 1.0f;
@@ -1757,7 +1772,19 @@ struct rfx_ao_chain {
   int32_t bn_ao = 0, bn_dn = 0;  // the AO pass's and the denoiser's BlueNoiseIndex
   struct rfx_group* group = nullptr;
   bool group_peer = false;  // attached to a group of n > 1: double-buffered planes, carry instantiations
+  // TRAA frame tail (rfx_ao_chain_enable_traa): K7 into traa_k7, then the TRAA pass and K9 into frame->output
+  bool traa_on = false;
+  rfx_traa_tail_options traa{};
+  HistPlane traa_acc;             // accumulated plane by tail parity (buf[prev] is the history)
+  rfx_plane traa_k7{};            // K7 output: the composer buffer between the AO and the TRAA EffectPass
+  uint64_t traa_frames = 0;       // tails rendered; traa_acc.buf[traa_frames & 1] is written next
+  float traa_keep = 0.0f;         // keepData of the TRAA pass
+  bool traa_have_prev = false;    // traa_prev holds the previous frame's camera
+  rfx_ao_traa_frame traa_prev{};
 };
+static void free_traa(rfx_ao_chain* ch) {
+  for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_k7}) if (p->ptr) rfx_plane_free(ch->ctx, p);
+}
 static int pass_latest(const rfx_ao_chain* ch);  // the buffer of every plane that holds the latest frame (rfx_group.inl)
 
 static void ao_target_size(const rfx_ao_chain_options& o, uint32_t& w, uint32_t& h, float& rx, float& ry) {
@@ -1797,6 +1824,7 @@ void rfx_ao_chain_destroy(rfx_ao_chain* ch) {
   cudaStreamSynchronize(ch->ctx->stream);
   for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ch->ctx, &p);
+  free_traa(ch);
   delete ch;
 }
 
@@ -1820,17 +1848,50 @@ rfx_status rfx_ao_chain_set_options(rfx_ao_chain* ch, const rfx_ao_chain_options
 rfx_status rfx_ao_chain_reset(rfx_ao_chain* ch) {
   if (!ch) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
-  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
+  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB, &ch->traa_acc})
     for (const rfx_plane& p : h->buf)
       if (p.ptr) CU(cudaMemset2DAsync(p.ptr, p.pitch, 0, (size_t)p.width * 8, p.height, ctx->stream));
   ch->bn_ao = ch->bn_dn = 0;
   ch->luma_phi = ch->opt.luma_phi; ch->depth_phi = ch->opt.depth_phi; ch->normal_phi = ch->opt.normal_phi;
+  ch->traa_keep = 0.0f;  // a new TRAA pass: keepData 0, and the first frame's previous camera is its own
+  ch->traa_have_prev = false;
+  return RFX_OK;
+}
+
+rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* ch, const rfx_traa_tail_options* opt) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (ch->group && rfx_group_world(ch->group) > 1)
+    return fail(ctx, RFX_ERR_UNSUPPORTED, "ao_chain_enable_traa: the chain is in a row-sharded group, whose peer mappings are fixed at attach time");
+  if (!opt) {
+    CU(cudaStreamSynchronize(ctx->stream));
+    free_traa(ch);
+    ch->traa_on = false;
+    return RFX_OK;
+  }
+  static const rfx_ssgi_compose_params no_compose{};
+  if (memcmp(&opt->compose, &no_compose, sizeof no_compose) != 0)
+    return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_enable_traa: the AO tail has no K5: `compose` must be all zero");
+  if (!ch->traa_k7.ptr) {
+    rfx_status st = RFX_OK;
+    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_k7})
+      if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
+    if (st != RFX_OK) { free_traa(ch); return st; }
+    local_views(ch->traa_acc);
+  }
+  ch->traa = *opt;
+  ch->traa_on = true;
+  ch->traa_keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
   return RFX_OK;
 }
 
 rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
-  if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1");
+  if (ch->traa_on && (which == 2 || which == 3)) {
+    *out = which == 2 ? ch->traa_k7 : ch->traa_acc.buf[(ch->traa_frames + 1) & 1];
+    return RFX_OK;
+  }
+  if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1 (2 / 3 with the TRAA tail on)");
   const HistPlane& h = which == 1 && ch->opt.iterations > 0 ? ch->dnB : ch->target;  // AOEffect's `texture`
   *out = h.buf[h.buf[1].ptr ? pass_latest(ch) : 0];
   return RFX_OK;
@@ -1839,13 +1900,15 @@ rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) 
 }  // extern "C"
 
 // One frame of the AO chain.  `ranges` == nullptr: whole planes.  Otherwise ranges[2k], ranges[2k+1] = output rows [a,b) of launch k
-// (K6 / K6h, K3 pass 0..2*iterations-1, K7) of this rank's band, widened by the halos the next launches recompute (rfx_ao_shard_ranges).
-static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f, const uint32_t* ranges) {
+// (K6 / K6h, K3 pass 0..2*iterations-1, K7[, the TRAA tail]) of this rank's band, widened by the halos the next launches recompute
+// (rfx_ao_shard_ranges).  `t`: the TRAA tail's camera, given exactly when the tail is on (the entry points check it).
+static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f, const uint32_t* ranges, const rfx_ao_traa_frame* t) {
   rfx_ctx* ctx = ch->ctx;
   const rfx_ao_chain_options& o = ch->opt;
   if (!f->depth || !f->velocity) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: depth and velocity are required");
   if (o.use_normal_plane && !f->normal) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: use_normal_plane needs frame->normal (RGBA8 view-space normals)");
   if (f->output && !f->input) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: K7 composes over frame->input: it may not be NULL with an output");
+  if (t && !f->output) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain: the TRAA tail renders into frame->output: it may not be NULL");
   if (f->depth->width != o.width || f->depth->height != o.height) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ao_chain: the depth plane must have the chain's size");
   const rfx_plane* normal = o.use_normal_plane ? f->normal : nullptr;
   // Alone the chain renders in place.  In a row-sharded group of n > 1 (rfx_group.inl) it writes buffer `wr` and a discarded pixel
@@ -1907,22 +1970,58 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     if (st != RFX_OK) return st;
     decoded = true;  // the velocity plane does not change within a frame; the first pass's rows are the widest
   }
-  // ---- K7  ao_compose.frag over AOEffect's `texture`
+  // ---- K7  ao_compose.frag over AOEffect's `texture` (with the TRAA tail: into the composer buffer the TRAA EffectPass reads)
   if (f->output) {
     rfx_ao_compose_params cp{};
     cp.power = o.power;
     memcpy(cp.color, o.color, 12);
     const Rows kr = launch_rows(ranges, k, (int)o.height);
     const HistPlane& tex = o.iterations > 0 ? ch->dnB : ch->target;
-    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, t ? &ch->traa_k7 : f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
     if (st != RFX_OK) return st;
+  }
+  k++;
+  // ---- the TRAA tail: TRAAEffect's temporal pass over the K7 plane, then K9 into frame->output
+  if (t) {
+    rfx_temporal_params cam{};
+    const rfx_ao_traa_frame& prev = ch->traa_have_prev ? ch->traa_prev : *t;  // TemporalReprojectPass.js:94-97 on the first frame
+    cam.cam = t->cam;
+    memcpy(cam.prev_view_matrix, prev.cam.view_matrix, 64); memcpy(cam.prev_camera_matrix_world, prev.cam.camera_matrix_world, 64);
+    memcpy(cam.prev_projection, prev.cam.projection, 64); memcpy(cam.prev_projection_inverse, prev.cam.projection_inverse, 64);
+    memcpy(cam.camera_pos, t->camera_pos, 12); memcpy(cam.prev_camera_pos, prev.camera_pos, 12);
+    const rfx_temporal_params tp = traa_params(cam, ch->traa, ch->traa_keep, t->camera_moved);
+    st = traa_launches(ctx, stream, tp, &ch->traa_k7, f->velocity, ch->traa_acc, (int)(ch->traa_frames & 1), ch->group_peer, f->output,
+                       launch_rows(ranges, k, (int)o.height));
+    if (st != RFX_OK) return st;
+    ch->traa_keep = 1.0f;
+    ch->traa_frames++;
+    ch->traa_prev = *t;
+    ch->traa_have_prev = true;
   }
   return RFX_OK;
 }
 
-extern "C" rfx_status rfx_ao_chain_render(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f) {
-  if (!ch || !f) return RFX_ERR_INVALID_ARG;
-  return ao_render_impl(ch, stream, f, nullptr);
+// The entry points: the tail's camera is given exactly when the tail is on.
+static rfx_status ao_check_traa(rfx_ao_chain* ch, const rfx_ao_traa_frame* t, const char* who) {
+  if (ch->traa_on && !t) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "%s: the TRAA tail is on and needs the camera (render with the _traa entry point)", who);
+  if (!ch->traa_on && t) return fail(ch->ctx, RFX_ERR_NOT_READY, "%s: the TRAA tail is off (rfx_ao_chain_enable_traa)", who);
+  return RFX_OK;
 }
+
+extern "C" {
+
+rfx_status rfx_ao_chain_render(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f) {
+  if (!ch || !f) return RFX_ERR_INVALID_ARG;
+  rfx_status st = ao_check_traa(ch, nullptr, "ao_chain_render");
+  return st != RFX_OK ? st : ao_render_impl(ch, stream, f, nullptr, nullptr);
+}
+
+rfx_status rfx_ao_chain_render_traa(rfx_ao_chain* ch, void* stream, const rfx_ao_frame* f, const rfx_ao_traa_frame* t) {
+  if (!ch || !f || !t) return RFX_ERR_INVALID_ARG;
+  rfx_status st = ao_check_traa(ch, t, "ao_chain_render_traa");
+  return st != RFX_OK ? st : ao_render_impl(ch, stream, f, nullptr, t);
+}
+
+}  // extern "C"
 
 #include "rfx_group.inl"

@@ -181,7 +181,8 @@ struct TemporalArgs {
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t s);
 // K2 of the per-pass chain in a row-sharded group: the history planes are read on the rank that owns each row (RGBA16F through
 // peer_h4_linear, RGBA32F through peer_f4_linear), and a discarded pixel carries last frame's texel of out0 / out1 (double-buffered)
-// from the owner.  a.hist0 / a.hist1 are ignored; history_linear and fast must be on.
+// from the owner.  a.hist0 / a.hist1 are ignored; history_linear must be on, and fast too except for the TRAA form (texture_count 1,
+// input_type DIFFUSE), which also has an exact instantiation.
 struct TemporalPeer {
   PeerPV hist0, hist1;
   PeerCarry carry;

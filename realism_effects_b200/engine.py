@@ -357,6 +357,7 @@ class AoChain:
 
     def __init__(self, ctx: Context, opt: abi.AoChainOptions):
         self.ctx, self.opt = ctx, opt
+        self.traa = None
         h = C.c_void_p()
         ctx._chk(ctx.lib.rfx_ao_chain_create(ctx.h, C.byref(opt), C.byref(h)))
         self.h = h
@@ -383,13 +384,40 @@ class AoChain:
         f.depth, f.velocity, f.normal, f.input, f.output = ptr(depth), ptr(velocity), ptr(normal), ptr(inp), ptr(out)
         return f
 
-    def render(self, cam_u: dict, depth, velocity, normal=None, inp=None, out=None, stream=None):
-        """one frame; out=None skips K7"""
+    def enable_traa(self, options: "abi.TraaTailOptions | None" = None, enable: bool = True):
+        """TRAA frame tail (K7 -> TRAA -> K9, include/rfx.h: rfx_ao_chain_enable_traa): render() then takes the TRAA camera and writes the
+        K9 frame to `out`; outputs 2 (the K7 plane) and 3 (the TRAA accumulated plane).  options: abi.make_traa_tail_options(...) without
+        `compose` (default: TRAAEffect's values); enable=False turns it off.  Enabling again replaces the options and resets the TRAA history."""
+        if not enable:
+            self.ctx._chk(self.ctx.lib.rfx_ao_chain_enable_traa(self.h, None))
+            self.traa = None
+            return
+        self.traa = options if options is not None else abi.make_traa_tail_options()
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_enable_traa(self.h, C.byref(self.traa)))
+
+    @staticmethod
+    def _traa_frame(traa_cam: dict, camera_moved: bool) -> abi.AoTraaFrame:
+        """traa_cam: the un-jittered camera's uniforms (synth.Camera.uniforms(): matrices, near / far, position)"""
+        t = abi.AoTraaFrame()
+        t.cam = abi.make_camera(traa_cam)
+        t.camera_pos[:] = [float(x) for x in traa_cam["position"]]
+        t.camera_moved = int(bool(camera_moved))
+        return t
+
+    def render(self, cam_u: dict, depth, velocity, normal=None, inp=None, out=None, stream=None, traa_cam: dict | None = None,
+               camera_moved: bool = True):
+        """one frame; out=None skips K7.  With the TRAA tail on, traa_cam (the un-jittered camera's uniforms) and camera_moved
+        (didCameraMove) feed the TRAA pass and `out` receives the K9 frame."""
         f = self._frame(cam_u, depth, velocity, normal, inp, out)
-        self.ctx._chk(self.ctx.lib.rfx_ao_chain_render(self.h, stream, C.byref(f)))
+        if traa_cam is None:
+            self.ctx._chk(self.ctx.lib.rfx_ao_chain_render(self.h, stream, C.byref(f)))
+        else:
+            t = self._traa_frame(traa_cam, camera_moved)
+            self.ctx._chk(self.ctx.lib.rfx_ao_chain_render_traa(self.h, stream, C.byref(f), C.byref(t)))
 
     def output(self, which: int = 1) -> Plane:
-        """0 the AO target, 1 the denoised plane K7 composes (the AO target with iterations 0)"""
+        """0 the AO target, 1 the denoised plane K7 composes (the AO target with iterations 0); with the TRAA tail on, 2 the K7 plane and
+        3 the TRAA accumulated plane"""
         p = Plane()
         self.ctx._chk(self.ctx.lib.rfx_ao_chain_output(self.h, which, C.byref(p)))
         return p

@@ -164,14 +164,16 @@ class ShardPlan:
 @dataclass
 class AoShardPlan:
     """Row ranges [a, b) per launch of one AO chain frame for the band `own`, in chain order: K6 / K6h, K3 pass 0..2*iterations-1, K7
-    (mirror of rfx_ao_shard_ranges).  No AO pass reads a produced plane at an arbitrary uv, so the only cross-row reads are K7's LINEAR
-    fetch at the pixel centre (1 row) and the Poisson taps (the halo of ShardPlan)."""
+    and, with `traa`, the TRAA tail (mirror of rfx_ao_shard_ranges).  No AO pass reads a produced plane at an arbitrary uv, so the only
+    cross-row reads are K7's LINEAR fetch at the pixel centre (1 row), the Poisson taps (the halo of ShardPlan) and the tail's reads of
+    the K7 plane (ShardPlan.TRAA_TAIL_ROWS)."""
 
     width: int
     height: int
     own: tuple
     iterations: int
     radius: float
+    traa: bool = False  # the TRAA tail runs as one more launch after K7 (rfx_ao_chain_enable_traa)
 
     K7_INPUT_ROWS = 1
 
@@ -181,13 +183,15 @@ class AoShardPlan:
 
     @property
     def n_launches(self) -> int:
-        return 2 + 2 * self.iterations
+        return 2 + 2 * self.iterations + (1 if self.traa else 0)
 
     @property
     def ranges(self) -> list:
         expand = lambda r, rows: (max(0, r[0] - rows), min(self.height, r[1] + rows))  # noqa: E731
         out = [tuple(self.own)]
-        r = expand(out[0], self.K7_INPUT_ROWS)
+        if self.traa:
+            out.append(expand(out[0], ShardPlan.TRAA_TAIL_ROWS))
+        r = expand(out[-1], self.K7_INPUT_ROWS)
         for _ in range(2 * self.iterations):
             out.append(r)
             r = expand(r, self.poisson_halo)
@@ -526,12 +530,25 @@ class InProcessGroup:
             ch.close()
 
 
+def _render_ao_band(ctx, chain, stream, frame: tuple, traa_cam, camera_moved: bool):
+    """rfx_ao_chain_render_sharded (traa_cam None) or rfx_ao_chain_render_sharded_traa for one member; frame: AoChain._frame's arguments"""
+    import ctypes as C
+
+    f = chain._frame(*frame)
+    if traa_cam is None:
+        ctx._chk(ctx.lib.rfx_ao_chain_render_sharded(chain.h, stream, C.byref(f)))
+    else:
+        t = chain._traa_frame(traa_cam, camera_moved)
+        ctx._chk(ctx.lib.rfx_ao_chain_render_sharded_traa(chain.h, stream, C.byref(f), C.byref(t)))
+
+
 class ShardedAoChain(ShardedSsgiChain):
     """This rank's member of a row-sharded AO chain: rfx_group_* + rfx_ao_chain_render_sharded.  Bands, rebalancing and the unique-id
     exchange are ShardedSsgiChain's; the host-buffer path is not (out of scope for AO)."""
 
     def __init__(self, ctx, ao_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
-                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None):
+                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None):
+        """traa: abi.TraaTailOptions (abi.make_traa_tail_options()) to render the TRAA tail too (the same on every rank), or None"""
         import ctypes as C
 
         from . import abi, engine
@@ -539,6 +556,8 @@ class ShardedAoChain(ShardedSsgiChain):
         self._abi, self.ctx, self.lib, self._C = abi, ctx, ctx.lib, C
         self.rank, self.world, unique_id = _group_unique_id(ctx, rank, world, unique_id, dist_group)
         self.chain = engine.AoChain(ctx, ao_options)
+        if traa is not None:  # before the attach: the group maps the tail's history plane then
+            self.chain.enable_traa(traa)
         g = C.c_void_p()
         ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, self.rank, self.world, C.byref(g)))
         self.g = g
@@ -547,10 +566,10 @@ class ShardedAoChain(ShardedSsgiChain):
         self.rebalance_every = rebalance_every
         self._host = None
 
-    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, stream=None):
-        """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective."""
-        f = self.chain._frame(cam_u, depth, velocity, normal, inp, out)
-        self.ctx._chk(self.lib.rfx_ao_chain_render_sharded(self.chain.h, stream, self._C.byref(f)))
+    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, stream=None, traa_cam=None, camera_moved: bool = True):
+        """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective.
+        traa_cam / camera_moved: as AoChain.render, with the TRAA tail on."""
+        _render_ao_band(self.ctx, self.chain, stream, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
 
     def download_band(self, which: int = 1):
         """this rank's rows of AoChain output `which` of the last frame (numpy)"""
@@ -564,7 +583,8 @@ class ShardedAoChain(ShardedSsgiChain):
 class InProcessAoGroup(InProcessGroup):
     """InProcessGroup for the AO chain (rfx_group_attach_ao_chains_inprocess): every member owns an AoChain with the same options."""
 
-    def __init__(self, ctxs, ao_options, world: int):
+    def __init__(self, ctxs, ao_options, world: int, traa=None):
+        """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None"""
         import ctypes as C
 
         from . import engine
@@ -574,6 +594,9 @@ class InProcessAoGroup(InProcessGroup):
         assert len(self.ctxs) == world
         self.lib = self.ctxs[0].lib
         self.chains = [engine.AoChain(c, ao_options) for c in self.ctxs]
+        if traa is not None:
+            for ch in self.chains:
+                ch.enable_traa(traa)
         self.groups = []
         for r, c in enumerate(self.ctxs):
             g = C.c_void_p()
@@ -583,12 +606,12 @@ class InProcessAoGroup(InProcessGroup):
         ca = (C.c_void_p * world)(*[ch.h.value for ch in self.chains])
         self.ctxs[0]._chk(self.lib.rfx_group_attach_ao_chains_inprocess(ga, ca, world))
 
-    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, wait: bool = True):
-        """one frame: every member renders its band (its rows of `out` too); all of them finish before the next frame starts"""
+    def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, wait: bool = True, traa_cam=None, camera_moved: bool = True):
+        """one frame: every member renders its band (its rows of `out` too); all of them finish before the next frame starts.
+        traa_cam / camera_moved: as AoChain.render, with the TRAA tail on."""
         self._last_bounds = self.bounds
         for c, ch in zip(self.ctxs, self.chains):
-            f = ch._frame(cam_u, depth, velocity, normal, inp, out)
-            c._chk(self.lib.rfx_ao_chain_render_sharded(ch.h, None, self._C.byref(f)))
+            _render_ao_band(c, ch, None, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
         if wait or len(set(self.ctxs)) > 1:
             for c in set(self.ctxs):
                 c.sync()
