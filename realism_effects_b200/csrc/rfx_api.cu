@@ -936,8 +936,31 @@ struct HistPlane {
   rfx_plane buf[2]{};
   PeerPV view[2]{};
 };
-struct rfx_ssgi_chain {
-  rfx_ctx* ctx;
+// The TRAA frame tail a chain can end with (rfx_*_chain_enable_traa): TRAAEffect's temporal pass over `mid` into the accumulated plane,
+// then K9.  `mid` is the composer buffer before the TRAA EffectPass: the SSGI chain's K5 output (per-pass tail only; the fused fast tail
+// has none), the AO chain's K7 output.
+struct TraaTail {
+  bool on = false;
+  rfx_traa_tail_options opt{};
+  HistPlane acc;        // accumulated plane by tail parity (buf[prev] is the history)
+  rfx_plane mid{};
+  rfx_plane out{};      // K9 output (SSGI; the AO tail writes frame->output)
+  uint64_t frames = 0;  // tails rendered; acc.buf[frames & 1] is written next
+  float keep = 0.0f;    // keepData of the TRAA pass
+  int cur() const { return (int)(frames & 1); }
+  const rfx_plane& latest() const { return acc.buf[(frames + 1) & 1]; }  // the accumulated plane of the latest frame
+  void advance() { keep = 1.0f; frames++; }  // after a frame's tail: keep the history from now on
+};
+// What a row-sharded group (rfx_group.inl) needs of a member chain; both chain kinds derive from it.
+struct GroupMember {
+  rfx_ctx* ctx = nullptr;
+  struct rfx_group* group = nullptr;  // row-sharded group the chain is attached to (rfx_group_attach_*)
+  // attached to a group of n > 1 (the SSGI fast chain excepted): the peer / carry instantiations and both buffers of every plane the chain
+  // keeps are in use.  A frame's kernels read last frame's rows on their owners and carry the texels of discarded pixels from there.
+  bool group_peer = false;
+  TraaTail tail;
+};
+struct rfx_ssgi_chain : GroupMember {
   rfx_ssgi_chain_options opt;
   rfx_plane ssgi_out{};
   // per-pass chain: single-buffered alone (buffer 0, rendered in place); buffer 1 of each plane the chain keeps is added by a group of
@@ -951,7 +974,6 @@ struct rfx_ssgi_chain {
   // the Poisson targets A / B of the fast chain, both planes of a target interleaved in one 16-byte texel (typed RGBA32F for their
   // size).  fdnA.buf[1] is used by row-sharded groups only (the A target double-buffered like B, see chain_render_fast).
   HistPlane fdnA, fdnB;
-  struct rfx_group* group = nullptr;  // row-sharded group this chain is attached to (rfx_group_attach_chain)
   uint64_t frame_idx = 0;    // frames completed (advances with the frame's last launch)
   bool views_valid = false;  // tr[]/dnB[] hold the split views of the current frame's interleaved planes
   // host-buffer entry points: two staging sets so frame i+1 uploads while frame i renders; H2D, kernels and D2H each get
@@ -968,21 +990,11 @@ struct rfx_ssgi_chain {
   float keep_data = 0.0f;  // SSGIEffect's constructor resets the denoiser (makeOptionsReactive -> reset())
   // blue-noise counters: one closure per material (BlueNoiseUtils.js:17-33)
   int32_t bn_trace = 0, bn_poisson = 0;
-  // TRAA frame tail (rfx_ssgi_chain_enable_traa): one more launch after K4
-  bool traa_on = false;
-  rfx_traa_tail_options traa{};
-  HistPlane traa_acc;                   // accumulated plane by tail parity (buf[prev] is the history)
-  rfx_plane traa_out{};                 // K9 output
-  rfx_plane traa_k5{};                  // K5 plane of the per-pass tail (chains other than the fast one, and the fast one with a debug view)
-  uint64_t traa_frames = 0;             // tails rendered; traa_acc.buf[traa_frames & 1] is written next
-  float traa_keep = 0.0f;               // keepData of the TRAA pass
-  rfx_temporal_params traa_tp{};        // the frame's camera and the previous-frame matrices its K2 used
+  // the TRAA tail (`tail`, one more launch after K4) reads the frame's camera and the previous-frame matrices its K2 used
+  rfx_temporal_params traa_tp{};
   // debug view of the tail's K5 (rfx_ssgi_chain_set_debug_view); RFX_DEBUG_VIEW_NONE: composed, isDebug off
   int32_t debug_view = RFX_DEBUG_VIEW_NONE;
   rfx_plane debug_gb{};                 // GBufferDebugPass target of the G-buffer channel views
-  // per-pass chain (not the fast one) attached to a group of n > 1: the peer / carry instantiations and both buffers of every plane
-  // it keeps are in use.  A frame's kernels read last frame's rows on their owners and carry the texels of discarded pixels from there.
-  bool group_peer = false;
   // optional per-pass event timing
   bool profiling = false;
   struct Span { cudaEvent_t a, b; int slot; };
@@ -1004,11 +1016,36 @@ static void set_view(HistPlane& h, int b, const void* const* base, int n) {
 static void local_views(HistPlane& h) {
   for (int b = 0; b < 2; b++) set_view(h, b, &h.buf[b].ptr, 1);
 }
-static std::array<HistPlane*, 10> every_hist_plane(rfx_ssgi_chain* ch) {  // whether the chain's configuration keeps it or not
-  return {&ch->composed, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->fdnA, &ch->fdnB, &ch->traa_acc};
+static std::array<HistPlane*, 9> every_hist_plane(rfx_ssgi_chain* ch) {  // whether the chain's configuration keeps it or not (the tail's aside)
+  return {&ch->composed, &ch->tr[0], &ch->tr[1], &ch->dnA[0], &ch->dnA[1], &ch->dnB[0], &ch->dnB[1], &ch->fdnA, &ch->fdnB};
 }
-// per-pass chain: the buffer of every plane it keeps that holds the latest frame (rfx_group.inl)
-static int pass_latest(const rfx_ssgi_chain* ch);
+// per-pass chain and AO chain: the buffer of every plane they keep that holds the latest frame (rfx_group.inl)
+static int pass_latest(const GroupMember* ch);
+
+static void traa_free(rfx_ctx* ctx, TraaTail& t) {
+  for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid}) if (p->ptr) rfx_plane_free(ctx, p);
+}
+// rfx_*_chain_enable_traa once the chain kind's own checks passed: NULL frees the tail's planes.  Otherwise the planes are allocated on
+// first use (`out` and `mid` where the chain asks for them; nothing is left allocated on failure), and the options replace the old ones.
+static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_options* opt, uint32_t W, uint32_t H, bool with_out, bool with_mid) {
+  if (!opt) {
+    CU(cudaStreamSynchronize(ctx->stream));
+    traa_free(ctx, t);
+    t.on = false;
+    return RFX_OK;
+  }
+  if (!t.acc.buf[0].ptr) {
+    rfx_status st = RFX_OK;
+    for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], with_out ? &t.out : nullptr, with_mid ? &t.mid : nullptr})
+      if (p && st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, p);
+    if (st != RFX_OK) { traa_free(ctx, t); return st; }
+    local_views(t.acc);
+  }
+  t.opt = *opt;
+  t.on = true;
+  t.keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
+  return RFX_OK;
+}
 
 static cudaEvent_t chain_event(rfx_ssgi_chain* ch) {
   if (!ch->event_pool.empty()) { cudaEvent_t e = ch->event_pool.back(); ch->event_pool.pop_back(); return e; }
@@ -1079,7 +1116,8 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   if (ch->s_dn) cudaStreamSynchronize(ch->s_dn);
   for (HistPlane* h : every_hist_plane(ch))
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ctx, &p);
-  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->traa_out, &ch->traa_k5, &ch->debug_gb,
+  traa_free(ctx, ch->tail);
+  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->debug_gb,
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
   for (IPlane* p : {&ch->nrdz, &ch->tr32}) if (p->p) cudaFree(p->p);
@@ -1128,36 +1166,15 @@ rfx_status rfx_ssgi_chain_set_options(rfx_ssgi_chain* ch, const rfx_ssgi_chain_o
 rfx_status rfx_ssgi_chain_reset(rfx_ssgi_chain* ch) {
   if (!ch) return RFX_ERR_INVALID_ARG;
   ch->keep_data = 0.0f;  // TemporalReprojectPass.reset()  :158-160
-  ch->traa_keep = 0.0f;  // the TRAA pass's too (TRAAEffect.reset)
+  ch->tail.keep = 0.0f;  // the TRAA pass's too (TRAAEffect.reset)
   return RFX_OK;
 }
 
 rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_options* opt) {
   if (!ch) return RFX_ERR_INVALID_ARG;
-  rfx_ctx* ctx = ch->ctx;
-  if (ch->group) return fail(ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
-  if (!opt) {
-    CU(cudaStreamSynchronize(ctx->stream));
-    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
-    ch->traa_on = false;
-    return RFX_OK;
-  }
-  if (!ch->traa_out.ptr) {
-    rfx_status st = RFX_OK;
-    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out})
-      if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
-    if (st == RFX_OK && (!ch->fastpath || ch->debug_view != RFX_DEBUG_VIEW_NONE))  // the fast chain's fused tail needs no K5 plane
-      st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
-    if (st != RFX_OK) {
-      for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_out, &ch->traa_k5}) if (p->ptr) rfx_plane_free(ctx, p);
-      return st;
-    }
-    local_views(ch->traa_acc);
-  }
-  ch->traa = *opt;
-  ch->traa_on = true;
-  ch->traa_keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
-  return RFX_OK;
+  if (ch->group) return fail(ch->ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
+  const bool k5 = !ch->fastpath || ch->debug_view != RFX_DEBUG_VIEW_NONE;  // the fast chain's fused tail needs no K5 plane
+  return traa_enable(ch->ctx, ch->tail, opt, ch->opt.width, ch->opt.height, true, k5);
 }
 
 }  // extern "C"
@@ -1186,8 +1203,8 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* o
   rfx_ctx* ctx = ch->ctx;
   if (which < 0 || which > 7) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..7");
   if (which >= 6) {
-    if (!ch->traa_on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
-    *out = which == 6 ? ch->traa_out : ch->traa_acc.buf[(ch->traa_frames + 1) & 1];
+    if (!ch->tail.on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
+    *out = which == 6 ? ch->tail.out : ch->tail.latest();
     return RFX_OK;
   }
   if (ch->fastpath) {
@@ -1236,8 +1253,8 @@ rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* ch, int32_t view) {
   rfx_status st = RFX_OK;
   if (ch->fastpath && plane && view >= RFX_DEBUG_VIEW_OUTPUT + 2) st = alloc_split_views(ch);
   if (st == RFX_OK && channel && !ch->debug_gb.ptr) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->debug_gb);
-  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->traa_on && !ch->traa_k5.ptr)  // the tail's K5 plane (the fused fast tail has none)
-    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->traa_k5);
+  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->tail.on && !ch->tail.mid.ptr)  // the tail's K5 plane (the fused fast tail has none)
+    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->tail.mid);
   if (st != RFX_OK) return st;
   ch->debug_view = view;
   return RFX_OK;
@@ -1317,27 +1334,28 @@ static rfx_status debug_view_plane(rfx_ssgi_chain* ch, void* stream, const rfx_s
 
 // The TRAA pass of a chain's frame tail (TRAAEffect, shared by the SSGI and AO chains).  traa_params: K2's uniforms, TRAAEffect's forced
 // options (TRAAEffect.js:21-31) over the TemporalReprojectPass defaults, on cam_tp's camera and previous-frame matrices.
-static rfx_temporal_params traa_params(const rfx_temporal_params& cam_tp, const rfx_traa_tail_options& o, float keep, int32_t camera_moved) {
+static rfx_temporal_params traa_params(const TraaTail& t, const rfx_temporal_params& cam_tp, int32_t camera_moved) {
+  const rfx_traa_tail_options& o = t.opt;
   rfx_temporal_params tp = cam_tp;
   tp.max_blend = o.max_blend; tp.neighborhood_clamp_intensity = o.neighborhood_clamp_intensity;
   tp.confidence_power = o.confidence_power; tp.log_transform = o.log_transform ? 1 : 0;
-  tp.keep_data = keep;
+  tp.keep_data = t.keep;
   tp.full_accumulate = o.full_accumulate && !camera_moved ? 1 : 0;
   tp.texture_count = 1; tp.input_type = RFX_INPUT_DIFFUSE; tp.history_linear = 1;
   tp.reproject_specular[0] = tp.reproject_specular[1] = 0;
   return tp;
 }
-// K2 in its TRAA form over `input` on the output rows kr +- 1 (K9's LINEAR fetch) into buffer `cur` of the accumulated plane, reading last
-// frame's buffer cur ^ 1 (in a row-sharded group of n > 1, `peer`: on the rank that owns each row), then K9 from it into `out` on kr.
-// `input` must hold rows kr +- RFX_TRAA_TAIL_ROWS.
-static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_params& tp, const rfx_plane* input, const rfx_plane* velocity,
-                                HistPlane& acc, int cur, bool peer, const rfx_plane* out, Rows kr) {
-  const int H = (int)acc.buf[cur].height;
+// K2 in its TRAA form over the tail's `mid` on the output rows kr +- 1 (K9's LINEAR fetch) into buffer cur() of the accumulated plane,
+// reading last frame's other buffer (in a row-sharded group of n > 1, `peer`: on the rank that owns each row), then K9 from it into `out`
+// on kr.  `mid` must hold rows kr +- RFX_TRAA_TAIL_ROWS.
+static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_params& tp, TraaTail& t, const rfx_plane* velocity, bool peer,
+                                const rfx_plane* out, Rows kr) {
+  const int cur = t.cur(), H = (int)t.acc.buf[cur].height;
   TemporalPeer tpeer{};
-  tpeer.hist0 = tpeer.hist1 = acc.view[cur ^ 1];
-  rfx_status st = temporal_reproject(ctx, stream, &tp, input, velocity, &acc.buf[cur ^ 1], nullptr, &acc.buf[cur], nullptr, std::max(0, kr.r0 - 1),
+  tpeer.hist0 = tpeer.hist1 = t.acc.view[cur ^ 1];
+  rfx_status st = temporal_reproject(ctx, stream, &tp, &t.mid, velocity, &t.acc.buf[cur ^ 1], nullptr, &t.acc.buf[cur], nullptr, std::max(0, kr.r0 - 1),
                                      std::min(H, kr.r1 + 1), peer ? &tpeer : nullptr);
-  if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+  if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &t.acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
   return st;
 }
 
@@ -1348,8 +1366,8 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   rfx_ctx* ctx = ch->ctx;
   const int W = (int)ch->opt.width, H = (int)ch->opt.height;
   const Rows kr = launch_rows(ranges, k, H);
-  const int cur = (int)(ch->traa_frames & 1), prev = cur ^ 1;
-  const rfx_temporal_params tp = traa_params(ch->traa_tp, ch->traa, ch->traa_keep, f->camera_moved);
+  TraaTail& tail = ch->tail;
+  const rfx_temporal_params tp = traa_params(tail, ch->traa_tp, f->camera_moved);
   const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
   if (ch->fastpath && !debug) {
     CTraaArgs a{};
@@ -1363,31 +1381,30 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
       return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: the TRAA tail needs an RGBA16F direct light plane");
     if (c.scene.w != W || c.scene.h != H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "chain: the direct light plane must match the chain size");
     c.W = W; c.H = H; c.row0 = 0; c.row1 = H;
-    const rfx_ssgi_compose_params& q = ch->traa.compose;
+    const rfx_ssgi_compose_params& q = tail.opt.compose;
     c.use_fog = q.use_fog; c.fog_exp2 = q.fog_exp2; c.perspective = q.perspective; c.is_debug = q.is_debug;
     memcpy(c.fog_color, q.fog_color, 12);
     c.fog_near = q.fog_near; c.fog_far = q.fog_far; c.fog_density = q.fog_density; c.camera_near = q.camera_near; c.camera_far = q.camera_far;
-    a.hist = ch->traa_acc.view[prev];
-    a.acc = rov(ch->traa_acc.buf[cur]);
-    a.out = rov(ch->traa_out);
+    a.hist = tail.acc.view[tail.cur() ^ 1];
+    a.acc = rov(tail.acc.buf[tail.cur()]);
+    a.out = rov(tail.out);
     LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
   } else {
     const int halo = RFX_TRAA_TAIL_ROWS;
     rfx_status st = RFX_OK;
-    rfx_ssgi_compose_params q = ch->traa.compose;
+    rfx_ssgi_compose_params q = tail.opt.compose;
     const rfx_plane* view = composed;
     if (debug && st == RFX_OK) {
       q.is_debug = 1;
       st = debug_view_plane(ch, stream, f, &view);
     }
     if (st == RFX_OK)
-      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &ch->traa_k5, (uint32_t)std::max(0, kr.r0 - halo),
+      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &tail.mid, (uint32_t)std::max(0, kr.r0 - halo),
                                    (uint32_t)std::min(H, kr.r1 + halo));
-    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, &ch->traa_k5, f->velocity, ch->traa_acc, cur, ch->group_peer, &ch->traa_out, kr);
+    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, tail, f->velocity, ch->group_peer, &tail.out, kr);
     if (st != RFX_OK) return st;
   }
-  ch->traa_keep = 1.0f;
-  ch->traa_frames++;
+  tail.advance();
   return RFX_OK;
 }
 
@@ -1543,8 +1560,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     LAUNCHED(launch_ccompose(a, cs));
   }
   // ---- TRAA tail (reads this frame's `composed`, so it runs before the planes change parity)
-  if (ch->traa_on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed.buf[cur], ranges, k_compose + 1)) != RFX_OK) return st;
-  if (on(ch->traa_on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
+  if (ch->tail.on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed.buf[cur], ranges, k_compose + 1)) != RFX_OK) return st;
+  if (on(ch->tail.on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
   return RFX_OK;
 }
 
@@ -1553,7 +1570,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
 // recompute locally (rfx_shard_ranges).  Only launches k in [k_begin, k_end) are issued, so a caller can wait between two
 // launches of a frame (rfx_ssgi_chain_submit_host waits before K4); per-frame state advances with the launch that consumes it.
 static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t k_begin, uint32_t k_end) {
-  if (ch->traa_on && !f->direct_light) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail composes over the direct light plane (the composer input buffer): it may not be NULL");
+  if (ch->tail.on && !f->direct_light) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail composes over the direct light plane (the composer input buffer): it may not be NULL");
   if (ch->fastpath) return chain_render_fast(ch, stream, f, ranges, k_begin, k_end);
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
@@ -1668,7 +1685,7 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
   }
   k++;
   // ---- TRAA tail over the effect's output (`composed`, or the temporal texture in denoiseMode "temporal")
-  if (ch->traa_on && on(k)) return chain_render_tail(ch, stream, f, &accumulated.buf[wr], ranges, k);
+  if (ch->tail.on && on(k)) return chain_render_tail(ch, stream, f, &accumulated.buf[wr], ranges, k);
   return RFX_OK;
 }
 
@@ -1762,30 +1779,17 @@ rfx_status rfx_ssgi_chain_render_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
 // ==========================================================================================
 // native AO chain: HBAOEffect.update / HorizonAOEffect.update (K6 or K6h -> K3 x 2*iterations -> K7) in one call
 // ==========================================================================================
-struct rfx_ao_chain {
-  rfx_ctx* ctx;
+struct rfx_ao_chain : GroupMember {
   rfx_ao_chain_options opt;
   float luma_phi, depth_phi, normal_phi;  // the denoiser's values: opt's, clamped where a setter changed them (AOEffect.js:106-110)
   // the planes a frame leaves for the next (a discarded pixel keeps its texel): alone single-buffered (buffer 0, rendered in place);
   // buffer 1 is added by a group of n > 1 (group_alloc_history)
   HistPlane target, dnA, dnB;
   int32_t bn_ao = 0, bn_dn = 0;  // the AO pass's and the denoiser's BlueNoiseIndex
-  struct rfx_group* group = nullptr;
-  bool group_peer = false;  // attached to a group of n > 1: double-buffered planes, carry instantiations
-  // TRAA frame tail (rfx_ao_chain_enable_traa): K7 into traa_k7, then the TRAA pass and K9 into frame->output
-  bool traa_on = false;
-  rfx_traa_tail_options traa{};
-  HistPlane traa_acc;             // accumulated plane by tail parity (buf[prev] is the history)
-  rfx_plane traa_k7{};            // K7 output: the composer buffer between the AO and the TRAA EffectPass
-  uint64_t traa_frames = 0;       // tails rendered; traa_acc.buf[traa_frames & 1] is written next
-  float traa_keep = 0.0f;         // keepData of the TRAA pass
+  // the TRAA tail (`tail`: K7 into tail.mid, then the TRAA pass and K9 into frame->output) reads the previous frame's camera
   bool traa_have_prev = false;    // traa_prev holds the previous frame's camera
   rfx_ao_traa_frame traa_prev{};
 };
-static void free_traa(rfx_ao_chain* ch) {
-  for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_k7}) if (p->ptr) rfx_plane_free(ch->ctx, p);
-}
-static int pass_latest(const rfx_ao_chain* ch);  // the buffer of every plane that holds the latest frame (rfx_group.inl)
 
 static void ao_target_size(const rfx_ao_chain_options& o, uint32_t& w, uint32_t& h, float& rx, float& ry) {
   const double s = o.resolution_scale == 0.0f ? 1.0 : (double)o.resolution_scale;
@@ -1824,7 +1828,7 @@ void rfx_ao_chain_destroy(rfx_ao_chain* ch) {
   cudaStreamSynchronize(ch->ctx->stream);
   for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ch->ctx, &p);
-  free_traa(ch);
+  traa_free(ch->ctx, ch->tail);
   delete ch;
 }
 
@@ -1848,12 +1852,12 @@ rfx_status rfx_ao_chain_set_options(rfx_ao_chain* ch, const rfx_ao_chain_options
 rfx_status rfx_ao_chain_reset(rfx_ao_chain* ch) {
   if (!ch) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
-  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB, &ch->traa_acc})
+  for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB, &ch->tail.acc})
     for (const rfx_plane& p : h->buf)
       if (p.ptr) CU(cudaMemset2DAsync(p.ptr, p.pitch, 0, (size_t)p.width * 8, p.height, ctx->stream));
   ch->bn_ao = ch->bn_dn = 0;
   ch->luma_phi = ch->opt.luma_phi; ch->depth_phi = ch->opt.depth_phi; ch->normal_phi = ch->opt.normal_phi;
-  ch->traa_keep = 0.0f;  // a new TRAA pass: keepData 0, and the first frame's previous camera is its own
+  ch->tail.keep = 0.0f;  // a new TRAA pass: keepData 0, and the first frame's previous camera is its own
   ch->traa_have_prev = false;
   return RFX_OK;
 }
@@ -1863,32 +1867,16 @@ rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* ch, const rfx_traa_tail_option
   rfx_ctx* ctx = ch->ctx;
   if (ch->group && rfx_group_world(ch->group) > 1)
     return fail(ctx, RFX_ERR_UNSUPPORTED, "ao_chain_enable_traa: the chain is in a row-sharded group, whose peer mappings are fixed at attach time");
-  if (!opt) {
-    CU(cudaStreamSynchronize(ctx->stream));
-    free_traa(ch);
-    ch->traa_on = false;
-    return RFX_OK;
-  }
   static const rfx_ssgi_compose_params no_compose{};
-  if (memcmp(&opt->compose, &no_compose, sizeof no_compose) != 0)
+  if (opt && memcmp(&opt->compose, &no_compose, sizeof no_compose) != 0)
     return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_enable_traa: the AO tail has no K5: `compose` must be all zero");
-  if (!ch->traa_k7.ptr) {
-    rfx_status st = RFX_OK;
-    for (rfx_plane* p : {&ch->traa_acc.buf[0], &ch->traa_acc.buf[1], &ch->traa_k7})
-      if (st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, p);
-    if (st != RFX_OK) { free_traa(ch); return st; }
-    local_views(ch->traa_acc);
-  }
-  ch->traa = *opt;
-  ch->traa_on = true;
-  ch->traa_keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
-  return RFX_OK;
+  return traa_enable(ctx, ch->tail, opt, ch->opt.width, ch->opt.height, false, true);
 }
 
 rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
-  if (ch->traa_on && (which == 2 || which == 3)) {
-    *out = which == 2 ? ch->traa_k7 : ch->traa_acc.buf[(ch->traa_frames + 1) & 1];
+  if (ch->tail.on && (which == 2 || which == 3)) {
+    *out = which == 2 ? ch->tail.mid : ch->tail.latest();
     return RFX_OK;
   }
   if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1 (2 / 3 with the TRAA tail on)");
@@ -1977,7 +1965,7 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     memcpy(cp.color, o.color, 12);
     const Rows kr = launch_rows(ranges, k, (int)o.height);
     const HistPlane& tex = o.iterations > 0 ? ch->dnB : ch->target;
-    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, t ? &ch->traa_k7 : f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, t ? &ch->tail.mid : f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
     if (st != RFX_OK) return st;
   }
   k++;
@@ -1989,12 +1977,10 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     memcpy(cam.prev_view_matrix, prev.cam.view_matrix, 64); memcpy(cam.prev_camera_matrix_world, prev.cam.camera_matrix_world, 64);
     memcpy(cam.prev_projection, prev.cam.projection, 64); memcpy(cam.prev_projection_inverse, prev.cam.projection_inverse, 64);
     memcpy(cam.camera_pos, t->camera_pos, 12); memcpy(cam.prev_camera_pos, prev.camera_pos, 12);
-    const rfx_temporal_params tp = traa_params(cam, ch->traa, ch->traa_keep, t->camera_moved);
-    st = traa_launches(ctx, stream, tp, &ch->traa_k7, f->velocity, ch->traa_acc, (int)(ch->traa_frames & 1), ch->group_peer, f->output,
+    st = traa_launches(ctx, stream, traa_params(ch->tail, cam, t->camera_moved), ch->tail, f->velocity, ch->group_peer, f->output,
                        launch_rows(ranges, k, (int)o.height));
     if (st != RFX_OK) return st;
-    ch->traa_keep = 1.0f;
-    ch->traa_frames++;
+    ch->tail.advance();
     ch->traa_prev = *t;
     ch->traa_have_prev = true;
   }
@@ -2003,8 +1989,8 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
 
 // The entry points: the tail's camera is given exactly when the tail is on.
 static rfx_status ao_check_traa(rfx_ao_chain* ch, const rfx_ao_traa_frame* t, const char* who) {
-  if (ch->traa_on && !t) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "%s: the TRAA tail is on and needs the camera (render with the _traa entry point)", who);
-  if (!ch->traa_on && t) return fail(ch->ctx, RFX_ERR_NOT_READY, "%s: the TRAA tail is off (rfx_ao_chain_enable_traa)", who);
+  if (ch->tail.on && !t) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "%s: the TRAA tail is on and needs the camera (render with the _traa entry point)", who);
+  if (!ch->tail.on && t) return fail(ch->ctx, RFX_ERR_NOT_READY, "%s: the TRAA tail is off (rfx_ao_chain_enable_traa)", who);
   return RFX_OK;
 }
 

@@ -232,39 +232,67 @@ class Context:
                                                      _r(depth), _r(out_gbuffer), _r(out_velocity), rows[0], rows[1]))
 
 
-class SsgiChain:
-    """Native SSGI chain (rfx_ssgi_chain): K1 -> K2 -> K3 x 2*iterations -> K4 with history."""
+class _Chain:
+    """What SsgiChain and AoChain share: an rfx_<kind>_chain handle (`_PREFIX`), its lifecycle, its TRAA frame tail and its outputs."""
 
-    def __init__(self, ctx: Context, opt: abi.ChainOptions):
-        self.ctx = ctx
-        self.opt = opt
+    _PREFIX = ""
+    _DEFAULT_OUTPUT = 0  # output() / download() without `which`
+
+    def __init__(self, ctx: Context, opt):
+        self.ctx, self.opt = ctx, opt
         self.traa = None
         h = C.c_void_p()
-        ctx._chk(ctx.lib.rfx_ssgi_chain_create(ctx.h, C.byref(opt), C.byref(h)))
+        ctx._chk(self._fn("create")(ctx.h, C.byref(opt), C.byref(h)))
         self.h = h
+
+    def _fn(self, name: str):
+        return getattr(self.ctx.lib, f"{self._PREFIX}_{name}")
 
     def close(self):
         if self.h:
-            self.ctx.lib.rfx_ssgi_chain_destroy(self.h)
+            self._fn("destroy")(self.h)
             self.h = None
 
     def reset(self):
-        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_reset(self.h))
+        self.ctx._chk(self._fn("reset")(self.h))
 
-    def set_options(self, opt: abi.ChainOptions):
-        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_set_options(self.h, C.byref(opt)))
+    def set_options(self, opt):
+        self.ctx._chk(self._fn("set_options")(self.h, C.byref(opt)))
         self.opt = opt
 
     def enable_traa(self, options: "abi.TraaTailOptions | None" = None, enable: bool = True):
-        """TRAA frame tail (K5 -> TRAA -> K9 after K4, include/rfx.h: rfx_ssgi_chain_enable_traa): outputs 6 (the K9 frame) and 7 (the
-        TRAA accumulated plane).  options: abi.make_traa_tail_options(...) (default: TRAAEffect's values, no fog); enable=False turns it off.
+        """TRAA frame tail (include/rfx.h: rfx_<kind>_chain_enable_traa; the class docstring names its outputs).  options:
+        abi.make_traa_tail_options(...) (default: TRAAEffect's values, no fog; the AO tail takes no `compose`); enable=False turns it off.
         Enabling again replaces the options and resets the TRAA history."""
         if not enable:
-            self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_enable_traa(self.h, None))
+            self.ctx._chk(self._fn("enable_traa")(self.h, None))
             self.traa = None
             return
         self.traa = options if options is not None else abi.make_traa_tail_options()
-        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_enable_traa(self.h, C.byref(self.traa)))
+        self.ctx._chk(self._fn("enable_traa")(self.h, C.byref(self.traa)))
+
+    def output(self, which: int | None = None) -> Plane:
+        """chain output `which` (the class docstring lists them; default: _DEFAULT_OUTPUT)"""
+        p = Plane()
+        self.ctx._chk(self._fn("output")(self.h, self._DEFAULT_OUTPUT if which is None else which, C.byref(p)))
+        return p
+
+    def download(self, which: int | None = None) -> np.ndarray:
+        p = self.output(which)
+        dt, ch = _NP_OF[p.format]
+        out = np.empty((p.height, p.width, ch), dt)
+        self.ctx.sync()
+        self.ctx._chk(self.ctx.lib.rfx_plane_download(self.ctx.h, None, C.byref(p), out.ctypes.data_as(C.c_void_p), 0))
+        self.ctx.sync()
+        return out
+
+
+class SsgiChain(_Chain):
+    """Native SSGI chain (rfx_ssgi_chain): K1 -> K2 -> K3 x 2*iterations -> K4 with history, and optionally the TRAA frame tail (K5 ->
+    TRAA -> K9 after K4).  Outputs: 0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA
+    accumulated plane."""
+
+    _PREFIX = "rfx_ssgi_chain"
 
     def set_debug_view(self, view: int):
         """the TRAA tail's K5 shows `view` (abi.DEBUG_VIEW_*; include/rfx.h: rfx_ssgi_chain_set_debug_view) instead of composed"""
@@ -285,21 +313,6 @@ class SsgiChain:
     def render(self, cam: abi.CameraS, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None):
         f = self._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render(self.h, stream, C.byref(f)))
-
-    def output(self, which: int = 0) -> Plane:
-        """0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA accumulated plane"""
-        p = Plane()
-        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_output(self.h, which, C.byref(p)))
-        return p
-
-    def download(self, which: int = 0) -> np.ndarray:
-        p = self.output(which)
-        dt, ch = _NP_OF[p.format]
-        out = np.empty((p.height, p.width, ch), dt)
-        self.ctx.sync()
-        self.ctx._chk(self.ctx.lib.rfx_plane_download(self.ctx.h, None, C.byref(p), out.ctypes.data_as(C.c_void_p), 0))
-        self.ctx.sync()
-        return out
 
     PROFILE_SLOTS = ("K1_ssgi_trace", "K2_temporal_reproject", "K3_poisson_pass0", "K3_poisson_pass1plus", "K4_gi_compose")
 
@@ -351,28 +364,14 @@ def ao_chain_options(width: int, height: int, options: dict | None = None, horiz
     return c
 
 
-class AoChain:
+class AoChain(_Chain):
     """Native AO chain (rfx_ao_chain): K6 or K6h -> K3 x 2*iterations -> K7 in one call, the launches of HBAOEffect.update /
-    HorizonAOEffect.update.  Options: ao_chain_options(...)."""
+    HorizonAOEffect.update, and optionally the TRAA frame tail (K7 -> TRAA -> K9): render() then takes the TRAA camera and writes the K9
+    frame to `out`.  Options: ao_chain_options(...).  Outputs: 0 the AO target, 1 the denoised plane K7 composes (the AO target with
+    iterations 0); with the TRAA tail on, 2 the K7 plane and 3 the TRAA accumulated plane."""
 
-    def __init__(self, ctx: Context, opt: abi.AoChainOptions):
-        self.ctx, self.opt = ctx, opt
-        self.traa = None
-        h = C.c_void_p()
-        ctx._chk(ctx.lib.rfx_ao_chain_create(ctx.h, C.byref(opt), C.byref(h)))
-        self.h = h
-
-    def close(self):
-        if self.h:
-            self.ctx.lib.rfx_ao_chain_destroy(self.h)
-            self.h = None
-
-    def reset(self):
-        self.ctx._chk(self.ctx.lib.rfx_ao_chain_reset(self.h))
-
-    def set_options(self, opt: abi.AoChainOptions):
-        self.ctx._chk(self.ctx.lib.rfx_ao_chain_set_options(self.h, C.byref(opt)))
-        self.opt = opt
+    _PREFIX = "rfx_ao_chain"
+    _DEFAULT_OUTPUT = 1
 
     @staticmethod
     def _frame(cam_u: dict, depth, velocity, normal=None, inp=None, out=None) -> abi.AoFrame:
@@ -383,17 +382,6 @@ class AoChain:
         ptr = lambda p: None if p is None else C.pointer(p.p)  # noqa: E731
         f.depth, f.velocity, f.normal, f.input, f.output = ptr(depth), ptr(velocity), ptr(normal), ptr(inp), ptr(out)
         return f
-
-    def enable_traa(self, options: "abi.TraaTailOptions | None" = None, enable: bool = True):
-        """TRAA frame tail (K7 -> TRAA -> K9, include/rfx.h: rfx_ao_chain_enable_traa): render() then takes the TRAA camera and writes the
-        K9 frame to `out`; outputs 2 (the K7 plane) and 3 (the TRAA accumulated plane).  options: abi.make_traa_tail_options(...) without
-        `compose` (default: TRAAEffect's values); enable=False turns it off.  Enabling again replaces the options and resets the TRAA history."""
-        if not enable:
-            self.ctx._chk(self.ctx.lib.rfx_ao_chain_enable_traa(self.h, None))
-            self.traa = None
-            return
-        self.traa = options if options is not None else abi.make_traa_tail_options()
-        self.ctx._chk(self.ctx.lib.rfx_ao_chain_enable_traa(self.h, C.byref(self.traa)))
 
     @staticmethod
     def _traa_frame(traa_cam: dict, camera_moved: bool) -> abi.AoTraaFrame:
@@ -414,18 +402,3 @@ class AoChain:
         else:
             t = self._traa_frame(traa_cam, camera_moved)
             self.ctx._chk(self.ctx.lib.rfx_ao_chain_render_traa(self.h, stream, C.byref(f), C.byref(t)))
-
-    def output(self, which: int = 1) -> Plane:
-        """0 the AO target, 1 the denoised plane K7 composes (the AO target with iterations 0); with the TRAA tail on, 2 the K7 plane and
-        3 the TRAA accumulated plane"""
-        p = Plane()
-        self.ctx._chk(self.ctx.lib.rfx_ao_chain_output(self.h, which, C.byref(p)))
-        return p
-
-    def download(self, which: int = 1) -> np.ndarray:
-        p = self.output(which)
-        out = np.empty((p.height, p.width, 4), np.float16)
-        self.ctx.sync()
-        self.ctx._chk(self.ctx.lib.rfx_plane_download(self.ctx.h, None, C.byref(p), out.ctypes.data_as(C.c_void_p), 0))
-        self.ctx.sync()
-        return out

@@ -31,6 +31,13 @@ import math
 from dataclasses import dataclass
 
 
+def _poisson_halo(radius: float, height: int, width: int | None) -> int:
+    """rows a Poisson tap can reach: the offset is rotated after the division by the resolution (poisson_denoise.frag:183-189), so the row
+    reach is radius * max(1, H / W); + 1 for the bilinear footprint / the quad-derivative helper row"""
+    stretch = max(1.0, height / width) if width else 1.0
+    return int(math.ceil(radius * stretch)) + 1
+
+
 @dataclass
 class ShardPlan:
     """Row ranges [a, b) per launch of one frame, in chain order: K1, K2, K3 pass 0..n-1, K4,
@@ -83,7 +90,7 @@ class ShardPlan:
             self.blocks = [self.block_of(self.rank, 0)]
             self.rows_per_rank = self.blocks[0][1] - self.blocks[0][0]
             self.r0, self.r1 = self.blocks[0]
-            self.poisson_halo = self._halo()
+            self.poisson_halo = _poisson_halo(self.radius, self.height, self.width)
             return
         nb = self.world * self.blocks_per_rank
         if self.height % nb:
@@ -92,13 +99,7 @@ class ShardPlan:
         self.rows_per_rank = self.block_rows * self.blocks_per_rank
         self.blocks = [self.block_of(self.rank, j) for j in range(self.blocks_per_rank)]
         self.r0, self.r1 = self.blocks[0]  # (single-block plans: the contiguous band)
-        self.poisson_halo = self._halo()
-
-    def _halo(self) -> int:
-        """rows a Poisson tap can reach: the offset is rotated after the division by the resolution (poisson_denoise.frag:183-189),
-        so the row reach is radius * max(1, H / W); + 1 for the bilinear footprint / the quad-derivative helper row"""
-        stretch = max(1.0, self.height / self.width) if self.width else 1.0
-        return int(math.ceil(self.radius * stretch)) + 1
+        self.poisson_halo = _poisson_halo(self.radius, self.height, self.width)
 
     def _expand(self, rng, rows):
         return (max(0, rng[0] - rows), min(self.height, rng[1] + rows))
@@ -179,7 +180,7 @@ class AoShardPlan:
 
     @property
     def poisson_halo(self) -> int:
-        return int(math.ceil(abs(self.radius) * max(1.0, self.height / self.width))) + 1
+        return _poisson_halo(abs(self.radius), self.height, self.width)
 
     @property
     def n_launches(self) -> int:
@@ -276,6 +277,7 @@ class ShardedSsgiChain:
     passed explicitly (`unique_id`, e.g. read from a file by a host without torch)."""
 
     INPUTS = (("depth", 4, True), ("gbuffer", 16, False), ("velocity", 16, True), ("direct", 8, False))  # name, bytes/px, sampled anywhere
+    _CHAIN, _ATTACH = "SsgiChain", "rfx_group_attach_chain"  # the member chain's engine class and its collective attach
 
     def __init__(self, ctx, chain_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
                  rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None):
@@ -287,13 +289,13 @@ class ShardedSsgiChain:
         self._abi, self.ctx, self.lib, self._C = abi, ctx, ctx.lib, C
         rank, world, unique_id = _group_unique_id(ctx, rank, world, unique_id, dist_group)
         self.rank, self.world = rank, world
-        self.chain = engine.SsgiChain(ctx, chain_options)
+        self.chain = getattr(engine, self._CHAIN)(ctx, chain_options)
         if traa is not None:  # before the attach: the group maps the tail's history plane then
             self.chain.enable_traa(traa)
         g = C.c_void_p()
         ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, rank, world, C.byref(g)))
         self.g = g
-        ctx._chk(self.lib.rfx_group_attach_chain(g, self.chain.h))
+        ctx._chk(getattr(self.lib, self._ATTACH)(g, self.chain.h))
         ctx._chk(self.lib.rfx_group_set_rebalance(g, int(rebalance_every), int(rebalance_lag)))
         self.rebalance_every = rebalance_every
         self._host = None
@@ -338,8 +340,8 @@ class ShardedSsgiChain:
         f = self.chain._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
         self.ctx._chk(self.lib.rfx_ssgi_chain_render_sharded(self.chain.h, stream, self._C.byref(f)))
 
-    def download_band(self, which: int = 0):
-        """this rank's rows of chain output `which` of the last frame (numpy)"""
+    def download_band(self, which: int | None = None):
+        """this rank's rows of chain output `which` (default: the chain's) of the last frame (numpy)"""
         b0, b1 = self.band_of_last_frame
         return self.chain.download(which)[b0:b1]
 
@@ -469,6 +471,8 @@ class InProcessGroup:
     renders the bands one after the other on one GPU — the N-band logic (halo recomputation, owner lookup of history rows, carried texels,
     moving borders) without N GPUs; with one context per device it is a single-process multi-GPU host."""
 
+    _CHAIN, _ATTACH = "SsgiChain", "rfx_group_attach_chains_inprocess"  # the members' engine class and their attach
+
     def __init__(self, ctxs, chain_options, world: int, traa=None):
         """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None"""
         import ctypes as C
@@ -479,7 +483,7 @@ class InProcessGroup:
         self.ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs] * world
         assert len(self.ctxs) == world
         self.lib = self.ctxs[0].lib
-        self.chains = [engine.SsgiChain(c, chain_options) for c in self.ctxs]
+        self.chains = [getattr(engine, self._CHAIN)(c, chain_options) for c in self.ctxs]
         if traa is not None:
             for ch in self.chains:
                 ch.enable_traa(traa)
@@ -490,7 +494,7 @@ class InProcessGroup:
             self.groups.append(g)
         ga = (C.c_void_p * world)(*[g.value for g in self.groups])
         ca = (C.c_void_p * world)(*[ch.h.value if hasattr(ch.h, "value") else ch.h for ch in self.chains])
-        self.ctxs[0]._chk(self.lib.rfx_group_attach_chains_inprocess(ga, ca, world))
+        self.ctxs[0]._chk(getattr(self.lib, self._ATTACH)(ga, ca, world))
 
     @property
     def bounds(self) -> tuple:
@@ -543,68 +547,26 @@ def _render_ao_band(ctx, chain, stream, frame: tuple, traa_cam, camera_moved: bo
 
 
 class ShardedAoChain(ShardedSsgiChain):
-    """This rank's member of a row-sharded AO chain: rfx_group_* + rfx_ao_chain_render_sharded.  Bands, rebalancing and the unique-id
-    exchange are ShardedSsgiChain's; the host-buffer path is not (out of scope for AO)."""
+    """This rank's member of a row-sharded AO chain: rfx_group_* + rfx_ao_chain_render_sharded.  The constructor (chain_options:
+    engine.ao_chain_options(...)), bands, rebalancing and the unique-id exchange are ShardedSsgiChain's; the host-buffer path is not (out of
+    scope for AO)."""
 
-    def __init__(self, ctx, ao_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
-                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None):
-        """traa: abi.TraaTailOptions (abi.make_traa_tail_options()) to render the TRAA tail too (the same on every rank), or None"""
-        import ctypes as C
-
-        from . import abi, engine
-
-        self._abi, self.ctx, self.lib, self._C = abi, ctx, ctx.lib, C
-        self.rank, self.world, unique_id = _group_unique_id(ctx, rank, world, unique_id, dist_group)
-        self.chain = engine.AoChain(ctx, ao_options)
-        if traa is not None:  # before the attach: the group maps the tail's history plane then
-            self.chain.enable_traa(traa)
-        g = C.c_void_p()
-        ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, self.rank, self.world, C.byref(g)))
-        self.g = g
-        ctx._chk(self.lib.rfx_group_attach_ao_chain(g, self.chain.h))
-        ctx._chk(self.lib.rfx_group_set_rebalance(g, int(rebalance_every), int(rebalance_lag)))
-        self.rebalance_every = rebalance_every
-        self._host = None
+    _CHAIN, _ATTACH = "AoChain", "rfx_group_attach_ao_chain"
 
     def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, stream=None, traa_cam=None, camera_moved: bool = True):
         """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective.
         traa_cam / camera_moved: as AoChain.render, with the TRAA tail on."""
         _render_ao_band(self.ctx, self.chain, stream, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
 
-    def download_band(self, which: int = 1):
-        """this rank's rows of AoChain output `which` of the last frame (numpy)"""
-        b0, b1 = self.band_of_last_frame
-        return self.chain.download(which)[b0:b1]
-
     def submit_host(self, *a, **k):
         raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the AO chain has no host-buffer path")
 
 
 class InProcessAoGroup(InProcessGroup):
-    """InProcessGroup for the AO chain (rfx_group_attach_ao_chains_inprocess): every member owns an AoChain with the same options."""
+    """InProcessGroup for the AO chain (rfx_group_attach_ao_chains_inprocess): every member owns an AoChain with the same options
+    (chain_options: engine.ao_chain_options(...))."""
 
-    def __init__(self, ctxs, ao_options, world: int, traa=None):
-        """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None"""
-        import ctypes as C
-
-        from . import engine
-
-        self._C, self.world = C, world
-        self.ctxs = list(ctxs) if isinstance(ctxs, (list, tuple)) else [ctxs] * world
-        assert len(self.ctxs) == world
-        self.lib = self.ctxs[0].lib
-        self.chains = [engine.AoChain(c, ao_options) for c in self.ctxs]
-        if traa is not None:
-            for ch in self.chains:
-                ch.enable_traa(traa)
-        self.groups = []
-        for r, c in enumerate(self.ctxs):
-            g = C.c_void_p()
-            c._chk(self.lib.rfx_group_create_inprocess(c.h, r, world, C.byref(g)))
-            self.groups.append(g)
-        ga = (C.c_void_p * world)(*[g.value for g in self.groups])
-        ca = (C.c_void_p * world)(*[ch.h.value for ch in self.chains])
-        self.ctxs[0]._chk(self.lib.rfx_group_attach_ao_chains_inprocess(ga, ca, world))
+    _CHAIN, _ATTACH = "AoChain", "rfx_group_attach_ao_chains_inprocess"
 
     def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, wait: bool = True, traa_cam=None, camera_moved: bool = True):
         """one frame: every member renders its band (its rows of `out` too); all of them finish before the next frame starts.
