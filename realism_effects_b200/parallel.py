@@ -1,9 +1,11 @@
 """Row-band sharding of the SSGI chain and the AO chain across N GPUs (one process per GPU).
 
 The product path is native: `rfx_group_*` / `rfx_ssgi_chain_render_sharded` in csrc/rfx_group.inl (C ABI, include/rfx.h).
-This module is the Python host binding of that API (`ShardedSsgiChain`) plus a pure-Python mirror of its host arithmetic
-(`ShardPlan`, `rebalance`) that the CPU tests check against the exported C functions `rfx_shard_ranges` / `rfx_shard_rebalance`
-and drive with the oracle as compute (tests/test_sharding_cpu.py).
+This module is the Python host binding of that API (`ShardedSsgiChain`, `ShardedAoChain`, and `InProcessGroup` / `InProcessAoGroup`
+for the members of one process) plus a pure-Python mirror of its host arithmetic that the CPU tests check against the exported C
+functions and drive with the oracle as compute (tests/test_sharding_cpu.py).  Every rank owns one contiguous row band.  `ShardPlan`
+and `AoShardPlan` give the row range of every launch of a frame for that band (`rfx_shard_ranges` / `rfx_ao_shard_ranges`): the last
+launch runs on the band, every launch before it on the next one's rows widened by what that one reads around them.
 
 Every kernel of the path writes disjoint output rows, so the produced planes are partitioned by row band (SURVEY.md §8e).
 Two kinds of inputs cross band borders:
@@ -20,8 +22,8 @@ Two kinds of inputs cross band borders:
     parity so no rank overwrites rows a peer may still read, and the frame ends with ONE tiny NCCL all-gather (each rank's
     device-timed kernel cost) that is also the frame barrier.
 
-Adaptive bands: one contiguous band per rank; every few frames the borders move towards equal device-timed cost
-(`rfx_shard_rebalance`: cost per row piecewise constant over the measured bands, damped, 16-row aligned; every rank derives the
+Adaptive bands: every few frames the borders move towards equal device-timed cost (`rfx_shard_rebalance`, mirrored by
+`rebalance`: cost per row piecewise constant over the measured bands, damped, 16-row aligned; every rank derives the
 same borders from the same gathered times).  All cross-frame state lives in the peer-readable planes, so borders move freely
 between frames and the result stays bit-identical to the single-GPU chain (tests/test_gpu_multi.py).
 """
@@ -38,20 +40,30 @@ def _poisson_halo(radius: float, height: int, width: int | None) -> int:
     return int(math.ceil(radius * stretch)) + 1
 
 
+def _widen_back(own, height: int, reaches) -> list:
+    """Row ranges [a, b) of the launches of one frame for the band `own` (mirror of widen_back in csrc/rfx_group.inl): the last launch
+    runs on the band, and every launch before it on the next launch's rows widened by what that one reads around them.  reaches[k]: the
+    rows launch k + 1 reads around its output rows, of what launch k wrote, so there is one launch more than reaches."""
+    a, b = own
+    out = [(a, b)]
+    for rows in reversed(reaches):
+        a, b = max(0, a - rows), min(height, b + rows)
+        out.append((a, b))
+    return out[::-1]
+
+
 @dataclass
 class ShardPlan:
-    """Row ranges [a, b) per launch of one frame, in chain order: K1, K2, K3 pass 0..n-1, K4,
-    for every row block this rank owns."""
+    """Row ranges [a, b) per launch of one SSGI chain frame for the contiguous band this rank owns, in chain order: K1, K2, K3 pass 0..n-1,
+    K4 and, with `traa`, the TRAA tail (mirror of rfx_shard_ranges)."""
 
     height: int
     world: int
     rank: int
     n_poisson_passes: int  # 2 * denoiseIterations
     radius: float
-    ssgi_mode: bool = True
-    blocks_per_rank: int = 1
-    mirror: bool = False  # True: odd super-blocks are assigned in REVERSE rank order (boustrophedon), see block_of()
-    bounds: tuple | None = None  # explicit band borders (world + 1 ascending rows, 0 .. height): one contiguous band per rank
+    ssgi_mode: bool = True       # as rfx_shard_ranges' ssgi_mode: the ranges do not depend on it (K4 runs in SSR mode too)
+    bounds: tuple | None = None  # band borders (world + 1 ascending rows, 0 .. height); None: equal bands of height / world rows
     width: int | None = None     # frame width: portrait frames (H > W) stretch the Poisson taps' row reach by H / W
     traa: bool = False           # the TRAA tail runs as one more launch after K4 (rfx_ssgi_chain_enable_traa)
     denoise_mode: int = 0        # 0 "full"; 1 "full_temporal" / 2 "temporal" run no Poisson pass, so their ranges are those of 0 passes
@@ -63,46 +75,17 @@ class ShardPlan:
     # the pixel centre; the TRAA form takes no derivative, so no quad row
     TRAA_TAIL_ROWS = 4
 
-    def block_of(self, rank: int, j: int):
-        """rows of the block `rank` owns inside super-block j.  With `mirror`, odd super-blocks run in reverse rank order, so a
-        rank that gets the cheapest end of one super-block (sky) gets the most expensive end of the next (floor): 2 blocks per
-        rank already balance a vertical cost gradient, at half the halo recompute of a 4-block cyclic assignment."""
-        if self.bounds is not None:
-            return (self.bounds[rank], self.bounds[rank + 1])
-        pos = (self.world - 1 - rank) if (self.mirror and j % 2 == 1) else rank
-        b = j * self.world + pos
-        return (b * self.block_rows, (b + 1) * self.block_rows)
-
-    def reversed_order(self, j: int) -> bool:
-        return self.mirror and j % 2 == 1
-
-    @property
-    def p2p(self) -> bool:
-        """the exchange cannot be a rank-ordered in-place all-gather (mirrored order or unequal bands)"""
-        return self.mirror or self.bounds is not None
-
     def __post_init__(self):
-        if self.bounds is not None:
-            b = tuple(int(x) for x in self.bounds)
-            if len(b) != self.world + 1 or b[0] != 0 or b[-1] != self.height or any(b[i] >= b[i + 1] for i in range(self.world)):
-                raise ValueError(f"bounds {b} are not {self.world + 1} ascending rows from 0 to {self.height}")
-            self.bounds, self.blocks_per_rank, self.block_rows = b, 1, None
-            self.blocks = [self.block_of(self.rank, 0)]
-            self.rows_per_rank = self.blocks[0][1] - self.blocks[0][0]
-            self.r0, self.r1 = self.blocks[0]
-            self.poisson_halo = _poisson_halo(self.radius, self.height, self.width)
-            return
-        nb = self.world * self.blocks_per_rank
-        if self.height % nb:
-            raise ValueError(f"height {self.height} is not divisible by world size x blocks per rank = {nb}")
-        self.block_rows = self.height // nb
-        self.rows_per_rank = self.block_rows * self.blocks_per_rank
-        self.blocks = [self.block_of(self.rank, j) for j in range(self.blocks_per_rank)]
-        self.r0, self.r1 = self.blocks[0]  # (single-block plans: the contiguous band)
+        if self.bounds is None:
+            if self.height % self.world:
+                raise ValueError(f"height {self.height} is not divisible by world size {self.world}")
+            self.bounds = tuple(self.height * i // self.world for i in range(self.world + 1))
+        b = tuple(int(x) for x in self.bounds)
+        if len(b) != self.world + 1 or b[0] != 0 or b[-1] != self.height or any(b[i] >= b[i + 1] for i in range(self.world)):
+            raise ValueError(f"bounds {b} are not {self.world + 1} ascending rows from 0 to {self.height}")
+        self.bounds = b
+        self.r0, self.r1 = b[self.rank], b[self.rank + 1]
         self.poisson_halo = _poisson_halo(self.radius, self.height, self.width)
-
-    def _expand(self, rng, rows):
-        return (max(0, rng[0] - rows), min(self.height, rng[1] + rows))
 
     @property
     def passes(self) -> int:
@@ -110,56 +93,26 @@ class ShardPlan:
         chain maps a full_temporal / temporal frame's K1, K2, K4 (and tail) launches onto these ranges (rfx_ssgi_chain_render_sharded)."""
         return self.n_poisson_passes if self.denoise_mode == 0 else 0
 
-    def ranges_for(self, own) -> list:
-        n = self.passes
-        k4 = self._expand(own, self.TRAA_TAIL_ROWS) if self.traa else own
-        k3 = [None] * n
-        nxt = k4
-        if n:
-            k3[n - 1] = self._expand(k4, self.K4_INPUT_ROWS)
-            for j in range(n - 2, -1, -1):
-                k3[j] = self._expand(k3[j + 1], self.poisson_halo)
-            nxt = self._expand(k3[0], self.poisson_halo)
-        k2 = nxt
-        k1 = self._expand(k2, self.K2_NEIGHBOURHOOD_ROWS)
-        return [k1, k2, *k3, k4] + ([own] if self.traa else [])  # K4 runs in both modes (SSR composes with inputType specular)
-
-    @property
-    def ranges(self) -> list:
-        """single-block plans: the per-launch ranges of the band"""
-        return self.ranges_for(self.blocks[0])
-
-    @property
-    def block_ranges(self) -> list:
-        """[block][launch] -> (row0, row1)"""
-        return [self.ranges_for(b) for b in self.blocks]
-
     @property
     def n_launches(self) -> int:
         return 3 + self.passes + (1 if self.traa else 0)
 
-    def super_block(self, j: int):
-        """rows of super-block j: N consecutive blocks, one per rank, in rank order (an in-place all-gather unit)"""
-        return (j * self.world * self.block_rows, (j + 1) * self.world * self.block_rows)
+    @property
+    def ranges(self) -> list:
+        n = self.passes
+        # K2 reads K1's output in its 5x5 window, every Poisson pass the previous target through its taps, K4 the last Poisson target at
+        # the pixel centre (nothing without a pass) and the tail `composed`.  K4 runs in both modes (SSR composes with inputType specular)
+        reaches = [self.K2_NEIGHBOURHOOD_ROWS] + [self.poisson_halo] * n + [self.K4_INPUT_ROWS if n else 0]
+        return _widen_back((self.r0, self.r1), self.height, reaches + ([self.TRAA_TAIL_ROWS] if self.traa else []))
 
     @property
-    def recompute_overhead(self) -> float:
-        """extra rows launched / rows owned (the price of exchanging nothing per pass)"""
-        tot = sum((b - a) for rs in self.block_ranges for a, b in rs)
-        return tot / (self.n_launches * self.rows_per_rank) - 1.0
-
-    @property
-    def local_input_rows(self) -> list:
-        """Rows of the PER-PIXEL input planes (G-buffer, direct light) this rank reads: the K1 range of each block (it contains
-        every later launch's range and the rows its Poisson taps reach) + 1 row each side, because K1's literal bilinear fetch
-        of the direct-light plane at the pixel centre touches row y +- 1 whenever ((y + .5) / H) * H - .5 is not exactly y.
-        The planes sampled at arbitrary screen positions (depth: ray-march taps; velocity: reprojected uv) are needed whole."""
-        return [self._expand(rs[0], 1) for rs in self.block_ranges]
-
-    @property
-    def gathered_planes(self):
-        """chain outputs (`rfx_ssgi_chain_output` index) that are all-gathered after the frame; `composed` first"""
-        return (0, 4, 5) if self.ssgi_mode else (4,)
+    def local_input_rows(self) -> tuple:
+        """Rows of the PER-PIXEL input planes (G-buffer, direct light) this rank reads: the K1 range (it contains every later launch's
+        range and the rows its Poisson taps reach) + 1 row each side, because K1's literal bilinear fetch of the direct-light plane at
+        the pixel centre touches row y +- 1 whenever ((y + .5) / H) * H - .5 is not exactly y.  The planes sampled at arbitrary screen
+        positions (depth: ray-march taps; velocity: reprojected uv) are needed whole."""
+        a, b = self.ranges[0]
+        return max(0, a - 1), min(self.height, b + 1)
 
 
 @dataclass
@@ -188,16 +141,8 @@ class AoShardPlan:
 
     @property
     def ranges(self) -> list:
-        expand = lambda r, rows: (max(0, r[0] - rows), min(self.height, r[1] + rows))  # noqa: E731
-        out = [tuple(self.own)]
-        if self.traa:
-            out.append(expand(out[0], ShardPlan.TRAA_TAIL_ROWS))
-        r = expand(out[-1], self.K7_INPUT_ROWS)
-        for _ in range(2 * self.iterations):
-            out.append(r)
-            r = expand(r, self.poisson_halo)
-        out.append(r)
-        return out[::-1]
+        reaches = [self.poisson_halo] * (2 * self.iterations) + [self.K7_INPUT_ROWS] + ([ShardPlan.TRAA_TAIL_ROWS] if self.traa else [])
+        return _widen_back(tuple(self.own), self.height, reaches)
 
 
 def rebalance(bounds, costs, measured_bounds=None, align: int = 16, min_rows: int = 64, max_share: float = 4.0, damping: float = 0.6):
@@ -404,7 +349,7 @@ class ShardedSsgiChain:
         bounds = self.begin_frame()
         b0, b1 = bounds[self.rank], bounds[self.rank + 1]
         plan = ShardPlan(H, self.world, self.rank, 2 * self.chain.opt.denoise_iterations, self.chain.opt.radius, True, bounds=bounds, width=W)
-        l0, l1 = plan.local_input_rows[0]
+        l0, l1 = plan.local_input_rows
         k = h["frames"] & 1
         st = h["staging"][k]
         h2d = 0

@@ -28,8 +28,6 @@ def _worker(rank, world, port, q, case):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     if case.get("exchange"):
         os.environ["RFX_GROUP_EXCHANGE"] = case["exchange"]
-    if case.get("barrier"):
-        os.environ["RFX_GROUP_BARRIER"] = case["barrier"]
     torch.cuda.set_device(rank)
     dist.init_process_group("gloo", rank=rank, world_size=world)  # control plane only: carries the 128-byte NCCL id
     try:
@@ -84,7 +82,6 @@ CASES = [
     dict(w=192, h=256, frames=4, iters=1, forced=[(0, 128, 256), (0, 64, 256), (0, 192, 256), (0, 112, 256)]),  # jumping borders
     dict(w=144, h=256, frames=3, iters=2),                                                   # portrait: Poisson halo = ceil(3 * 256/144) + 1
     dict(w=256, h=256, frames=4, iters=1, every=1, exchange="allgather"),                    # the replicated fallback (no peer mappings)
-    dict(w=256, h=256, frames=6, iters=1, every=1, barrier="flags"),                         # frame barrier through peer-memory flags instead of NCCL
 ]
 
 

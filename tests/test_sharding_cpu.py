@@ -1,5 +1,5 @@
-"""CPU tests of the multi-GPU host logic: the row-block ShardPlan (halo recompute ranges) and the per-frame all-gather,
-exercised with world_size = 2 over gloo with the ORACLE standing in for the kernels (each "launch" commits only its row
+"""CPU tests of the multi-GPU host logic: the contiguous-band ShardPlan (halo recompute ranges) and the per-frame exchange of every
+rank's band, exercised with world_size = 2 and 3 over gloo with the ORACLE standing in for the kernels (each "launch" commits only its row
 range, like a row-sharded kernel).  The sharded result must equal the single-process chain bit for bit — if a halo were
 one row short, a pass would read a stale row and the comparison would fail."""
 import os
@@ -22,48 +22,43 @@ def test_shard_plan_ranges():
     k1, k2, p0, p1, p2, p3, k4 = p.ranges
     assert k4 == own and p3 == (809, 1081) and p2 == (805, 1085) and p1 == (801, 1089) and p0 == (797, 1093)
     assert k2 == (793, 1097) and k1 == (791, 1099)
-    assert 0 < p.recompute_overhead < 0.15
+    assert (p.r0, p.r1) == own
+    overhead = sum(b - a for a, b in p.ranges) / (p.n_launches * (p.r1 - p.r0)) - 1.0  # extra rows launched / rows owned
+    assert 0 < overhead < 0.15                                                    # the price of exchanging nothing per pass
     first, last = ShardPlan(2160, 8, 0, 4, 3.0), ShardPlan(2160, 8, 7, 4, 3.0)
     assert first.ranges[0][0] == 0 and last.ranges[0][1] == 2160                 # clipped at the frame border
     assert ShardPlan(2160, 1, 0, 4, 3.0).ranges == [(0, 2160)] * 7               # one GPU: whole planes
     assert ShardPlan(64, 2, 1, 0, 3.0).ranges == [(30, 64), (32, 64), (32, 64)]   # denoiseIterations = 0: K1, K2, K4 only
     assert len(ShardPlan(64, 2, 0, 2, 3.0, ssgi_mode=False).ranges) == 5          # SSR composes too (inputType specular)
-    cyc = ShardPlan(2160, 2, 1, 4, 3.0, True, 4)                                  # block-cyclic: rank 1 of 2, 4 blocks each of 270 rows
-    assert cyc.blocks == [(270, 540), (810, 1080), (1350, 1620), (1890, 2160)] and cyc.super_block(2) == (1080, 1620)
-    assert cyc.rows_per_rank == 1080 and len(cyc.block_ranges) == 4 and cyc.block_ranges[3][-1] == (1890, 2160)
-    # every assignment (cyclic, mirrored) is a partition of the rows
-    for mirror in (False, True):
-        owned = sorted(b for r in range(4) for b in ShardPlan(2160, 4, r, 4, 3.0, True, 3, mirror).blocks)
+    # the bands are a partition of the rows
+    for world in (1, 2, 3, 4, 8):
+        owned = [(p.r0, p.r1) for p in (ShardPlan(2160, world, r, 4, 3.0) for r in range(world))]
         assert owned[0][0] == 0 and owned[-1][1] == 2160 and all(a[1] == b[0] for a, b in zip(owned, owned[1:]))
-    m = ShardPlan(2160, 4, 0, 4, 3.0, True, 2, True)
-    assert m.blocks == [(0, 270), (1890, 2160)]                                   # mirrored: bottom-most + top-most block
     with pytest.raises(ValueError):
         ShardPlan(2161, 8, 0, 4, 3.0)
     assert ShardPlan(2160, 8, 0, 4, 11.0).poisson_halo == 12                      # demo radius 11 (SURVEY §8e)
 
 
-def sharded_oracle_chain(inp, o, rank, world, all_gather_rows, blocks_per_rank=1, bounds_per_frame=None, exchange_a=True):
-    """The chain of chain_harness.run_oracle_chain, but every pass commits only its planned rows (all owned blocks) into this rank's
-    planes.  bounds_per_frame: explicit (unequal) band borders, one tuple per frame - the adaptive-band mode moves them between frames.
+def sharded_oracle_chain(inp, o, rank, world, all_gather_rows, bounds_per_frame=None, exchange_a=True):
+    """The chain of chain_harness.run_oracle_chain, but every pass commits only its planned rows into this rank's planes, and
+    all_gather_rows(plane, plan) completes a plane from the other ranks' bands after the frame.  bounds_per_frame: explicit band
+    borders, one tuple per frame (the adaptive-band mode moves them between frames); None: equal bands.
     exchange_a: the A Poisson target's rows take part in the per-frame exchange like B's (what the native group does, by carrying a
     discarded texel from the rank that owns the row: DESIGN.md §5); False reproduces the pre-fix behaviour."""
     import orc
 
     H, W = inp.height, inp.width
-    plan = ShardPlan(H, world, rank, 2 * o.denoise_iterations, o.radius, True, blocks_per_rank)
     env = orc.Env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
     z32, z16 = (lambda: np.zeros((H, W, 4), np.float32)), (lambda: np.zeros((H, W, 4), np.float16))
     ssgi, tr, dnA, dnB, composed = z32(), [z32(), z32()], [z16(), z16()], [z16(), z16()], z32()
     keep_data, prev, bn_t, bn_p = 0.0, None, 0, 0
 
-    def commit(dst, new, rngs_of_blocks):
-        for rng in rngs_of_blocks:
-            dst[rng[0]:rng[1]] = new[rng[0]:rng[1]]
+    def commit(dst, new, rng):
+        dst[rng[0]:rng[1]] = new[rng[0]:rng[1]]
 
     for t, fr in enumerate(inp.frames):
-        if bounds_per_frame is not None:
-            plan = ShardPlan(H, world, rank, 2 * o.denoise_iterations, o.radius, True, bounds=bounds_per_frame[t])
-        rngs = iter(list(zip(*plan.block_ranges)))  # per launch: the ranges of every owned block
+        plan = ShardPlan(H, world, rank, 2 * o.denoise_iterations, o.radius, True, bounds=bounds_per_frame[t] if bounds_per_frame else None)
+        rngs = iter(plan.ranges)
         cam = abi.make_camera(fr["cam"])
         bn_t = ch.next_blue(o.blue_noise_start, bn_t)
         sp = ch.ssgi_params(o, cam, bn_t, (inp.env_map.shape[1], inp.env_map.shape[0]))
@@ -90,53 +85,44 @@ def sharded_oracle_chain(inp, o, rank, world, all_gather_rows, blocks_per_rank=1
     return dict(composed=composed, dn0=dnB[0], dn1=dnB[1], tr0=tr[0], ssgi=ssgi, plan=plan)
 
 
-def _worker(rank, world, port, q, bpr, bounds_per_frame=None):
+def exchange_bands(plane, plan):
+    """every rank's band of `plane` to every other rank (equal or unequal bands): what the native group's peer reads see after a frame"""
+    mine = torch.from_numpy(np.ascontiguousarray(plane[plan.r0:plan.r1]).view(np.uint8).reshape(-1))
+    reqs, theirs = [], {}
+    for peer in range(plan.world):
+        if peer != plan.rank:
+            p0, p1 = plan.bounds[peer], plan.bounds[peer + 1]
+            theirs[peer] = torch.empty((p1 - p0) * plane[0].nbytes, dtype=torch.uint8)
+            reqs += [dist.isend(mine, peer), dist.irecv(theirs[peer], peer)]
+    for r in reqs:
+        r.wait()
+    for peer, t in theirs.items():
+        p0, p1 = plan.bounds[peer], plan.bounds[peer + 1]
+        plane[p0:p1] = t.numpy().view(plane.dtype).reshape(p1 - p0, *plane.shape[1:])
+
+
+def _worker(rank, world, port, q, bounds_per_frame):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), OMP_NUM_THREADS="2")
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         o = ch.Opts(steps=8, refine_steps=2, denoise_iterations=1)
         inp = ch.make_inputs(96, 64, 2)
-
-        def all_gather_rows(plane, plan):
-            if plan.p2p:  # unequal bands: every rank's band to every other rank, like ShardedSsgiChain._exchange's send/recv group
-                b0, b1 = plan.blocks[0]
-                mine = torch.from_numpy(np.ascontiguousarray(plane[b0:b1]).view(np.uint8).reshape(-1))
-                for peer in range(world):
-                    if peer == rank:
-                        continue
-                    p0, p1 = plan.block_of(peer, 0)
-                    theirs = torch.empty((p1 - p0) * plane[0].nbytes, dtype=torch.uint8)
-                    reqs = [dist.isend(mine, peer), dist.irecv(theirs, peer)]
-                    for r in reqs:
-                        r.wait()
-                    plane[p0:p1] = theirs.numpy().view(plane.dtype).reshape(p1 - p0, *plane.shape[1:])
-                return
-            for j, (b0, b1) in enumerate(plan.blocks):  # one collective per super-block, like ShardedSsgiChain._gather
-                mine = torch.from_numpy(np.ascontiguousarray(plane[b0:b1]).view(np.uint8).reshape(-1))
-                parts = [torch.empty_like(mine) for _ in range(world)]
-                dist.all_gather(parts, mine)
-                s0, _ = plan.super_block(j)
-                for g, t in enumerate(parts):
-                    plane[s0 + g * plan.block_rows:s0 + (g + 1) * plan.block_rows] = t.numpy().view(plane.dtype).reshape(plan.block_rows, *plane.shape[1:])
-
-        out = sharded_oracle_chain(inp, o, rank, world, all_gather_rows, blocks_per_rank=bpr, bounds_per_frame=bounds_per_frame)
-        q.put((rank, {k: v.tobytes() for k, v in out.items() if k != "plan"}, out["plan"].blocks))
+        out = sharded_oracle_chain(inp, o, rank, world, exchange_bands, bounds_per_frame=bounds_per_frame)
+        q.put((rank, {k: v.tobytes() for k, v in out.items() if k != "plan"}, (out["plan"].r0, out["plan"].r1)))
     finally:
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("bpr", [1, 2, "moving-bands"])
-def test_two_rank_sharded_chain_equals_single_process_bit_exact(bpr):
-    bounds = None
-    if bpr == "moving-bands":  # adaptive mode: unequal bands whose border moves between the frames
-        bpr, bounds = 1, [(0, 16, 64), (0, 48, 64)]
+@pytest.mark.parametrize("bounds_per_frame", [None, [(0, 16, 64)] * 2, [(0, 16, 64), (0, 48, 64)]],
+                         ids=["equal-bands", "unequal-bands", "moving-bands"])  # moving: the adaptive mode moves the border between frames
+def test_two_rank_sharded_bands_equal_single_process_bit_exact(bounds_per_frame):
     s = socket.socket()
     s.bind(("127.0.0.1", 0))
     port = s.getsockname()[1]
     s.close()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q, bpr, bounds)) for r in range(2)]
+    procs = [ctx.Process(target=_worker, args=(r, 2, port, q, bounds_per_frame)) for r in range(2)]
     for p in procs:
         p.start()
     results = dict()
@@ -149,13 +135,12 @@ def test_two_rank_sharded_chain_equals_single_process_bit_exact(bpr):
     o = ch.Opts(steps=8, refine_steps=2, denoise_iterations=1)
     inp = ch.make_inputs(96, 64, 2)
     ref = ch.run_oracle_chain(inp, o)[-1]
-    for rank, (planes, blocks) in results.items():
-        for k in ("composed", "dn0", "dn1"):                       # gathered planes: the whole frame must match on every rank
+    for rank, (planes, (r0, r1)) in results.items():
+        for k in ("composed", "dn0", "dn1"):                       # exchanged planes: the whole frame must match on every rank
             assert planes[k] == ref[k].tobytes(), (rank, k)
-        for k in ("tr0", "ssgi"):                                  # not gathered: this rank's own rows must match
+        for k in ("tr0", "ssgi"):                                  # not exchanged: this rank's own rows must match
             got = np.frombuffer(planes[k], ref[k].dtype).reshape(ref[k].shape)
-            for r0, r1 in blocks:
-                assert got[r0:r1].tobytes() == ref[k][r0:r1].tobytes(), (rank, k)
+            assert got[r0:r1].tobytes() == ref[k][r0:r1].tobytes(), (rank, k)
 
 
 def _worker3(rank, world, port, q, exchange_a):
@@ -164,16 +149,7 @@ def _worker3(rank, world, port, q, exchange_a):
     try:
         o = ch.Opts(steps=6, refine_steps=1, denoise_iterations=2)
         inp = ch.make_inputs(*WIDE_CASE, fov=75.0)
-
-        def all_gather_rows(plane, plan):  # equal bands: one rank-ordered all-gather per plane
-            b0, b1 = plan.blocks[0]
-            mine = torch.from_numpy(np.ascontiguousarray(plane[b0:b1]).view(np.uint8).reshape(-1))
-            parts = [torch.empty_like(mine) for _ in range(world)]
-            dist.all_gather(parts, mine)
-            for g, t in enumerate(parts):
-                plane[g * plan.block_rows:(g + 1) * plan.block_rows] = t.numpy().view(plane.dtype).reshape(plan.block_rows, *plane.shape[1:])
-
-        out = sharded_oracle_chain(inp, o, rank, world, all_gather_rows, exchange_a=exchange_a)
+        out = sharded_oracle_chain(inp, o, rank, world, exchange_bands, exchange_a=exchange_a)
         q.put((rank, {k: v.tobytes() for k, v in out.items() if k != "plan"}))
     finally:
         dist.destroy_process_group()
@@ -217,20 +193,24 @@ def test_three_ranks_two_denoise_iterations_with_the_a_target_taken_from_its_own
 
 def test_host_path_row_sets_cover_what_each_launch_reads():
     """ShardPlan.local_input_rows (G-buffer / direct-light rows a rank uploads) contains every launch's output rows plus the
-    rows its Poisson taps and quad helpers reach; the ranks' own blocks (uploaded + all-gathered depth / velocity) tile the frame."""
-    from realism_effects_b200.parallel import ShardPlan
+    rows its Poisson taps and quad helpers reach; the ranks' own bands (uploaded + all-gathered depth / velocity) tile the frame.
+    Equal bands, and the bands one rebalancing step makes of them when the cost grows down the frame."""
+    from realism_effects_b200.parallel import ShardPlan, rebalance
 
-    for world, bpr, H, radius, iters in ((2, 1, 128, 3.0, 1), (2, 4, 4320, 8.0, 2), (8, 4, 17280, 8.0, 2), (4, 2, 960, 12.5, 3)):
-        covered = np.zeros(H, np.int32)
-        for rank in range(world):
-            p = ShardPlan(H, world, rank, 2 * iters, radius, True, bpr)
-            for (a, b), launches, (la, lb) in zip(p.blocks, p.block_ranges, p.local_input_rows):
+    for world, H, radius, iters in ((2, 128, 3.0, 1), (2, 4320, 8.0, 2), (8, 17280, 8.0, 2), (4, 960, 12.5, 3)):
+        equal = ShardPlan(H, world, 0, 2 * iters, radius).bounds
+        for bounds in (equal, rebalance(equal, [1.0 + 2.0 * r for r in range(world)])):
+            covered = np.zeros(H, np.int32)
+            for rank in range(world):
+                p = ShardPlan(H, world, rank, 2 * iters, radius, True, bounds=bounds)
+                a, b = p.r0, p.r1
+                la, lb = p.local_input_rows
                 covered[a:b] += 1
                 assert la <= a and lb >= b
-                for k, (r0, r1) in enumerate(launches):
+                for k, (r0, r1) in enumerate(p.ranges):
                     reach = p.poisson_halo if 2 <= k < 2 + p.n_poisson_passes else 0   # K3 passes read G-buffer rows around their output
-                    assert la <= max(0, r0 - reach) and lb >= min(H, r1 + reach), (world, rank, k)
-        assert (covered == 1).all()
+                    assert la <= max(0, r0 - reach) and lb >= min(H, r1 + reach), (world, bounds, rank, k)
+            assert (covered == 1).all()
 
 
 def test_rebalance_moves_borders_towards_equal_cost():
