@@ -433,6 +433,15 @@ rfx_status rfx_gbuffer_debug_launch(rfx_ctx* ctx, void* stream, int32_t mode, co
 rfx_status rfx_traa_compose_launch(rfx_ctx* ctx, void* stream, const rfx_plane* accumulated,
                                    const rfx_plane* out, uint32_t row0, uint32_t row1);
 
+/* K9 + K8 as one EffectPass: `new EffectPass(camera, traaEffect, motionBlurEffect)`, the second pass of the reference README's SSGI frame
+ * (readme.md:141-151).  Per pixel, inputColor = vec4(K9's LINEAR fetch of `accumulated` at the pixel centre .rgb, 1), kept in fp32 as the
+ * merged shader keeps it; then motion_blur.frag's body with velocity NEAREST and the samples + 1 LINEAR taps from `input`, the pass's
+ * input buffer (the frame before TRAA: MotionBlurEffect.update binds inputBuffer.texture, src/motion-blur/MotionBlurEffect.js:87-90).
+ * A still pixel writes inputColor.  velocity RGBA32F, accumulated / input / out RGBA16F of one size; out may alias neither. */
+rfx_status rfx_traa_motion_blur_launch(rfx_ctx* ctx, void* stream, const rfx_motion_blur_params* p, const rfx_plane* velocity,
+                                       const rfx_plane* accumulated, const rfx_plane* input, const rfx_plane* out,
+                                       uint32_t row0, uint32_t row1);
+
 /* ---- SSGI chain (native mirror of SSGIEffect.update, src/ssgi/SSGIEffect.js:372-404 +
  *      src/denoise/Denoiser.js:97-107): owns ssgiOut / trOut / dnA / dnB / composed and the
  *      cross-frame state (prev matrices, keepData, history). ---------------------------- */
@@ -502,8 +511,18 @@ typedef struct rfx_traa_tail_options {
  * direct_light is RFX_ERR_INVALID_ARG; rfx_ssgi_chain_reset resets the TRAA history too.  A chain attached to a group
  * (rfx_group_attach_chain*) cannot change its tail: RFX_ERR_UNSUPPORTED. */
 rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* chain, const rfx_traa_tail_options* opt);
-/* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the K9 output (RGBA16F), 7 the TRAA
- * accumulated plane of the latest frame (RGBA16F; next frame's history).  6 / 7 with the tail off: RFX_ERR_NOT_READY. */
+/* Motion-blur stage of the TRAA tail: `new EffectPass(camera, traaEffect, motionBlurEffect)` as the reference README wires the SSGI frame
+ * (readme.md:141-151).  With the stage on, rfx_traa_motion_blur_launch replaces K9 and writes output 6; its taps read the tail's K5 plane
+ * (the TRAA pass's input buffer), so the fast chain runs its tail as the per-pass launches K5 -> K2 -> the merged pass (same TRAA bytes
+ * as its fused tail).  p == NULL turns the stage off.  The host passes every frame's values before the frame, as MotionBlurEffect.update
+ * sets them (frame, delta_time; resolution = the window size).  Tail off: RFX_ERR_NOT_READY (enable_traa(NULL) turns the stage off
+ * with the tail).  samples < 1: RFX_ERR_INVALID_ARG.  On a chain attached to a group the stage cannot be turned on or off
+ * (RFX_ERR_UNSUPPORTED); its values can change (every rank passes the same).  In a row-sharded group of n > 1 a frame with the stage has
+ * two phases: rfx_ssgi_chain_render_sharded, then rfx_ssgi_chain_render_sharded_finish. */
+rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* chain, const rfx_motion_blur_params* p);
+/* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the tail's output (RGBA16F: K9's, or
+ * with the motion-blur stage on the merged TRAA + motion-blur pass's), 7 the TRAA accumulated plane of the latest frame (RGBA16F; next
+ * frame's history).  6 / 7 with the tail off: RFX_ERR_NOT_READY. */
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane* out);
 /* Debug view of the TRAA tail: SSGIEffect's `outputTexture` (src/ssgi/SSGIEffect.js:228-251, picked from the "Debug" list of
  * example/SSGIDebugGUI.js:78-114).  With a view selected, the tail's K5 runs with isDebug and samples the view instead of `composed`
@@ -598,6 +617,15 @@ rfx_status rfx_group_get_last_bounds(const rfx_group* group, uint32_t* bounds); 
 rfx_status rfx_group_allgather_rows(rfx_group* group, void* stream, const rfx_plane* plane, const uint32_t* bounds);
 /* collective: one frame; this rank renders its band from full-frame input planes and joins the frame's collective on `stream` */
 rfx_status rfx_ssgi_chain_render_sharded(rfx_ssgi_chain* chain, void* stream, const rfx_ssgi_frame* frame);
+/* The second phase of a frame with the TRAA tail's motion-blur stage (rfx_ssgi_chain_set_motion_blur before the attach; members whose stage
+ * is on and off: RFX_ERR_INVALID_ARG).  The merged TRAA + motion-blur pass taps this frame's K5 plane at a data-dependent reach, so in a
+ * group of n > 1 render_sharded stops after the TRAA pass (phase 1) and this call runs the frame's barrier, then the merged pass on the band
+ * and the frame's end.  The K5 plane is one more kept plane (double-buffered by tail parity, peer-mapped at attach); its rows are read on
+ * their owners.  The barrier: across processes one more NCCL all-gather on `stream`; in-process the host calls render_sharded for every
+ * member before this call for any; with RFX_GROUP_EXCHANGE=allgather the exchange of every rank's K5 band.  Call it after every
+ * render_sharded: a frame without a second phase (the stage off, or n = 1) returns RFX_OK at once.  render_sharded while a frame waits
+ * for this call, and this call with no frame waiting: RFX_ERR_NOT_READY.  Results are bit-identical to one chain. */
+rfx_status rfx_ssgi_chain_render_sharded_finish(rfx_ssgi_chain* chain, void* stream);
 /* pure host arithmetic, exported for hosts that plan their bands with it (and for the CPU tests): the ranges render_sharded uses,
  * rows [ranges[2k], ranges[2k+1]) of launch k (K1, K2, K3 pass 0.., K4) for the band [own0, own1); n_launches = 3 + n_poisson_passes.
  * n_launches = 4 + n_poisson_passes: the same with the TRAA tail as the last launch; it runs on the band and K4 on the band widened
@@ -670,6 +698,11 @@ rfx_status rfx_ao_chain_render(rfx_ao_chain* chain, void* stream, const rfx_ao_f
  * frame after enabling renders with keepData 0 too.  opt == NULL turns the tail off and frees its planes.  A chain attached to a group
  * of n > 1 cannot change its tail: RFX_ERR_UNSUPPORTED. */
 rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* chain, const rfx_traa_tail_options* opt);
+/* Motion-blur stage of the AO chain's TRAA tail, as rfx_ssgi_chain_set_motion_blur: the merged TRAA + motion-blur pass replaces K9 and
+ * writes frame->output; its taps read the K7 plane (output 2).  Tail off: RFX_ERR_NOT_READY; on a chain in a group of n > 1 the stage
+ * cannot be turned on or off (RFX_ERR_UNSUPPORTED).  In such a group a frame with the stage has two phases:
+ * rfx_ao_chain_render_sharded_traa, then rfx_ao_chain_render_sharded_finish. */
+rfx_status rfx_ao_chain_set_motion_blur(rfx_ao_chain* chain, const rfx_motion_blur_params* p);
 /* What the TRAA pass needs and rfx_ao_frame lacks: near / far, the perspective flag and the position of the UN-jittered camera (jittering
  * the rasteriser, TAAUtils.js, stays the host's job), and didCameraMove (src/utils/SceneUtils.js:17-27) for fullAccumulate.  The chain
  * keeps the previous frame's camera; on the first frame and after rfx_ao_chain_reset the previous camera is the current one. */
@@ -700,6 +733,9 @@ rfx_status rfx_group_attach_ao_chains_inprocess(rfx_group* const* groups, rfx_ao
 rfx_status rfx_ao_chain_render_sharded(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame);
 /* collective: rfx_ao_chain_render_traa in a group.  Tail off: RFX_ERR_NOT_READY. */
 rfx_status rfx_ao_chain_render_sharded_traa(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame, const rfx_ao_traa_frame* traa);
+/* collective: the second phase of a frame with the motion-blur stage, as rfx_ssgi_chain_render_sharded_finish (the kept plane is the K7
+ * plane, output 2) */
+rfx_status rfx_ao_chain_render_sharded_finish(rfx_ao_chain* chain, void* stream);
 /* pure host arithmetic: rows [ranges[2k], ranges[2k+1]) of launch k (K6 / K6h, Poisson pass 0 .. 2*iterations-1, K7) for the band
  * [own0, own1); n_launches = 2 + 2 * iterations.  K7 runs on the band, the last Poisson pass on the band +- 1 row (K7's LINEAR fetch at
  * the pixel centre; with iterations 0 K6 gets those rows), and every earlier launch on the next one's range widened by the Poisson halo

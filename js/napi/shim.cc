@@ -349,13 +349,36 @@ napi_value AoCompose(napi_env env, napi_callback_info info) {  // aoCompose(ctx,
         "rfx_ao_compose_launch");
   return undefined(env);
 }
-napi_value MotionBlur(napi_env env, napi_callback_info info) {  // motionBlur(ctx, params, velocity, input, out)
-  ARGS(5); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
-  Obj b{env, argv[1]};
+static rfx_motion_blur_params motion_blur_params(napi_env env, napi_value v) {  // {intensity, jitter, deltaTime, frame, samples, resolution}
+  Obj b{env, v};
   rfx_motion_blur_params p{};
   p.intensity = (float)b.num("intensity", 1); p.jitter = (float)b.num("jitter", 1); p.delta_time = (float)b.num("deltaTime", 1.0 / 60); p.frame = (int32_t)b.num("frame", 0);
   p.samples = (int32_t)b.num("samples", 16); b.floats("resolution", p.resolution, 2);
+  return p;
+}
+napi_value MotionBlur(napi_env env, napi_callback_info info) {  // motionBlur(ctx, params, velocity, input, out)
+  ARGS(5); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  const rfx_motion_blur_params p = motion_blur_params(env, argv[1]);
   CHECK(c, rfx_motion_blur_launch(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), unwrap<rfx_plane>(env, argv[4]), 0, 0), "rfx_motion_blur_launch");
+  return undefined(env);
+}
+// traaMotionBlur(ctx, params, velocity, accumulated, input, out): EffectPass(camera, traaEffect, motionBlurEffect) in one launch; `input` is
+// the pass's input buffer (the frame before TRAA)
+napi_value TraaMotionBlur(napi_env env, napi_callback_info info) {
+  ARGS(6); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  const rfx_motion_blur_params p = motion_blur_params(env, argv[1]);
+  CHECK(c, rfx_traa_motion_blur_launch(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), unwrap<rfx_plane>(env, argv[4]),
+                                       unwrap<rfx_plane>(env, argv[5]), 0, 0), "rfx_traa_motion_blur_launch");
+  return undefined(env);
+}
+// chainSetMotionBlur(ctx, chain, params | null): the motion-blur stage of the chain's TRAA tail, this frame's values; null turns it off
+napi_value ChainSetMotionBlur(napi_env env, napi_callback_info info) {
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  napi_valuetype t = napi_undefined;
+  napi_typeof(env, argv[2], &t);
+  rfx_motion_blur_params p{};
+  if (t == napi_object) p = motion_blur_params(env, argv[2]);
+  CHECK(ctx, rfx_ssgi_chain_set_motion_blur(unwrap<rfx_ssgi_chain>(env, argv[1]), t == napi_object ? &p : nullptr), "rfx_ssgi_chain_set_motion_blur");
   return undefined(env);
 }
 napi_value TraaCompose(napi_env env, napi_callback_info info) {  // traaCompose(ctx, accumulated, out)
@@ -467,7 +490,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("planeUpload", PlaneUpload), FN("planeDownload", PlaneDownload), FN("chainCreate", ChainCreate), FN("chainSetOptions", ChainSetOptions),
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
       FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
-      FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur),
+      FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur), FN("traaMotionBlur", TraaMotionBlur), FN("chainSetMotionBlur", ChainSetMotionBlur),
       FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),
       FN("groupDestroy", GroupDestroy), FN("chainRenderSharded", ChainRenderSharded),

@@ -256,6 +256,7 @@ def _sig(lib):
     lib.rfx_ao_compose_launch.argtypes = [vp, vp, _P(AoComposeParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_motion_blur_launch.argtypes = [vp, vp, _P(MotionBlurParams), PP, PP, PP, u32, u32]
     lib.rfx_traa_compose_launch.argtypes = [vp, vp, PP, PP, u32, u32]
+    lib.rfx_traa_motion_blur_launch.argtypes = [vp, vp, _P(MotionBlurParams), PP, PP, PP, PP, u32, u32]
     lib.rfx_gbuffer_debug_launch.argtypes = [vp, vp, C.c_int32, PP, PP, u32, u32]
     lib.rfx_ssgi_chain_set_debug_view.argtypes = [vp, C.c_int32]
     lib.rfx_effects_launch.argtypes = [vp, vp, _P(EffectsParams), PP, PP, PP, PP, u32, u32]
@@ -269,6 +270,9 @@ def _sig(lib):
     lib.rfx_ssgi_chain_render.argtypes = [vp, vp, _P(SsgiFrame)]
     lib.rfx_ssgi_chain_output.argtypes = [vp, C.c_int32, PP]
     lib.rfx_ssgi_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
+    lib.rfx_ssgi_chain_set_motion_blur.argtypes = [vp, _P(MotionBlurParams)]
+    lib.rfx_ssgi_chain_render_sharded_finish.argtypes = [vp, vp]
+    lib.rfx_ao_chain_render_sharded_finish.argtypes = [vp, vp]
     lib.rfx_ssgi_chain_render_host.argtypes = [vp, _P(SsgiHostFrame)]
     lib.rfx_ssgi_chain_submit_host.argtypes = [vp, _P(SsgiHostFrame)]
     lib.rfx_ssgi_chain_wait_host.argtypes = [vp, C.c_int32]
@@ -306,6 +310,7 @@ def _sig(lib):
     lib.rfx_ao_chain_render.argtypes = [vp, vp, _P(AoFrame)]
     lib.rfx_ao_chain_output.argtypes = [vp, C.c_int32, PP]
     lib.rfx_ao_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
+    lib.rfx_ao_chain_set_motion_blur.argtypes = [vp, _P(MotionBlurParams)]
     lib.rfx_ao_chain_render_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
     lib.rfx_ao_chain_render_sharded_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
     lib.rfx_group_attach_ao_chain.argtypes = [vp, vp]
@@ -331,6 +336,8 @@ EXPORTS = [
     "rfx_ao_chain_create", "rfx_ao_chain_destroy", "rfx_ao_chain_set_options", "rfx_ao_chain_reset", "rfx_ao_chain_render", "rfx_ao_chain_output",
     "rfx_group_attach_ao_chain", "rfx_group_attach_ao_chains_inprocess", "rfx_ao_chain_render_sharded", "rfx_ao_shard_ranges",
     "rfx_ao_chain_enable_traa", "rfx_ao_chain_render_traa", "rfx_ao_chain_render_sharded_traa",
+    "rfx_traa_motion_blur_launch", "rfx_ssgi_chain_set_motion_blur", "rfx_ao_chain_set_motion_blur",
+    "rfx_ssgi_chain_render_sharded_finish", "rfx_ao_chain_render_sharded_finish",
 ]
 
 

@@ -184,17 +184,13 @@ cudaError_t launch_ao_compose(const AoComposeArgs& a, cudaStream_t s) {
   return cudaGetLastError();
 }
 
-__global__ void __launch_bounds__(256) motion_blur_kernel(const __grid_constant__ MotionBlurArgs a) {
-  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
-  if (x >= a.W || y >= a.row1) return;
-  const v2 vUv = pixel_uv(x, y, a.W, a.H);
-  const v4 inputColor = tex_h4_linear(a.input, vUv);
+// K8 for pixel (x, y) given the effect's inputColor: motion_blur.frag's mainImage, velocity NEAREST at the pixel, the samples + 1 taps
+// LINEAR through `tap` (the input buffer).  Shared by motion_blur_kernel and traa_motion_blur_kernel.
+template <class S>
+RFX_D v4 motion_blur_px(const MotionBlurArgs& a, const S& tap, v4 inputColor, v2 vUv, int x, int y) {
   const float4 vt = ld_f4(a.velocity, x, y);
   v2 velocity = mk2(vt.x, vt.y);
-  if (!(dot(velocity, velocity) > 0.000000001f)) {
-    st_h4(a.out.p, a.out.pitch, x, y, inputColor);
-    return;
-  }
+  if (!(dot(velocity, velocity) > 0.000000001f)) return inputColor;
   velocity = velocity * a.intensity;
   // blueNoise(vUv, frame) with `resolution` = window size (MotionBlurEffect.js:94): blue_noise.glsl:37-45
   v2 bnv;
@@ -224,14 +220,41 @@ __global__ void __launch_bounds__(256) motion_blur_kernel(const __grid_constant_
   v3 c = xyz(inputColor);
   for (float i = 0.0f; i <= samplesFloat; i++) {
     const v2 ruv = mix(startUv, endUv, i / samplesFloat);
-    c = c + xyz(tex_h4_linear(a.input, ruv));
+    c = c + xyz(tap.linear(ruv));
   }
   c = c / (samplesFloat + 2.0f);
-  st_h4(a.out.p, a.out.pitch, x, y, mk4(c, inputColor.w));
+  return mk4(c, inputColor.w);
+}
+__global__ void __launch_bounds__(256) motion_blur_kernel(const __grid_constant__ MotionBlurArgs a) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= a.W || y >= a.row1) return;
+  const v2 vUv = pixel_uv(x, y, a.W, a.H);
+  st_h4(a.out.p, a.out.pitch, x, y, motion_blur_px(a, PlaneH4{a.input}, tex_h4_linear(a.input, vUv), vUv, x, y));
 }
 cudaError_t launch_motion_blur(const MotionBlurArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);
   motion_blur_kernel<<<grid, 256, 0, s>>>(a);
+  return cudaGetLastError();
+}
+
+// TRAAEffect + MotionBlurEffect in one EffectPass: inputColor = K9's colour of the accumulated plane (kept in fp32, as in the merged
+// shader), then K8 with its taps on the input buffer.  PEER: the input buffer's rows are read on the ranks that own them.
+template <bool PEER>
+__global__ void __launch_bounds__(256) traa_motion_blur_kernel(const __grid_constant__ TraaMotionBlurArgs a, const __grid_constant__ PeerPV in) {
+  const MotionBlurArgs& m = a.mb;
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = m.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= m.W || y >= m.row1) return;
+  const v2 vUv = pixel_uv(x, y, m.W, m.H);
+  const v4 inputColor = traa_compose_px(PlaneH4{a.acc}, x, y, m.W, m.H);
+  v4 c;
+  if constexpr (PEER) c = motion_blur_px(m, PeerH4{in}, inputColor, vUv, x, y);
+  else c = motion_blur_px(m, PlaneH4{m.input}, inputColor, vUv, x, y);
+  st_h4(m.out.p, m.out.pitch, x, y, c);
+}
+cudaError_t launch_traa_motion_blur(const TraaMotionBlurArgs& a, cudaStream_t s, const PeerPV* peer) {
+  dim3 grid((a.mb.W + 31) / 32, (a.mb.row1 - a.mb.row0 + 7) / 8);
+  if (peer) traa_motion_blur_kernel<true><<<grid, 256, 0, s>>>(a, *peer);
+  else traa_motion_blur_kernel<false><<<grid, 256, 0, s>>>(a, PeerPV{});
   return cudaGetLastError();
 }
 

@@ -809,23 +809,53 @@ rfx_status rfx_ao_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ao_compos
   return ao_compose(ctx, stream, p, depth, ao, input, out, row0, row1);
 }
 
+}  // extern "C"
+
+// K8's arguments (rfx_motion_blur_launch and the merged TRAA + motion-blur pass): the planes, the rows and the uniforms
+static rfx_status motion_blur_args(rfx_ctx* ctx, const char* who, const rfx_motion_blur_params* p, const rfx_plane* velocity, const rfx_plane* input,
+                                   const rfx_plane* out, uint32_t row0, uint32_t row1, MotionBlurArgs& a) {
+  if (!pv(velocity, RFX_FMT_RGBA32F, a.velocity) || !pv(input, RFX_FMT_RGBA16F, a.input) || !ov(out, RFX_FMT_RGBA16F, a.out))
+    return fail(ctx, RFX_ERR_BAD_FORMAT, "%s: velocity RGBA32F, input/out RGBA16F required", who);
+  a.W = (int)out->width; a.H = (int)out->height;
+  if (a.velocity.w != a.W || a.velocity.h != a.H || a.input.w != a.W || a.input.h != a.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "%s: plane sizes differ", who);
+  if (input->ptr == out->ptr) return fail(ctx, RFX_ERR_INVALID_ARG, "%s: in-place is not allowed", who);
+  if (p->samples < 1) return fail(ctx, RFX_ERR_INVALID_ARG, "%s: samples < 1", who);
+  rows(row0, row1, out->height, a.row0, a.row1);
+  a.intensity = p->intensity; a.jitter = p->jitter; a.delta_time = p->delta_time; a.res_x = p->resolution[0]; a.res_y = p->resolution[1];
+  a.samples = p->samples;
+  return blue_for(ctx, p->frame, a.blue);
+}
+
+// The merged TRAA + motion-blur pass over output rows [row0, row1) (0, 0: all).  peer: the input buffer's rows live on their owners
+// (a row-sharded group of n > 1); its local plane is `input`.
+static rfx_status traa_motion_blur(rfx_ctx* ctx, void* stream, const rfx_motion_blur_params* p, const rfx_plane* velocity, const rfx_plane* acc,
+                                   const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1, const PeerPV* peer) {
+  TraaMotionBlurArgs a{};
+  rfx_status st = motion_blur_args(ctx, "traa_motion_blur", p, velocity, input, out, row0, row1, a.mb);
+  if (st != RFX_OK) return st;
+  if (!pv(acc, RFX_FMT_RGBA16F, a.acc)) return fail(ctx, RFX_ERR_BAD_FORMAT, "traa_motion_blur: accumulated RGBA16F required");
+  if (a.acc.w != a.mb.W || a.acc.h != a.mb.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "traa_motion_blur: plane sizes differ");
+  if (acc->ptr == out->ptr) return fail(ctx, RFX_ERR_INVALID_ARG, "traa_motion_blur: out may not alias accumulated");
+  LAUNCHED(launch_traa_motion_blur(a, pick(ctx, stream), peer));
+  return RFX_OK;
+}
+
+extern "C" {
+
 rfx_status rfx_motion_blur_launch(rfx_ctx* ctx, void* stream, const rfx_motion_blur_params* p, const rfx_plane* velocity, const rfx_plane* input,
                                   const rfx_plane* out, uint32_t row0, uint32_t row1) {
   if (!ctx || !p || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "motion_blur: null argument");
   MotionBlurArgs a{};
-  if (!pv(velocity, RFX_FMT_RGBA32F, a.velocity) || !pv(input, RFX_FMT_RGBA16F, a.input) || !ov(out, RFX_FMT_RGBA16F, a.out))
-    return fail(ctx, RFX_ERR_BAD_FORMAT, "motion_blur: velocity RGBA32F, input/out RGBA16F required");
-  a.W = (int)out->width; a.H = (int)out->height;
-  if (a.velocity.w != a.W || a.velocity.h != a.H || a.input.w != a.W || a.input.h != a.H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "motion_blur: plane sizes differ");
-  if (input->ptr == out->ptr) return fail(ctx, RFX_ERR_INVALID_ARG, "motion_blur: in-place is not allowed");
-  if (p->samples < 1) return fail(ctx, RFX_ERR_INVALID_ARG, "motion_blur: samples < 1");
-  rows(row0, row1, out->height, a.row0, a.row1);
-  a.intensity = p->intensity; a.jitter = p->jitter; a.delta_time = p->delta_time; a.res_x = p->resolution[0]; a.res_y = p->resolution[1];
-  a.samples = p->samples;
-  rfx_status st = blue_for(ctx, p->frame, a.blue);
+  rfx_status st = motion_blur_args(ctx, "motion_blur", p, velocity, input, out, row0, row1, a);
   if (st != RFX_OK) return st;
   LAUNCHED(launch_motion_blur(a, pick(ctx, stream)));
   return RFX_OK;
+}
+
+rfx_status rfx_traa_motion_blur_launch(rfx_ctx* ctx, void* stream, const rfx_motion_blur_params* p, const rfx_plane* velocity, const rfx_plane* acc,
+                                       const rfx_plane* input, const rfx_plane* out, uint32_t row0, uint32_t row1) {
+  if (!ctx || !p || !acc || !out) return fail(ctx, RFX_ERR_INVALID_ARG, "traa_motion_blur: null argument");
+  return traa_motion_blur(ctx, stream, p, velocity, acc, input, out, row0, row1, nullptr);
 }
 
 rfx_status rfx_gbuffer_debug_launch(rfx_ctx* ctx, void* stream, int32_t mode, const rfx_plane* gbuffer, const rfx_plane* out, uint32_t row0, uint32_t row1) {
@@ -938,17 +968,30 @@ struct HistPlane {
 };
 // The TRAA frame tail a chain can end with (rfx_*_chain_enable_traa): TRAAEffect's temporal pass over `mid` into the accumulated plane,
 // then K9.  `mid` is the composer buffer before the TRAA EffectPass: the SSGI chain's K5 output (per-pass tail only; the fused fast tail
-// has none), the AO chain's K7 output.
+// has none), the AO chain's K7 output.  With the motion-blur stage on (rfx_*_chain_set_motion_blur), the merged TRAA + motion-blur pass
+// replaces K9; its taps read all of `mid`.  `mid` is single-buffered (buffer 0) unless a row-sharded group with the stage gave it buffer 1:
+// then it goes by tail parity like `acc`, so that a rank's next frame never writes rows a slower peer's merged pass still reads.
 struct TraaTail {
   bool on = false;
   rfx_traa_tail_options opt{};
   HistPlane acc;        // accumulated plane by tail parity (buf[prev] is the history)
-  rfx_plane mid{};
+  HistPlane mid;
   rfx_plane out{};      // K9 output (SSGI; the AO tail writes frame->output)
+  bool blur = false;    // the motion-blur stage
+  rfx_motion_blur_params blur_p{};  // this frame's MotionBlurEffect uniforms
+  // In a row-sharded group of n > 1 with the stage on, a frame has two phases (rfx_*_chain_render_sharded, then _finish): the merged pass
+  // reads this frame's `mid` rows on their owners, so it waits for the frame's barrier.  `pending`: phase 1 ran, the merged pass did not.
+  bool split = false;
+  bool pending = false;
+  rfx_plane p2_velocity{}, p2_out{};  // what phase 2 launches on: the frame's velocity plane and output
+  int p2_r0 = 0, p2_r1 = 0;           // ... and the band
   uint64_t frames = 0;  // tails rendered; acc.buf[frames & 1] is written next
   float keep = 0.0f;    // keepData of the TRAA pass
   int cur() const { return (int)(frames & 1); }
+  int mid_cur() const { return mid.buf[1].ptr ? cur() : 0; }
+  rfx_plane& mid_w() { return mid.buf[mid_cur()]; }  // this frame's `mid`
   const rfx_plane& latest() const { return acc.buf[(frames + 1) & 1]; }  // the accumulated plane of the latest frame
+  const rfx_plane& mid_latest() const { return mid.buf[mid.buf[1].ptr ? (int)((frames + 1) & 1) : 0]; }  // `mid` of the latest frame
   void advance() { keep = 1.0f; frames++; }  // after a frame's tail: keep the history from now on
 };
 // What a row-sharded group (rfx_group.inl) needs of a member chain; both chain kinds derive from it.
@@ -1023,7 +1066,7 @@ static std::array<HistPlane*, 9> every_hist_plane(rfx_ssgi_chain* ch) {  // whet
 static int pass_latest(const GroupMember* ch);
 
 static void traa_free(rfx_ctx* ctx, TraaTail& t) {
-  for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid}) if (p->ptr) rfx_plane_free(ctx, p);
+  for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid.buf[0], &t.mid.buf[1]}) if (p->ptr) rfx_plane_free(ctx, p);
 }
 // rfx_*_chain_enable_traa once the chain kind's own checks passed: NULL frees the tail's planes.  Otherwise the planes are allocated on
 // first use (`out` and `mid` where the chain asks for them; nothing is left allocated on failure), and the options replace the old ones.
@@ -1032,18 +1075,36 @@ static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_opt
     CU(cudaStreamSynchronize(ctx->stream));
     traa_free(ctx, t);
     t.on = false;
+    t.blur = false;  // the stage ends the tail: it goes with it
     return RFX_OK;
   }
   if (!t.acc.buf[0].ptr) {
     rfx_status st = RFX_OK;
-    for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], with_out ? &t.out : nullptr, with_mid ? &t.mid : nullptr})
+    for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], with_out ? &t.out : nullptr, with_mid ? &t.mid.buf[0] : nullptr})
       if (p && st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, p);
     if (st != RFX_OK) { traa_free(ctx, t); return st; }
     local_views(t.acc);
+    local_views(t.mid);
   }
   t.opt = *opt;
   t.on = true;
   t.keep = 0.0f;  // a new TemporalReprojectPass, or TemporalReprojectPass.reset()
+  return RFX_OK;
+}
+// rfx_*_chain_set_motion_blur: `fixed` = the chain's tail cannot change (it is attached to a group), so neither can the stage; its values can.
+// Turning the stage on allocates `mid` where the chain has none (the fused fast tail): the merged pass needs the whole input buffer.
+static rfx_status traa_set_blur(rfx_ctx* ctx, TraaTail& t, const rfx_motion_blur_params* p, bool fixed, uint32_t W, uint32_t H) {
+  if (!t.on) return fail(ctx, RFX_ERR_NOT_READY, "set_motion_blur: the motion-blur stage shares the TRAA tail's pass, and the tail is off");
+  if (fixed && (p != nullptr) != t.blur)
+    return fail(ctx, RFX_ERR_UNSUPPORTED, "set_motion_blur: the chain is attached to a group, whose planes are fixed at attach time: the stage cannot be turned on or off");
+  if (p && p->samples < 1) return fail(ctx, RFX_ERR_INVALID_ARG, "set_motion_blur: samples < 1");
+  if (p && !t.mid.buf[0].ptr) {
+    rfx_status st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, &t.mid.buf[0]);
+    if (st != RFX_OK) return st;
+    local_views(t.mid);
+  }
+  t.blur = p != nullptr;
+  if (p) t.blur_p = *p;
   return RFX_OK;
 }
 
@@ -1177,6 +1238,11 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_op
   return traa_enable(ch->ctx, ch->tail, opt, ch->opt.width, ch->opt.height, true, k5);
 }
 
+rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* ch, const rfx_motion_blur_params* p) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  return traa_set_blur(ch->ctx, ch->tail, p, ch->group != nullptr, ch->opt.width, ch->opt.height);
+}
+
 }  // extern "C"
 // fast chain: tr[]/dnB[] buffer 0 := the reference-format views of the interleaved planes, dn from fdnB.buf[parity]
 static rfx_status split_views(rfx_ssgi_chain* ch, int parity, cudaStream_t s) {
@@ -1253,8 +1319,8 @@ rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* ch, int32_t view) {
   rfx_status st = RFX_OK;
   if (ch->fastpath && plane && view >= RFX_DEBUG_VIEW_OUTPUT + 2) st = alloc_split_views(ch);
   if (st == RFX_OK && channel && !ch->debug_gb.ptr) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->debug_gb);
-  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->tail.on && !ch->tail.mid.ptr)  // the tail's K5 plane (the fused fast tail has none)
-    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->tail.mid);
+  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->tail.on && !ch->tail.mid.buf[0].ptr)  // the tail's K5 plane (the fused fast tail has none)
+    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->tail.mid.buf[0]);
   if (st != RFX_OK) return st;
   ch->debug_view = view;
   return RFX_OK;
@@ -1347,16 +1413,37 @@ static rfx_temporal_params traa_params(const TraaTail& t, const rfx_temporal_par
 }
 // K2 in its TRAA form over the tail's `mid` on the output rows kr +- 1 (K9's LINEAR fetch) into buffer cur() of the accumulated plane,
 // reading last frame's other buffer (in a row-sharded group of n > 1, `peer`: on the rank that owns each row), then K9 from it into `out`
-// on kr.  `mid` must hold rows kr +- RFX_TRAA_TAIL_ROWS.
+// on kr, or with the motion-blur stage on the merged TRAA + motion-blur pass, whose taps read all of `mid`.  `mid` must hold rows
+// kr +- RFX_TRAA_TAIL_ROWS (with the stage alone: every row).  Then the tail advances.  With a split frame (t.split) the merged pass and
+// the advance wait for phase 2 (traa_blur_finish): this returns with t.pending set.
 static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_params& tp, TraaTail& t, const rfx_plane* velocity, bool peer,
                                 const rfx_plane* out, Rows kr) {
   const int cur = t.cur(), H = (int)t.acc.buf[cur].height;
   TemporalPeer tpeer{};
   tpeer.hist0 = tpeer.hist1 = t.acc.view[cur ^ 1];
-  rfx_status st = temporal_reproject(ctx, stream, &tp, &t.mid, velocity, &t.acc.buf[cur ^ 1], nullptr, &t.acc.buf[cur], nullptr, std::max(0, kr.r0 - 1),
+  rfx_status st = temporal_reproject(ctx, stream, &tp, &t.mid_w(), velocity, &t.acc.buf[cur ^ 1], nullptr, &t.acc.buf[cur], nullptr, std::max(0, kr.r0 - 1),
                                      std::min(H, kr.r1 + 1), peer ? &tpeer : nullptr);
-  if (st == RFX_OK) st = rfx_traa_compose_launch(ctx, stream, &t.acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+  if (st != RFX_OK) return st;
+  if (t.blur && t.split) {
+    t.p2_velocity = *velocity; t.p2_out = *out; t.p2_r0 = kr.r0; t.p2_r1 = kr.r1;
+    t.pending = true;
+    return RFX_OK;
+  }
+  if (t.blur) st = traa_motion_blur(ctx, stream, &t.blur_p, velocity, &t.acc.buf[cur], &t.mid_w(), out, (uint32_t)kr.r0, (uint32_t)kr.r1, nullptr);
+  else st = rfx_traa_compose_launch(ctx, stream, &t.acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+  if (st == RFX_OK) t.advance();
   return st;
+}
+// Phase 2 of a split frame, after the frame's barrier: the merged pass on the band, its taps reading this frame's `mid` through `mid_view`
+// (each row on its owner, or the local plane once the rows were replicated), then the tail advances.
+static rfx_status traa_blur_finish(rfx_ctx* ctx, void* stream, TraaTail& t, const PeerPV& mid_view) {
+  const int cur = t.cur();
+  rfx_status st = traa_motion_blur(ctx, stream, &t.blur_p, &t.p2_velocity, &t.acc.buf[cur], &t.mid_w(), &t.p2_out, (uint32_t)t.p2_r0, (uint32_t)t.p2_r1,
+                                   mid_view.n > 1 ? &mid_view : nullptr);
+  if (st != RFX_OK) return st;
+  t.pending = false;
+  t.advance();
+  return RFX_OK;
 }
 
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
@@ -1369,7 +1456,9 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   TraaTail& tail = ch->tail;
   const rfx_temporal_params tp = traa_params(tail, ch->traa_tp, f->camera_moved);
   const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
-  if (ch->fastpath && !debug) {
+  // the fused kernel never writes the K5 plane, and the motion-blur stage samples all of it: with the stage on, the per-pass launches
+  // (which also measured faster than the fused tail at 4K, DESIGN.md §4)
+  if (ch->fastpath && !debug && !tail.blur) {
     CTraaArgs a{};
     TemporalArgs& t = a.t;
     if (!pv(f->velocity, RFX_FMT_RGBA32F, t.velocity)) return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: velocity must be RGBA32F");
@@ -1399,10 +1488,12 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
       st = debug_view_plane(ch, stream, f, &view);
     }
     if (st == RFX_OK)
-      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &tail.mid, (uint32_t)std::max(0, kr.r0 - halo),
+      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &tail.mid_w(), (uint32_t)std::max(0, kr.r0 - halo),
                                    (uint32_t)std::min(H, kr.r1 + halo));
-    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, tail, f->velocity, ch->group_peer, &tail.out, kr);
-    if (st != RFX_OK) return st;
+    // the TRAA history rows live on their owners in a group of n > 1: the per-pass chain's peer forms, and the fast chain's tail when the
+    // motion-blur stage takes it off its fused kernel (which reads the history through the views itself)
+    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, tail, f->velocity, ch->group_peer || tail.split, &tail.out, kr);
+    return st;  // the per-pass tail advances in traa_launches
   }
   tail.advance();
   return RFX_OK;
@@ -1873,10 +1964,15 @@ rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* ch, const rfx_traa_tail_option
   return traa_enable(ctx, ch->tail, opt, ch->opt.width, ch->opt.height, false, true);
 }
 
+rfx_status rfx_ao_chain_set_motion_blur(rfx_ao_chain* ch, const rfx_motion_blur_params* p) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  return traa_set_blur(ch->ctx, ch->tail, p, ch->group && rfx_group_world(ch->group) > 1, ch->opt.width, ch->opt.height);
+}
+
 rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
   if (ch->tail.on && (which == 2 || which == 3)) {
-    *out = which == 2 ? ch->tail.mid : ch->tail.latest();
+    *out = which == 2 ? ch->tail.mid_latest() : ch->tail.latest();
     return RFX_OK;
   }
   if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1 (2 / 3 with the TRAA tail on)");
@@ -1965,7 +2061,7 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     memcpy(cp.color, o.color, 12);
     const Rows kr = launch_rows(ranges, k, (int)o.height);
     const HistPlane& tex = o.iterations > 0 ? ch->dnB : ch->target;
-    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, t ? &ch->tail.mid : f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
+    st = ao_compose(ctx, stream, &cp, f->depth, &tex.buf[wr], f->input, t ? &ch->tail.mid_w() : f->output, (uint32_t)kr.r0, (uint32_t)kr.r1);
     if (st != RFX_OK) return st;
   }
   k++;
@@ -1980,7 +2076,6 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     st = traa_launches(ctx, stream, traa_params(ch->tail, cam, t->camera_moved), ch->tail, f->velocity, ch->group_peer, f->output,
                        launch_rows(ranges, k, (int)o.height));
     if (st != RFX_OK) return st;
-    ch->tail.advance();
     ch->traa_prev = *t;
     ch->traa_have_prev = true;
   }

@@ -290,6 +290,20 @@ struct PlaneH4 {
   const PV& t;
   RFX_D v4 linear(v2 uv) const { return tex_h4_linear(t, uv); }
 };
+// the same over a plane whose rows live on their owners (a row-sharded group)
+struct PeerH4 {
+  const PeerPV& t;
+  RFX_D v4 linear(v2 uv) const { return peer_h4_linear(t, uv); }
+};
+
+// TRAAEffect + MotionBlurEffect as one EffectPass (the reference README's SSGI frame): K9's colour is K8's inputColor, and K8's taps
+// sample the pass's input buffer `mb.input` (the frame before TRAA).  `mb.out` gets every pixel of rows [mb.row0, mb.row1).
+// peer != nullptr: `mb.input` is ignored and the taps read peer->local's rows on their owners.
+struct TraaMotionBlurArgs {
+  MotionBlurArgs mb;
+  PV acc;  // TRAA accumulated plane of this frame
+};
+cudaError_t launch_traa_motion_blur(const TraaMotionBlurArgs& a, cudaStream_t s, const PeerPV* peer = nullptr);
 // K9 for pixel (x, y) of the W x H target (traa_compose.frag:3-6): the accumulated plane fetched LINEAR at the pixel centre, a = 1
 template <class S>
 RFX_D v4 traa_compose_px(const S& acc, int x, int y, int W, int H) {

@@ -704,6 +704,10 @@ class MotionBlurEffect(_Reactive):
     def update(self, renderer=None, inputBuffer=None, deltaTime=1 / 60, outputBuffer=None, window=None):
         """window = (innerWidth, innerHeight): the reference feeds the CSS window size as `resolution` (A10)."""
         ctx: engine.Context = inputBuffer.ctx
+        ctx.motion_blur(self.params(inputBuffer, deltaTime, window), self.velocityPass.texture, inputBuffer, outputBuffer)
+
+    def params(self, inputBuffer, deltaTime=1 / 60, window=None) -> abi.MotionBlurParams:
+        """this frame's uniforms (MotionBlurEffect.update, :87-102); advances the frame counter"""
         p = abi.MotionBlurParams()
         p.intensity, p.jitter = self._options["intensity"], self._options["jitter"]
         p.delta_time = max(1 / 1000, deltaTime)
@@ -711,7 +715,7 @@ class MotionBlurEffect(_Reactive):
         p.frame = self._frame % 4096  # renderer.info.render.frame % 4096
         p.samples = int(self._options["samples"])
         self._frame += 1
-        ctx.motion_blur(p, self.velocityPass.texture, inputBuffer, outputBuffer)
+        return p
 
 
 def getMaxMipLevel(width: int, height: int) -> int:
@@ -811,15 +815,26 @@ class SparkleEffect:
 class EffectPass:
     """postprocessing's `new EffectPass(camera, ...effects)` for the four effects above: the effects of one pass are merged into one
     fullscreen program — here ONE launch of rfx_effects_launch (csrc/k_fx.cu) — in which every effect samples the pass's input buffer
-    and the colour flows from one effect to the next in the given order."""
+    and the colour flows from one effect to the next in the given order.
+
+    `EffectPass(camera, traaEffect, motionBlurEffect)`, the second pass of the reference README's SSGI frame (readme.md:141-151), runs
+    TRAAEffect's temporal pass and then ONE launch of rfx_traa_motion_blur_launch: K9's colour is motion blur's inputColor, and its taps
+    sample the pass's input buffer (the frame before TRAA)."""
 
     def __init__(self, camera, *effects):
         if not 1 <= len(effects) <= 4:
             raise ValueError("EffectPass: 1..4 effects")
         self._camera, self.effects = camera, list(effects)
 
-    def render(self, renderer, inputBuffer, outputBuffer, deltaTime=None, stencilTest=None):
+    def render(self, renderer, inputBuffer, outputBuffer, deltaTime=None, stencilTest=None, window=None):
+        """window: MotionBlurEffect's `resolution` (the TRAA + motion-blur pass only; default the buffer's size)"""
         ctx: engine.Context = inputBuffer.ctx
+        if len(self.effects) == 2 and isinstance(self.effects[0], TRAAEffect) and isinstance(self.effects[1], MotionBlurEffect):
+            traa, mb = self.effects
+            traa.update(renderer, inputBuffer, deltaTime)
+            p = mb.params(inputBuffer, 1 / 60 if deltaTime is None else deltaTime, window)
+            ctx.traa_motion_blur(p, mb.velocityPass.texture, traa.temporalReprojectPass.accumulated, inputBuffer, outputBuffer)
+            return
         p = abi.make_effects_params(self._camera.uniforms(), [e.fx_id for e in self.effects])
         depth = velocity = None
         for e in self.effects:

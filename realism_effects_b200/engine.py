@@ -215,6 +215,10 @@ class Context:
     def traa_compose(self, acc, out, rows=(0, 0), stream=None):
         self._chk(self.lib.rfx_traa_compose_launch(self.h, stream, _r(acc), _r(out), rows[0], rows[1]))
 
+    def traa_motion_blur(self, p, velocity, acc, inp, out, rows=(0, 0), stream=None):
+        """K9 + K8 as one EffectPass: inputColor from the accumulated plane, the taps from `inp` (the pass's input buffer)"""
+        self._chk(self.lib.rfx_traa_motion_blur_launch(self.h, stream, C.byref(p), _r(velocity), _r(acc), _r(inp), _r(out), rows[0], rows[1]))
+
     def effects(self, p, inp, depth, velocity, out, rows=(0, 0), stream=None):
         """merged cosmetic effects (abi.make_effects_params): Sharpness / LensDistortion / GradualBackground / Sparkle in one launch"""
         self._chk(self.lib.rfx_effects_launch(self.h, stream, C.byref(p), _r(inp), _r(depth), _r(velocity), _r(out), rows[0], rows[1]))
@@ -270,6 +274,12 @@ class _Chain:
             return
         self.traa = options if options is not None else abi.make_traa_tail_options()
         self.ctx._chk(self._fn("enable_traa")(self.h, C.byref(self.traa)))
+
+    def set_motion_blur(self, params: "abi.MotionBlurParams | None"):
+        """Motion-blur stage of the TRAA tail (include/rfx.h: rfx_<kind>_chain_set_motion_blur): TRAAEffect and MotionBlurEffect as one
+        EffectPass, whose result replaces the K9 output.  params: this frame's MotionBlurEffect uniforms, passed before every frame
+        (frame, delta_time change); None turns the stage off."""
+        self.ctx._chk(self._fn("set_motion_blur")(self.h, C.byref(params) if params is not None else None))
 
     def output(self, which: int | None = None) -> Plane:
         """chain output `which` (the class docstring lists them; default: _DEFAULT_OUTPUT)"""

@@ -225,8 +225,9 @@ class ShardedSsgiChain:
     _CHAIN, _ATTACH = "SsgiChain", "rfx_group_attach_chain"  # the member chain's engine class and its collective attach
 
     def __init__(self, ctx, chain_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
-                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None):
-        """traa: abi.TraaTailOptions (abi.make_traa_tail_options()) to render the TRAA tail too (the same on every rank), or None"""
+                 rebalance_every: int = 4, rebalance_lag: int = 2, dist_group=None, traa=None, motion_blur=None):
+        """traa: abi.TraaTailOptions (abi.make_traa_tail_options()) to render the TRAA tail too (the same on every rank), or None.
+        motion_blur: abi.MotionBlurParams to turn the tail's motion-blur stage on (with traa; set_motion_blur updates it per frame)"""
         import ctypes as C
 
         from . import abi, engine
@@ -237,6 +238,8 @@ class ShardedSsgiChain:
         self.chain = getattr(engine, self._CHAIN)(ctx, chain_options)
         if traa is not None:  # before the attach: the group maps the tail's history plane then
             self.chain.enable_traa(traa)
+        if motion_blur is not None:  # before the attach too: the group maps the plane the stage's taps read
+            self.chain.set_motion_blur(motion_blur)
         g = C.c_void_p()
         ctx._chk(self.lib.rfx_group_create(ctx.h, unique_id, rank, world, C.byref(g)))
         self.g = g
@@ -280,10 +283,20 @@ class ShardedSsgiChain:
         return tuple(int(x) for x in b)
 
     # ---- device-resident frame ---------------------------------------------------------------------------------------
+    def set_motion_blur(self, params):
+        """this frame's MotionBlurEffect uniforms (the same on every rank; the stage was turned on at construction)"""
+        self.chain.set_motion_blur(params)
+
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None):
-        """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective."""
+        """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collectives.  Both
+        phases of a frame with the motion-blur stage (render_sharded, then render_sharded_finish; the latter is a no-op otherwise)."""
         f = self.chain._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
         self.ctx._chk(self.lib.rfx_ssgi_chain_render_sharded(self.chain.h, stream, self._C.byref(f)))
+        self._finish(stream)
+
+    def _finish(self, stream):
+        fn = "rfx_ao_chain_render_sharded_finish" if self._CHAIN == "AoChain" else "rfx_ssgi_chain_render_sharded_finish"
+        self.ctx._chk(getattr(self.lib, fn)(self.chain.h, stream))
 
     def download_band(self, which: int | None = None):
         """this rank's rows of chain output `which` (default: the chain's) of the last frame (numpy)"""
@@ -418,8 +431,9 @@ class InProcessGroup:
 
     _CHAIN, _ATTACH = "SsgiChain", "rfx_group_attach_chains_inprocess"  # the members' engine class and their attach
 
-    def __init__(self, ctxs, chain_options, world: int, traa=None):
-        """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None"""
+    def __init__(self, ctxs, chain_options, world: int, traa=None, motion_blur=None):
+        """traa: abi.TraaTailOptions to render the TRAA tail on every member, or None; motion_blur: abi.MotionBlurParams to turn the tail's
+        motion-blur stage on (set_motion_blur updates it per frame)"""
         import ctypes as C
 
         from . import abi, engine
@@ -432,6 +446,9 @@ class InProcessGroup:
         if traa is not None:
             for ch in self.chains:
                 ch.enable_traa(traa)
+        if motion_blur is not None:
+            for ch in self.chains:
+                ch.set_motion_blur(motion_blur)
         self.groups = []
         for r, c in enumerate(self.ctxs):
             g = C.c_void_p()
@@ -453,6 +470,11 @@ class InProcessGroup:
         for c, g in zip(self.ctxs, self.groups):
             c._chk(self.lib.rfx_group_set_bounds(g, b))
 
+    def set_motion_blur(self, params):
+        """this frame's MotionBlurEffect uniforms for every member (the stage was turned on at construction)"""
+        for ch in self.chains:
+            ch.set_motion_blur(params)
+
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, wait: bool = True):
         """one frame: every member renders its band; all of them finish before the next frame starts (the host is the barrier).
         wait=False skips the host wait: only for members that share one context, whose stream orders the members and the frames."""
@@ -460,7 +482,19 @@ class InProcessGroup:
         for c, ch in zip(self.ctxs, self.chains):
             f = ch._frame(cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved)
             c._chk(self.lib.rfx_ssgi_chain_render_sharded(ch.h, None, self._C.byref(f)))
-        if wait or len(set(self.ctxs)) > 1:
+        self._finish(wait)
+
+    def _finish(self, wait: bool):
+        """phase 2 of every member (a no-op without the motion-blur stage), after phase 1 of every member: one stream orders them; members
+        on several contexts are synchronised in between"""
+        fn = "rfx_ao_chain_render_sharded_finish" if self._CHAIN == "AoChain" else "rfx_ssgi_chain_render_sharded_finish"
+        several = len(set(self.ctxs)) > 1
+        if several:
+            for c in set(self.ctxs):
+                c.sync()
+        for c, ch in zip(self.ctxs, self.chains):
+            c._chk(getattr(self.lib, fn)(ch.h, None))
+        if wait or several:
             for c in set(self.ctxs):
                 c.sync()
 
@@ -502,6 +536,7 @@ class ShardedAoChain(ShardedSsgiChain):
         """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective.
         traa_cam / camera_moved: as AoChain.render, with the TRAA tail on."""
         _render_ao_band(self.ctx, self.chain, stream, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
+        self._finish(stream)
 
     def submit_host(self, *a, **k):
         raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the AO chain has no host-buffer path")
@@ -519,6 +554,4 @@ class InProcessAoGroup(InProcessGroup):
         self._last_bounds = self.bounds
         for c, ch in zip(self.ctxs, self.chains):
             _render_ao_band(c, ch, None, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
-        if wait or len(set(self.ctxs)) > 1:
-            for c in set(self.ctxs):
-                c.sync()
+        self._finish(wait)
