@@ -717,6 +717,31 @@ rfx_status rfx_ao_chain_render_traa(rfx_ao_chain* chain, void* stream, const rfx
  * iterations 0), of the latest frame; with the TRAA tail on, 2 the K7 output and 3 the TRAA accumulated plane (next frame's history).
  * 2 / 3 with the tail off: RFX_ERR_INVALID_ARG. */
 rfx_status rfx_ao_chain_output(rfx_ao_chain* chain, int32_t which, rfx_plane* out);
+/* host-buffer frame: uploads the input planes from (pinned) host memory into chain-owned staging planes, renders the frame
+ * (rfx_ao_chain_render, or rfx_ao_chain_render_traa with the TRAA tail on) and downloads out_color and out_ao.  Rows tightly packed. */
+typedef struct rfx_ao_host_frame {
+  float projection[16], projection_inverse[16], camera_matrix_world[16], view_matrix[16];
+  const float* depth;             /* W*H     fp32                                                                              */
+  const float* velocity;          /* W*H*4   fp32, VelocityDepthNormalPass layout                                              */
+  const uint8_t* normal;          /* W*H*4   RGBA8; required iff use_normal_plane                                              */
+  const uint16_t* input;          /* W*H*4   fp16 scene colour; NULL: no K7                                                    */
+  uint16_t* out_color;            /* W*H*4   fp16: what rfx_ao_frame.output receives; required iff input                       */
+  uint16_t* out_ao;               /* fp16 x 4, the size of output 1 (the plane K7 composes: W x H, or the AO target's size with
+                                     iterations 0); may be NULL; required if input is NULL                                     */
+  const rfx_ao_traa_frame* traa;  /* required iff the TRAA tail is on (then input / out_color are required)                     */
+} rfx_ao_host_frame;
+rfx_status rfx_ao_chain_render_host(rfx_ao_chain* chain, const rfx_ao_host_frame* frame);
+/* Pipelined form, as rfx_ssgi_chain_submit_host: submit enqueues the frame's H2D copies (copy stream, staging set frame&1), its
+ * kernels (context stream) and its D2H (third stream), ordered by events only, and returns without waiting.  wait_host blocks until
+ * at most max_in_flight (0 or 1) submitted frames are incomplete.  A frame's host buffers must stay untouched until it is complete,
+ * so a caller alternates two host buffer sets:
+ *     submit(frame i, set i&1);  wait_host(chain, 1);   // frame i-1 is complete, its set is free for frame i+1
+ * render_host(f) == submit_host(f) + wait_host(chain, 0).  Results are bit-identical to rfx_ao_chain_render / _render_traa on device
+ * planes.  A missing required pointer, or max_in_flight outside 0..1: RFX_ERR_INVALID_ARG.  A chain attached to a group of n > 1:
+ * RFX_ERR_UNSUPPORTED (each rank uploads its own rows and renders with rfx_ao_chain_render_sharded).  Between render_sharded and
+ * render_sharded_finish: RFX_ERR_NOT_READY. */
+rfx_status rfx_ao_chain_submit_host(rfx_ao_chain* chain, const rfx_ao_host_frame* frame);
+rfx_status rfx_ao_chain_wait_host(rfx_ao_chain* chain, int32_t max_in_flight);
 /* Row-sharded AO.  A group takes an AO chain or an SSGI chain, never both (RFX_ERR_INVALID_ARG).  No AO pass reads a produced plane at
  * an arbitrary uv: K6 / K6h read the caller's depth, the Poisson taps and K7 are bounded stencils, recomputed on widened ranges
  * (rfx_ao_shard_ranges).  In a group of n > 1 the AO target and Poisson targets A / B are double-buffered by frame parity and

@@ -662,3 +662,22 @@ export class InProcessGroup {
 	output(r, which = 0) { return rfx.chainOutput(this.ctxs[r], this.chains[r], which) }
 	dispose() { this.groups.forEach(g => rfx.groupDestroy(g)); this.chains.forEach(ch => rfx.chainDestroy(ch)); this.ctxs.forEach(c => rfx.ctxDestroy(c)) }
 }
+
+// ---- the native AO chain from host buffers (rfx_ao_chain_render_host / _submit_host / _wait_host) ---------------------------------------------
+// For hosts whose depth, velocity and colour live in host memory (offline compositing of rendered passes, a CPU-side or remote renderer):
+// K6 or K6h -> Poisson -> K7 on the GPU, with the uploads of frame i+1 and the download of frame i-1 running under frame i's kernels.
+// options: HBAOEffect's keys (HorizonAOEffect's with horizon: true) plus width / height and useNormalPass.  host: { depth: Float32Array,
+// velocity: Float32Array (VelocityDepthNormalPass layout), normal: Uint8Array (useNormalPass), input: Uint16Array RGBA16F | null,
+// outColor: Uint16Array | null (with input), outAo: Uint16Array | null (output 1, the plane K7 composes; required without input) }.
+export class AOHostChain {
+	constructor(options, device = 0) {
+		this.ctx = context(device)
+		this.chain = rfx.aoChainCreate(this.ctx, { ...defaultAOOptions, ...options })
+	}
+	frame(camera, host) { return { ...cameraBlock(camera), ...host } }
+	renderHost(camera, host) { rfx.aoChainRenderHost(this.ctx, this.chain, this.frame(camera, host)) }
+	// pipelined: alternate two host sets; after submitHost(frame i) waitHost(1) returns once frame i-1 is complete and its set is free
+	submitHost(camera, host) { rfx.aoChainSubmitHost(this.ctx, this.chain, this.frame(camera, host)) }
+	waitHost(maxInFlight = 0) { rfx.aoChainWaitHost(this.ctx, this.chain, maxInFlight) }
+	dispose() { rfx.aoChainDestroy(this.chain) }
+}

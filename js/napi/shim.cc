@@ -7,7 +7,8 @@
 //   c++ -std=c++17 -shared -fPIC -I<node prefix>/include/node -I../../include shim.cc -L../../realism_effects_b200/csrc -lrfx -o rfx_napi.node
 //
 // JS-side types: ctx / chain / plane are externals; matrices are Float32Array(16); planes travel as externals created by planeAlloc
-// (device memory) — host typed arrays cross only in planeUpload / planeDownload / envBuild / chainRenderHost.
+// (device memory) — host typed arrays cross only in planeUpload / planeDownload / envBuild / chainRenderHost /
+// aoChainRenderHost / aoChainSubmitHost.
 #include <node_api.h>
 
 #include <cstring>
@@ -226,6 +227,61 @@ napi_value ChainWaitHost(napi_env env, napi_callback_info info) {  // chainWaitH
   ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
   int32_t n = 0; napi_get_value_int32(env, argv[2], &n);
   CHECK(ctx, rfx_ssgi_chain_wait_host(unwrap<rfx_ssgi_chain>(env, argv[1]), n), "rfx_ssgi_chain_wait_host");
+  return undefined(env);
+}
+// ---- AO chain ---------------------------------------------------------------------------------------------------------------
+// aoChainCreate(ctx, options) -> aoChain: options = HBAOEffect's keys (src/ao/AOEffect.js:8-21 + PoissonDenoisePass's) or, with
+// horizon: true, HorizonAOEffect's; plus width, height and useNormalPass (the frames carry a normal plane)
+napi_value AoChainCreate(napi_env env, napi_callback_info info) {
+  ARGS(2); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  Obj b{env, argv[1]};
+  rfx_ao_chain_options o{};
+  o.width = (uint32_t)b.num("width", 0); o.height = (uint32_t)b.num("height", 0);
+  o.algorithm = b.num("horizon", 0) != 0 ? RFX_AO_HORIZON : RFX_AO_HBAO;
+  o.resolution_scale = (float)b.num("resolutionScale", 1); o.use_normal_plane = (int32_t)b.num("useNormalPass", 0);
+  o.spp = (int32_t)b.num("spp", 8); o.distance = (float)b.num("distance", 2); o.distance_power = (float)b.num("distancePower", 1);
+  o.bias = (float)b.num("bias", 40); o.thickness = (float)b.num("thickness", 0.075);
+  o.directions = (int32_t)b.num("directions", 8); o.steps = (int32_t)b.num("steps", 32); o.angle_bias = (float)b.num("angleBias", 0.1);
+  o.intensity = (float)b.num("intensity", 1); o.max_radius_pixels = (float)b.num("maxRadiusPixels", 64);
+  o.iterations = (int32_t)b.num("iterations", 1); o.radius = (float)b.num("radius", 3); o.phi = (float)b.num("phi", 0.5);
+  o.luma_phi = (float)b.num("lumaPhi", 5); o.depth_phi = (float)b.num("depthPhi", 2); o.normal_phi = (float)b.num("normalPhi", 3.25);
+  o.power = (float)b.num("power", 2);
+  b.floats("color", o.color, 3);
+  o.blue_noise_start = (int32_t)b.num("blueNoiseStart", 1234567); o.denoise_blue_noise_start = (int32_t)b.num("denoiseBlueNoiseStart", 1234567);
+  rfx_ao_chain* ch = nullptr;
+  CHECK(ctx, rfx_ao_chain_create(ctx, &o, &ch), "rfx_ao_chain_create");
+  return external(env, ch);
+}
+napi_value AoChainDestroy(napi_env env, napi_callback_info info) { ARGS(1); rfx_ao_chain_destroy(unwrap<rfx_ao_chain>(env, argv[0])); return undefined(env); }
+// aoChainRenderHost(ctx, aoChain, frame) / aoChainSubmitHost(ctx, aoChain, frame), frame = {projection, projectionInverse, matrixWorld,
+// matrixWorldInverse: Float32Array(16), depth: Float32Array, velocity: Float32Array, normal: Uint8Array|null, input: Uint16Array|null,
+// outColor: Uint16Array|null, outAo: Uint16Array|null} (a chain without the TRAA tail).  Submit only enqueues the frame; the caller
+// pairs it with aoChainWaitHost(ctx, aoChain, 1) and keeps the frame's typed arrays untouched until it completed.
+bool read_ao_host_frame(napi_env env, napi_value o, rfx_ao_host_frame* f) {
+  Obj b{env, o};
+  if (!b.f32("projection", f->projection, 16) || !b.f32("projectionInverse", f->projection_inverse, 16) ||
+      !b.f32("matrixWorld", f->camera_matrix_world, 16) || !b.f32("matrixWorldInverse", f->view_matrix, 16))
+    return false;
+  auto ptr = [&](const char* k) { return b.has(k) ? typed_ptr(env, b.get(k)) : nullptr; };
+  f->depth = (const float*)ptr("depth"); f->velocity = (const float*)ptr("velocity"); f->normal = (const uint8_t*)ptr("normal");
+  f->input = (const uint16_t*)ptr("input"); f->out_color = (uint16_t*)ptr("outColor"); f->out_ao = (uint16_t*)ptr("outAo");
+  return true;
+}
+napi_value AoChainHost(napi_env env, napi_callback_info info, bool sync) {
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  rfx_ao_host_frame f{};
+  if (!read_ao_host_frame(env, argv[2], &f)) { napi_throw_type_error(env, nullptr, "frame: expected Float32Array(16) matrices"); return nullptr; }
+  rfx_ao_chain* ch = unwrap<rfx_ao_chain>(env, argv[1]);
+  rfx_status st = sync ? rfx_ao_chain_render_host(ch, &f) : rfx_ao_chain_submit_host(ch, &f);
+  CHECK(ctx, st, sync ? "rfx_ao_chain_render_host" : "rfx_ao_chain_submit_host");
+  return undefined(env);
+}
+napi_value AoChainRenderHost(napi_env env, napi_callback_info info) { return AoChainHost(env, info, true); }
+napi_value AoChainSubmitHost(napi_env env, napi_callback_info info) { return AoChainHost(env, info, false); }
+napi_value AoChainWaitHost(napi_env env, napi_callback_info info) {  // aoChainWaitHost(ctx, aoChain, maxInFlight)
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  int32_t n = 0; napi_get_value_int32(env, argv[2], &n);
+  CHECK(ctx, rfx_ao_chain_wait_host(unwrap<rfx_ao_chain>(env, argv[1]), n), "rfx_ao_chain_wait_host");
   return undefined(env);
 }
 napi_value ChainReset(napi_env env, napi_callback_info info) { ARGS(1); rfx_ssgi_chain_reset(unwrap<rfx_ssgi_chain>(env, argv[0])); return undefined(env); }
@@ -489,6 +545,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("envBuild", EnvBuild), FN("envSet", EnvSet), FN("envClear", EnvClear), FN("planeAlloc", PlaneAlloc), FN("planeFree", PlaneFree),
       FN("planeUpload", PlaneUpload), FN("planeDownload", PlaneDownload), FN("chainCreate", ChainCreate), FN("chainSetOptions", ChainSetOptions),
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
+      FN("aoChainCreate", AoChainCreate), FN("aoChainDestroy", AoChainDestroy), FN("aoChainRenderHost", AoChainRenderHost), FN("aoChainSubmitHost", AoChainSubmitHost), FN("aoChainWaitHost", AoChainWaitHost),
       FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
       FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur), FN("traaMotionBlur", TraaMotionBlur), FN("chainSetMotionBlur", ChainSetMotionBlur),
       FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),

@@ -191,6 +191,13 @@ class AoTraaFrame(C.Structure):
     _fields_ = [("cam", CameraS), ("camera_pos", F3), ("camera_moved", C.c_int32)]
 
 
+class AoHostFrame(C.Structure):
+    """rfx_ao_host_frame: the camera matrices, host pointers of the input planes and of the two downloads, and the TRAA camera"""
+    _fields_ = [("projection", F16), ("projection_inverse", F16), ("camera_matrix_world", F16), ("view_matrix", F16),
+                ("depth", C.c_void_p), ("velocity", C.c_void_p), ("normal", C.c_void_p), ("input", C.c_void_p),
+                ("out_color", C.c_void_p), ("out_ao", C.c_void_p), ("traa", C.POINTER(AoTraaFrame))]
+
+
 def make_camera(u: dict, perspective: "bool | None" = None) -> CameraS:
     """u: dict from synth.Camera.uniforms() (float32 column-major arrays); perspective: camera.isPerspectiveCamera (default: u["perspective"], else True)."""
     if perspective is None:
@@ -317,6 +324,9 @@ def _sig(lib):
     lib.rfx_group_attach_ao_chains_inprocess.argtypes = [_P(vp), _P(vp), C.c_int32]
     lib.rfx_ao_chain_render_sharded.argtypes = [vp, vp, _P(AoFrame)]
     lib.rfx_ao_shard_ranges.argtypes = [u32, u32, u32, u32, C.c_int32, C.c_float, U32P, u32]
+    lib.rfx_ao_chain_render_host.argtypes = [vp, _P(AoHostFrame)]
+    lib.rfx_ao_chain_submit_host.argtypes = [vp, _P(AoHostFrame)]
+    lib.rfx_ao_chain_wait_host.argtypes = [vp, C.c_int32]
 
 
 EXPORTS = [
@@ -338,6 +348,7 @@ EXPORTS = [
     "rfx_ao_chain_enable_traa", "rfx_ao_chain_render_traa", "rfx_ao_chain_render_sharded_traa",
     "rfx_traa_motion_blur_launch", "rfx_ssgi_chain_set_motion_blur", "rfx_ao_chain_set_motion_blur",
     "rfx_ssgi_chain_render_sharded_finish", "rfx_ao_chain_render_sharded_finish",
+    "rfx_ao_chain_render_host", "rfx_ao_chain_submit_host", "rfx_ao_chain_wait_host",
 ]
 
 

@@ -1003,6 +1003,43 @@ struct GroupMember {
   bool group_peer = false;
   TraaTail tail;
 };
+// The copy pipeline of a chain's host-buffer path (rfx_*_chain_submit_host): two staging sets, so frame i+1 uploads while frame i
+// renders; H2D, kernels and D2H each get their own stream and are ordered by events only.  Frame i uses set i & 1: ev_up[set] fires
+// after its upload, ev_rendered[set] after its kernels, ev_dn[set] after its download.  Created at the first submit.
+struct HostPipe {
+  bool ready = false;
+  cudaStream_t s_up = nullptr, s_dn = nullptr;
+  cudaEvent_t ev_up[2]{}, ev_rendered[2]{}, ev_dn[2]{};
+  uint64_t submitted = 0;  // frames submitted
+  int set() const { return (int)(submitted & 1); }
+};
+static rfx_status host_pipe_init(rfx_ctx* ctx, HostPipe& p) {
+  if (p.ready) return RFX_OK;
+  CU(cudaStreamCreateWithFlags(&p.s_up, cudaStreamNonBlocking));
+  CU(cudaStreamCreateWithFlags(&p.s_dn, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; i++) {
+    CU(cudaEventCreateWithFlags(&p.ev_up[i], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&p.ev_rendered[i], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&p.ev_dn[i], cudaEventDisableTiming));
+  }
+  p.ready = true;
+  return RFX_OK;
+}
+static void host_pipe_destroy(HostPipe& p) {  // after the chain's last frame: waits for its copies
+  if (p.s_up) cudaStreamSynchronize(p.s_up);
+  if (p.s_dn) cudaStreamSynchronize(p.s_dn);
+  for (int i = 0; i < 2; i++) for (cudaEvent_t e : {p.ev_up[i], p.ev_rendered[i], p.ev_dn[i]}) if (e) cudaEventDestroy(e);
+  if (p.s_up) cudaStreamDestroy(p.s_up);
+  if (p.s_dn) cudaStreamDestroy(p.s_dn);
+}
+// Blocks until at most `max_in_flight` (0 or 1; larger values do not wait) submitted frames are incomplete.  Frames complete in
+// submission order: a complete frame's downloads are filled and its host input buffers may be overwritten.
+static rfx_status host_pipe_wait(rfx_ctx* ctx, const HostPipe& p, int32_t max_in_flight) {
+  if (p.submitted == 0 || !p.ready) return RFX_OK;
+  if (max_in_flight == 0) { CU(cudaEventSynchronize(p.ev_dn[(p.submitted - 1) & 1])); }
+  else if (max_in_flight == 1 && p.submitted >= 2) { CU(cudaEventSynchronize(p.ev_dn[(p.submitted - 2) & 1])); }
+  return RFX_OK;
+}
 struct rfx_ssgi_chain : GroupMember {
   rfx_ssgi_chain_options opt;
   rfx_plane ssgi_out{};
@@ -1019,13 +1056,9 @@ struct rfx_ssgi_chain : GroupMember {
   HistPlane fdnA, fdnB;
   uint64_t frame_idx = 0;    // frames completed (advances with the frame's last launch)
   bool views_valid = false;  // tr[]/dnB[] hold the split views of the current frame's interleaved planes
-  // host-buffer entry points: two staging sets so frame i+1 uploads while frame i renders; H2D, kernels and D2H each get
-  // their own stream and are ordered by events only (see rfx_ssgi_chain_submit_host)
+  // host-buffer entry points: the staging sets of the four input planes and their copy pipeline (see rfx_ssgi_chain_submit_host)
   rfx_plane in_depth[2]{}, in_gb[2]{}, in_vel[2]{}, in_direct[2]{};
-  bool have_staging = false;
-  cudaStream_t s_up = nullptr, s_dn = nullptr;
-  cudaEvent_t ev_up[2]{}, ev_rendered[2]{}, ev_dn[2]{};
-  uint64_t host_submitted = 0;
+  HostPipe host;
   int dn_buf[2] = {-1, -1};  // fast chain: which composed buffer the D2H of staging set 0 / 1 reads
   // cross-frame state (TemporalReprojectPass.js:203-213)
   bool have_prev = false;
@@ -1173,8 +1206,7 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   if (!ch) return;
   rfx_ctx* ctx = ch->ctx;
   cudaStreamSynchronize(ctx->stream);
-  if (ch->s_up) cudaStreamSynchronize(ch->s_up);
-  if (ch->s_dn) cudaStreamSynchronize(ch->s_dn);
+  host_pipe_destroy(ch->host);
   for (HistPlane* h : every_hist_plane(ch))
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ctx, &p);
   traa_free(ctx, ch->tail);
@@ -1182,9 +1214,6 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
   for (IPlane* p : {&ch->nrdz, &ch->tr32}) if (p->p) cudaFree(p->p);
-  for (int i = 0; i < 2; i++) for (cudaEvent_t e : {ch->ev_up[i], ch->ev_rendered[i], ch->ev_dn[i]}) if (e) cudaEventDestroy(e);
-  if (ch->s_up) cudaStreamDestroy(ch->s_up);
-  if (ch->s_dn) cudaStreamDestroy(ch->s_dn);
   for (auto& sp : ch->spans) { cudaEventDestroy(sp.a); cudaEventDestroy(sp.b); }
   for (cudaEvent_t e : ch->event_pool) cudaEventDestroy(e);
   delete ch;
@@ -1795,29 +1824,22 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
   if (!ch || !hf || !hf->depth || !hf->gbuffer || !hf->velocity || !hf->out_composed) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
   rfx_status st = RFX_OK;
-  if (!ch->have_staging) {
+  HostPipe& hp = ch->host;
+  if (!hp.ready) {
     auto alloc = [&](int fmt, rfx_plane* p) { if (st == RFX_OK) st = rfx_plane_alloc(ctx, fmt, ch->opt.width, ch->opt.height, p); };
     for (int i = 0; i < 2; i++) {
       alloc(RFX_FMT_R32F, &ch->in_depth[i]); alloc(RFX_FMT_RGBA32F, &ch->in_gb[i]); alloc(RFX_FMT_RGBA32F, &ch->in_vel[i]); alloc(RFX_FMT_RGBA16F, &ch->in_direct[i]);
     }
-    if (st != RFX_OK) return st;
-    CU(cudaStreamCreateWithFlags(&ch->s_up, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&ch->s_dn, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-      CU(cudaEventCreateWithFlags(&ch->ev_up[i], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&ch->ev_rendered[i], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&ch->ev_dn[i], cudaEventDisableTiming));
-    }
-    ch->have_staging = true;
+    if (st != RFX_OK || (st = host_pipe_init(ctx, hp)) != RFX_OK) return st;
   }
-  const int set = (int)(ch->host_submitted & 1);
-  if (ch->host_submitted >= 2) CU(cudaStreamWaitEvent(ch->s_up, ch->ev_rendered[set], 0));
-  if ((st = rfx_plane_upload(ctx, ch->s_up, &ch->in_depth[set], hf->depth, 0)) != RFX_OK) return st;
-  if ((st = rfx_plane_upload(ctx, ch->s_up, &ch->in_gb[set], hf->gbuffer, 0)) != RFX_OK) return st;
-  if (hf->direct_light && (st = rfx_plane_upload(ctx, ch->s_up, &ch->in_direct[set], hf->direct_light, 0)) != RFX_OK) return st;
-  if ((st = rfx_plane_upload(ctx, ch->s_up, &ch->in_vel[set], hf->velocity, 0)) != RFX_OK) return st;
-  CU(cudaEventRecord(ch->ev_up[set], ch->s_up));
-  CU(cudaStreamWaitEvent(ctx->stream, ch->ev_up[set], 0));
+  const int set = hp.set();
+  if (hp.submitted >= 2) CU(cudaStreamWaitEvent(hp.s_up, hp.ev_rendered[set], 0));
+  if ((st = rfx_plane_upload(ctx, hp.s_up, &ch->in_depth[set], hf->depth, 0)) != RFX_OK) return st;
+  if ((st = rfx_plane_upload(ctx, hp.s_up, &ch->in_gb[set], hf->gbuffer, 0)) != RFX_OK) return st;
+  if (hf->direct_light && (st = rfx_plane_upload(ctx, hp.s_up, &ch->in_direct[set], hf->direct_light, 0)) != RFX_OK) return st;
+  if ((st = rfx_plane_upload(ctx, hp.s_up, &ch->in_vel[set], hf->velocity, 0)) != RFX_OK) return st;
+  CU(cudaEventRecord(hp.ev_up[set], hp.s_up));
+  CU(cudaStreamWaitEvent(ctx->stream, hp.ev_up[set], 0));
   rfx_ssgi_frame f{};
   f.cam = hf->cam;
   f.depth = &ch->in_depth[set]; f.gbuffer = &ch->in_gb[set]; f.velocity = &ch->in_vel[set]; f.direct_light = hf->direct_light ? &ch->in_direct[set] : nullptr;
@@ -1829,7 +1851,7 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     // frames ago (long finished in steady state); frame i-1's D2H keeps running under this frame's kernels
     const int cur = (int)(ch->frame_idx & 1);
     for (int q = 0; q < 2; q++)
-      if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, ch->ev_dn[q], 0));
+      if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[q], 0));
     if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, 0xffffffffu)) != RFX_OK) return st;
     result = &ch->composed.buf[cur];
     ch->dn_buf[set] = cur;
@@ -1837,14 +1859,14 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     const uint32_t n_launches = 3u + 2u * (uint32_t)ch->opt.denoise_iterations;
     const uint32_t split = n_launches - 1;  // K4 is the only launch that writes `composed`
     if (split && (st = chain_render_impl(ch, nullptr, &f, nullptr, 0, split)) != RFX_OK) return st;
-    if (ch->host_submitted >= 1) CU(cudaStreamWaitEvent(ctx->stream, ch->ev_dn[set ^ 1], 0));
+    if (hp.submitted >= 1) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[set ^ 1], 0));
     if ((st = chain_render_impl(ch, nullptr, &f, nullptr, split, 0xffffffffu)) != RFX_OK) return st;
   }
-  CU(cudaEventRecord(ch->ev_rendered[set], ctx->stream));
-  CU(cudaStreamWaitEvent(ch->s_dn, ch->ev_rendered[set], 0));
-  if ((st = rfx_plane_download(ctx, ch->s_dn, result, hf->out_composed, 0)) != RFX_OK) return st;
-  CU(cudaEventRecord(ch->ev_dn[set], ch->s_dn));
-  ch->host_submitted++;
+  CU(cudaEventRecord(hp.ev_rendered[set], ctx->stream));
+  CU(cudaStreamWaitEvent(hp.s_dn, hp.ev_rendered[set], 0));
+  if ((st = rfx_plane_download(ctx, hp.s_dn, result, hf->out_composed, 0)) != RFX_OK) return st;
+  CU(cudaEventRecord(hp.ev_dn[set], hp.s_dn));
+  hp.submitted++;
   return RFX_OK;
 }
 
@@ -1852,11 +1874,7 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
 // filled and its input buffers may be overwritten.  Frames complete in submission order.
 rfx_status rfx_ssgi_chain_wait_host(rfx_ssgi_chain* ch, int32_t max_in_flight) {
   if (!ch || max_in_flight < 0) return RFX_ERR_INVALID_ARG;
-  rfx_ctx* ctx = ch->ctx;
-  if (ch->host_submitted == 0 || !ch->have_staging) return RFX_OK;
-  if (max_in_flight == 0) { CU(cudaEventSynchronize(ch->ev_dn[(ch->host_submitted - 1) & 1])); }
-  else if (max_in_flight == 1 && ch->host_submitted >= 2) { CU(cudaEventSynchronize(ch->ev_dn[(ch->host_submitted - 2) & 1])); }
-  return RFX_OK;
+  return host_pipe_wait(ch->ctx, ch->host, max_in_flight);
 }
 
 // synchronous form: one frame in, its result out
@@ -1880,6 +1898,10 @@ struct rfx_ao_chain : GroupMember {
   // the TRAA tail (`tail`: K7 into tail.mid, then the TRAA pass and K9 into frame->output) reads the previous frame's camera
   bool traa_have_prev = false;    // traa_prev holds the previous frame's camera
   rfx_ao_traa_frame traa_prev{};
+  // host-buffer path (rfx_ao_chain_submit_host): per staging set the input planes and the two planes its D2H reads; each plane is
+  // allocated (for both sets) by the first frame that needs it
+  HostPipe host;
+  rfx_plane in_depth[2]{}, in_vel[2]{}, in_normal[2]{}, in_input[2]{}, out_color[2]{}, out_ao[2]{};
 };
 
 static void ao_target_size(const rfx_ao_chain_options& o, uint32_t& w, uint32_t& h, float& rx, float& ry) {
@@ -1917,9 +1939,13 @@ rfx_status rfx_ao_chain_create(rfx_ctx* ctx, const rfx_ao_chain_options* opt, rf
 void rfx_ao_chain_destroy(rfx_ao_chain* ch) {
   if (!ch) return;
   cudaStreamSynchronize(ch->ctx->stream);
+  host_pipe_destroy(ch->host);
   for (HistPlane* h : {&ch->target, &ch->dnA, &ch->dnB})
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ch->ctx, &p);
   traa_free(ch->ctx, ch->tail);
+  for (int i = 0; i < 2; i++)
+    for (rfx_plane* p : {&ch->in_depth[i], &ch->in_vel[i], &ch->in_normal[i], &ch->in_input[i], &ch->out_color[i], &ch->out_ao[i]})
+      if (p->ptr) rfx_plane_free(ch->ctx, p);
   delete ch;
 }
 
@@ -2101,6 +2127,95 @@ rfx_status rfx_ao_chain_render_traa(rfx_ao_chain* ch, void* stream, const rfx_ao
   if (!ch || !f || !t) return RFX_ERR_INVALID_ARG;
   rfx_status st = ao_check_traa(ch, t, "ao_chain_render_traa");
   return st != RFX_OK ? st : ao_render_impl(ch, stream, f, nullptr, t);
+}
+
+}  // extern "C"
+
+// Host-buffer path: the pipeline of rfx_ssgi_chain_submit_host around ao_render_impl's launches.  Frame i uploads into staging set
+// i & 1 on the copy stream, renders on the context stream once ev_up fires, and downloads on the third stream once its kernels are done.
+// Hazards, all resolved on the device:
+//   staging set reuse - the upload of frame i+2 waits for frame i's kernels (ev_rendered);
+//   the downloaded planes - the chain renders its kept planes (AO target, Poisson targets, the tail's K7 and accumulated planes) in place,
+//     so frame i+1's kernels overwrite what frame i's D2H would read.  The tail's output and K7's output are frame->output, which here
+//     is the set's out_color plane.  Output 1 (Poisson target B, or the AO target) is copied on the context stream into the set's out_ao
+//     plane after the frame's kernels: a device copy of W*H*8 bytes, where ordering frame i+1's first writer of that plane after frame
+//     i's D2H would serialise the PCIe download with the next frame's kernels.  Both per-set planes are next written by frame i+2,
+//     whose kernels wait for frame i's D2H (ev_dn).
+static rfx_status ao_host_planes(rfx_ao_chain* ch, const rfx_ao_host_frame* hf) {
+  const uint32_t W = ch->opt.width, H = ch->opt.height;
+  rfx_status st = RFX_OK;
+  auto need = [&](bool used, int fmt, rfx_plane* p) {
+    for (int i = 0; i < 2; i++)
+      if (used && st == RFX_OK && !p[i].ptr) st = rfx_plane_alloc(ch->ctx, fmt, W, H, &p[i]);
+  };
+  need(true, RFX_FMT_R32F, ch->in_depth);
+  need(true, RFX_FMT_RGBA32F, ch->in_vel);
+  need(ch->opt.use_normal_plane != 0, RFX_FMT_RGBA8, ch->in_normal);
+  need(hf->input != nullptr, RFX_FMT_RGBA16F, ch->in_input);
+  need(hf->input != nullptr, RFX_FMT_RGBA16F, ch->out_color);
+  need(hf->out_ao != nullptr, RFX_FMT_RGBA16F, ch->out_ao);  // output 1 is at most W x H (the AO target is smaller with resolution_scale < 1)
+  return st != RFX_OK ? st : host_pipe_init(ch->ctx, ch->host);
+}
+
+extern "C" {
+
+rfx_status rfx_ao_chain_submit_host(rfx_ao_chain* ch, const rfx_ao_host_frame* hf) {
+  if (!ch || !hf) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (ch->tail.pending) return fail(ctx, RFX_ERR_NOT_READY, "ao_chain_submit_host: the last row-sharded frame waits for its second phase (render_sharded_finish)");
+  if (ch->group && rfx_group_world(ch->group) > 1)
+    return fail(ctx, RFX_ERR_UNSUPPORTED, "ao_chain_submit_host: the chain is in a row-sharded group of n > 1, whose ranks upload their own rows (parallel.ShardedAoChain.submit_host)");
+  if (!hf->depth || !hf->velocity) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_submit_host: depth and velocity are required");
+  if (ch->opt.use_normal_plane && !hf->normal) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_submit_host: use_normal_plane needs the normal plane");
+  if ((hf->input != nullptr) != (hf->out_color != nullptr)) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_submit_host: input and out_color go together (K7 composes input into out_color)");
+  if (!hf->input && !hf->out_ao) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_submit_host: without input the frame downloads out_ao, which may not be NULL then");
+  if (ch->tail.on && !hf->input) return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_submit_host: the TRAA tail renders into out_color over input: both are required");
+  rfx_status st = ao_check_traa(ch, hf->traa, "ao_chain_submit_host");
+  if (st != RFX_OK || (st = ao_host_planes(ch, hf)) != RFX_OK) return st;
+  HostPipe& hp = ch->host;
+  const int set = hp.set();
+  if (hp.submitted >= 2) CU(cudaStreamWaitEvent(hp.s_up, hp.ev_rendered[set], 0));
+  if ((st = rfx_plane_upload(ctx, hp.s_up, &ch->in_depth[set], hf->depth, 0)) != RFX_OK) return st;
+  if ((st = rfx_plane_upload(ctx, hp.s_up, &ch->in_vel[set], hf->velocity, 0)) != RFX_OK) return st;
+  if (ch->opt.use_normal_plane && (st = rfx_plane_upload(ctx, hp.s_up, &ch->in_normal[set], hf->normal, 0)) != RFX_OK) return st;
+  if (hf->input && (st = rfx_plane_upload(ctx, hp.s_up, &ch->in_input[set], hf->input, 0)) != RFX_OK) return st;
+  CU(cudaEventRecord(hp.ev_up[set], hp.s_up));
+  CU(cudaStreamWaitEvent(ctx->stream, hp.ev_up[set], 0));
+  if (hp.submitted >= 2) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[set], 0));  // out_color / out_ao of this set: frame i-2's D2H
+  rfx_ao_frame f{};
+  memcpy(f.projection, hf->projection, 64); memcpy(f.projection_inverse, hf->projection_inverse, 64);
+  memcpy(f.camera_matrix_world, hf->camera_matrix_world, 64); memcpy(f.view_matrix, hf->view_matrix, 64);
+  f.depth = &ch->in_depth[set]; f.velocity = &ch->in_vel[set];
+  f.normal = ch->opt.use_normal_plane ? &ch->in_normal[set] : nullptr;
+  f.input = hf->input ? &ch->in_input[set] : nullptr;
+  f.output = hf->input ? &ch->out_color[set] : nullptr;
+  if ((st = ao_render_impl(ch, nullptr, &f, nullptr, hf->traa)) != RFX_OK) return st;
+  rfx_plane ao{};
+  if (hf->out_ao) {
+    rfx_plane o1{};
+    if ((st = rfx_ao_chain_output(ch, 1, &o1)) != RFX_OK) return st;
+    ao = ch->out_ao[set];
+    ao.width = o1.width; ao.height = o1.height;
+    CU(cudaMemcpy2DAsync(ao.ptr, ao.pitch, o1.ptr, o1.pitch, (size_t)o1.width * 8, o1.height, cudaMemcpyDeviceToDevice, ctx->stream));
+  }
+  CU(cudaEventRecord(hp.ev_rendered[set], ctx->stream));
+  CU(cudaStreamWaitEvent(hp.s_dn, hp.ev_rendered[set], 0));
+  if (hf->input && (st = rfx_plane_download(ctx, hp.s_dn, &ch->out_color[set], hf->out_color, 0)) != RFX_OK) return st;
+  if (hf->out_ao && (st = rfx_plane_download(ctx, hp.s_dn, &ao, hf->out_ao, 0)) != RFX_OK) return st;
+  CU(cudaEventRecord(hp.ev_dn[set], hp.s_dn));
+  hp.submitted++;
+  return RFX_OK;
+}
+
+rfx_status rfx_ao_chain_wait_host(rfx_ao_chain* ch, int32_t max_in_flight) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  if (max_in_flight < 0 || max_in_flight > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_wait_host: max_in_flight must be 0 or 1 (two staging sets)");
+  return host_pipe_wait(ch->ctx, ch->host, max_in_flight);
+}
+
+rfx_status rfx_ao_chain_render_host(rfx_ao_chain* ch, const rfx_ao_host_frame* hf) {
+  rfx_status st = rfx_ao_chain_submit_host(ch, hf);
+  return st != RFX_OK ? st : rfx_ao_chain_wait_host(ch, 0);
 }
 
 }  // extern "C"

@@ -412,3 +412,36 @@ class AoChain(_Chain):
         else:
             t = self._traa_frame(traa_cam, camera_moved)
             self.ctx._chk(self.ctx.lib.rfx_ao_chain_render_traa(self.h, stream, C.byref(f), C.byref(t)))
+
+    def host_frame(self, cam_u: dict, depth, velocity, normal=None, inp=None, out_color=None, out_ao=None, traa_cam: dict | None = None,
+                   camera_moved: bool = True) -> abi.AoHostFrame:
+        """rfx_ao_host_frame over host arrays (numpy, or CPU torch tensors, pinned for asynchronous copies; rows tightly packed):
+        depth float32 H x W, velocity float32 H x W x 4, normal uint8 H x W x 4, inp float16 H x W x 4; out_color float16 H x W x 4 and
+        out_ao float16 (output 1's size) x 4 receive the frame.  traa_cam / camera_moved: as render(), with the TRAA tail on.  The
+        arrays must outlive the frame: the returned struct holds their addresses only."""
+        hf = abi.AoHostFrame()
+        for k in ("projection", "projection_inverse", "camera_matrix_world", "view_matrix"):
+            abi.set_f16(getattr(hf, k), cam_u[k])
+
+        def addr(a):
+            if a is None:
+                return None
+            return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
+
+        hf.depth, hf.velocity, hf.normal, hf.input = addr(depth), addr(velocity), addr(normal), addr(inp)
+        hf.out_color, hf.out_ao = addr(out_color), addr(out_ao)
+        if traa_cam is not None:
+            hf._traa = self._traa_frame(traa_cam, camera_moved)  # kept alive with the struct
+            hf.traa = C.pointer(hf._traa)
+        return hf
+
+    def render_host(self, hf: abi.AoHostFrame):
+        """one frame from host buffers (host_frame(...)), complete on return (include/rfx.h: rfx_ao_chain_render_host)"""
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_render_host(self.h, C.byref(hf)))
+
+    def submit_host(self, hf: abi.AoHostFrame):
+        """Pipelined host path: enqueue H2D -> chain -> D2H for one frame and return (include/rfx.h: rfx_ao_chain_submit_host)."""
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_submit_host(self.h, C.byref(hf)))
+
+    def wait_host(self, max_in_flight: int = 0):
+        self.ctx._chk(self.ctx.lib.rfx_ao_chain_wait_host(self.h, int(max_in_flight)))

@@ -144,6 +144,21 @@ class AoShardPlan:
         reaches = [self.poisson_halo] * (2 * self.iterations) + [self.K7_INPUT_ROWS] + ([ShardPlan.TRAA_TAIL_ROWS] if self.traa else [])
         return _widen_back(tuple(self.own), self.height, reaches)
 
+    @property
+    def local_input_rows(self) -> tuple:
+        """Rows of the PER-PIXEL input planes (velocity, normal, input) this rank reads, for the chain without the TRAA tail: the K6 / K6h
+        range (every later launch's range lies inside it) widened by the Poisson halo when there is a Poisson pass.
+          * velocity: the Poisson passes read it at their pixel (and its quad partner row, y ^ 1) and at taps up to the halo away; the fast
+            path decodes it once, on pass 0's range widened by the same halo (launch_gbuffer_decode).  Pass 0's range is the widest.
+          * normal: K6 / K6h fetch it NEAREST at the pixel centre, which is the pixel's own row: K6's range.
+          * input: K7 fetches it LINEAR at the pixel centre, which touches row y +- 1 (K7_INPUT_ROWS), and K7 runs on the band, so the rows
+            are the band +- 1: inside the last Poisson pass's range, or K6's range with iterations 0.
+        depth is sampled anywhere (K6 projects its samples, K6h marches up to maxRadiusPixels) and is needed whole.  With the TRAA tail the
+        TRAA pass reads velocity at reprojected uvs, so this plan does not cover it."""
+        a, b = self.ranges[0]
+        halo = self.poisson_halo if self.iterations > 0 else 0
+        return max(0, a - halo), min(self.height, b + halo)
+
 
 def rebalance(bounds, costs, measured_bounds=None, align: int = 16, min_rows: int = 64, max_share: float = 4.0, damping: float = 0.6):
     """New band borders from per-rank costs (any unit) measured with `measured_bounds` (default: `bounds`).
@@ -221,7 +236,8 @@ class ShardedSsgiChain:
     The 128-byte NCCL unique id travels over torch.distributed (any backend) when a process group is initialised, or is
     passed explicitly (`unique_id`, e.g. read from a file by a host without torch)."""
 
-    INPUTS = (("depth", 4, True), ("gbuffer", 16, False), ("velocity", 16, True), ("direct", 8, False))  # name, bytes/px, sampled anywhere
+    # name, bytes/px, sampled anywhere, format
+    INPUTS = (("depth", 4, True, "FMT_R32F"), ("gbuffer", 16, False, "FMT_RGBA32F"), ("velocity", 16, True, "FMT_RGBA32F"), ("direct", 8, False, "FMT_RGBA16F"))
     _CHAIN, _ATTACH = "SsgiChain", "rfx_group_attach_chain"  # the member chain's engine class and its collective attach
 
     def __init__(self, ctx, chain_options, rank: int | None = None, world: int | None = None, unique_id: bytes | None = None,
@@ -326,16 +342,13 @@ class ShardedSsgiChain:
         abi = self._abi
         dev = torch.device("cuda", self.ctx.device)
         W, H = self.chain.opt.width, self.chain.opt.height
-        fmts = dict(depth=abi.FMT_R32F, gbuffer=abi.FMT_RGBA32F, velocity=abi.FMT_RGBA32F, direct=abi.FMT_RGBA16F)
         h = dict(torch=torch, W=W, H=H, staging=[], frames=0)
         for _ in range(2):
             st = {}
-            for name, bpp, _g in self.INPUTS:
+            for name, bpp, _g, fmt in self.INPUTS:
                 t = torch.zeros(H * W * bpp, dtype=torch.uint8, device=dev)
-                st[name] = (t, _raw_plane(abi, t.data_ptr(), W, H, W * bpp, fmts[name]), W * bpp)
+                st[name] = (t, _raw_plane(abi, t.data_ptr(), W, H, W * bpp, getattr(abi, fmt)), W * bpp)
             h["staging"].append(st)
-        cap = H if self.world == 1 else min(H, int(self.MAX_SHARE * H / self.world) + 16)
-        h["out_dev"] = [torch.empty(cap * W * 16, dtype=torch.uint8, device=dev) for _ in range(2)]
         h["up"], h["dn"] = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
         h["main"] = torch.cuda.ExternalStream(self.ctx.stream, device=dev)
         h["ev_up"] = [torch.cuda.Event() for _ in range(2)]
@@ -355,21 +368,36 @@ class ShardedSsgiChain:
         if o.mode != self._abi.MODE_SSGI or o.denoise_mode != 0:
             raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path renders the fast SSGI chain only "
                                      "(mode SSGI, denoiseMode \"full\"): its upload rows are planned for that chain")
+
+        def rows(bounds):
+            return ShardPlan(o.height, self.world, self.rank, 2 * o.denoise_iterations, o.radius, True, bounds=bounds, width=o.width).local_input_rows
+
+        def render(st, plane):
+            self.render(cam, plane("depth"), plane("gbuffer"), plane("velocity"), plane("direct"), camera_pos, camera_moved)
+            # `composed` is double-buffered by frame parity: the plane of frame i is next written by frame i+2, which waits for this
+            # frame's D2H through ev_dn, so the rows go D2H straight from the plane
+            return self.chain.output(0)
+
+        return self._submit_host_frame(host, rows, render, out_host)
+
+    def _submit_host_frame(self, host: dict, local_rows, render, out_host):
+        """submit_host's pipeline: this rank's uploads into staging set (frame & 1) on the copy stream, the all-gather of the planes sampled
+        anywhere, render(staging set, plane of name) -> the plane whose band goes D2H, then that band on the third stream.
+        local_rows(bounds): the rows of the per-pixel input planes this rank reads."""
         if self._host is None:
             self._host_init()
         h = self._host
         torch, W, H = h["torch"], h["W"], h["H"]
         bounds = self.begin_frame()
         b0, b1 = bounds[self.rank], bounds[self.rank + 1]
-        plan = ShardPlan(H, self.world, self.rank, 2 * self.chain.opt.denoise_iterations, self.chain.opt.radius, True, bounds=bounds, width=W)
-        l0, l1 = plan.local_input_rows
+        l0, l1 = local_rows(bounds)
         k = h["frames"] & 1
         st = h["staging"][k]
         h2d = 0
         with torch.cuda.stream(h["up"]):
             if h["frames"] >= 2:
                 h["up"].wait_event(h["ev_rendered"][k])   # frame i-2 no longer reads this staging set
-            for name, bpp, anywhere in self.INPUTS:
+            for name, bpp, anywhere, _fmt in self.INPUTS:
                 if host.get(name) is None:
                     continue
                 t, _pl, pitch = st[name]
@@ -379,21 +407,19 @@ class ShardedSsgiChain:
             h["ev_up"][k].record(h["up"])
         with torch.cuda.stream(h["main"]):
             h["main"].wait_event(h["ev_up"][k])
-        if self.world > 1:  # complete depth / velocity from the other ranks' uploads (NVLink), ordered on the context stream
+            if h["frames"] >= 2:
+                h["main"].wait_event(h["ev_dn"][k])       # what frame i-2's D2H read (the set's staged output) may be written again
+        if self.world > 1:  # complete the planes sampled anywhere from the other ranks' uploads (NVLink), ordered on the context stream
             bnd = (self._C.c_uint32 * (self.world + 1))(*bounds)
-            for name, _bpp, anywhere in self.INPUTS:
+            for name, _bpp, anywhere, _fmt in self.INPUTS:
                 if anywhere and host.get(name) is not None:
                     self.ctx._chk(self.lib.rfx_group_allgather_rows(self.g, None, self._C.byref(st[name][1]), bnd))
-        pw = lambda n: _PlaneRef(st[n][1]) if host.get(n) is not None else None  # noqa: E731
-        self.render(cam, pw("depth"), pw("gbuffer"), pw("velocity"), pw("direct"), camera_pos, camera_moved)
-        p = self.chain.output(0)
-        nbytes = (b1 - b0) * W * 16
+        p = render(st, lambda n: _PlaneRef(st[n][1]) if host.get(n) is not None else None)
+        nbytes = (b1 - b0) * W * self._abi.FMT_BYTES[p.format]
         with torch.cuda.stream(h["main"]):
             h["ev_rendered"][k].record(h["main"])
         with torch.cuda.stream(h["dn"]):
             h["dn"].wait_event(h["ev_rendered"][k])
-            # `composed` is double-buffered by frame parity: the plane of frame i is next written by frame i+2, which waits for this
-            # copy through ev_dn (wait_host is called with at most one frame in flight), so the rows go D2H straight from the plane
             self.ctx._chk(self.lib.rfx_plane_download_rows(self.ctx.h, h["dn"].cuda_stream, self._C.byref(p), out_host.data_ptr(), b0, b1))
             h["ev_dn"][k].record(h["dn"])
         h["frames"] += 1
@@ -525,12 +551,25 @@ def _render_ao_band(ctx, chain, stream, frame: tuple, traa_cam, camera_moved: bo
         ctx._chk(ctx.lib.rfx_ao_chain_render_sharded_traa(chain.h, stream, C.byref(f), C.byref(t)))
 
 
+class _CudaRows:
+    """rows [0, n) x `row_bytes` bytes of device memory at `ptr` with a row pitch, for torch.as_tensor (__cuda_array_interface__)"""
+
+    def __init__(self, ptr: int, n: int, row_bytes: int, pitch: int):
+        self.__cuda_array_interface__ = {"shape": (n, row_bytes), "strides": (pitch, 1), "typestr": "|u1", "data": (ptr, False), "version": 2}
+
+
 class ShardedAoChain(ShardedSsgiChain):
     """This rank's member of a row-sharded AO chain: rfx_group_* + rfx_ao_chain_render_sharded.  The constructor (chain_options:
-    engine.ao_chain_options(...)), bands, rebalancing and the unique-id exchange are ShardedSsgiChain's; the host-buffer path is not (out of
-    scope for AO)."""
+    engine.ao_chain_options(...)), bands, rebalancing and the unique-id exchange are ShardedSsgiChain's.
+
+    Host-buffer path (submit_host / wait_host, without the TRAA tail): every rank moves only its share over PCIe.  depth, which K6 / K6h
+    sample anywhere, goes up as the rank's band and is completed from the other ranks' bands with rfx_group_allgather_rows; velocity,
+    the normal plane and the scene colour go up as AoShardPlan.local_input_rows.  The rank's band of the K7 output (or, without a scene
+    colour, of output 1) comes back D2H.  H2D, kernels and D2H run on three streams with two staging sets, as
+    rfx_ao_chain_submit_host does on one GPU."""
 
     _CHAIN, _ATTACH = "AoChain", "rfx_group_attach_ao_chain"
+    INPUTS = (("depth", 4, True, "FMT_R32F"), ("velocity", 16, False, "FMT_RGBA32F"), ("normal", 4, False, "FMT_RGBA8"), ("input", 8, False, "FMT_RGBA16F"))
 
     def render(self, cam_u, depth, velocity, normal=None, inp=None, out=None, stream=None, traa_cam=None, camera_moved: bool = True):
         """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collective.
@@ -538,8 +577,45 @@ class ShardedAoChain(ShardedSsgiChain):
         _render_ao_band(self.ctx, self.chain, stream, (cam_u, depth, velocity, normal, inp, out), traa_cam, camera_moved)
         self._finish(stream)
 
-    def submit_host(self, *a, **k):
-        raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the AO chain has no host-buffer path")
+    def _host_init(self):
+        super()._host_init()
+        h, abi = self._host, self._abi
+        W, H = h["W"], h["H"]
+        for st in h["staging"]:  # the plane the set's D2H reads: K7's output, or the band of output 1 copied out of the chain's plane
+            t = h["torch"].zeros(H * W * 8, dtype=h["torch"].uint8, device=st["depth"][0].device)
+            st["out"] = (t, _raw_plane(abi, t.data_ptr(), W, H, W * 8, abi.FMT_RGBA16F), W * 8)
+
+    def submit_host(self, cam_u: dict, host: dict, out_host):
+        """One frame from host planes (dict name -> CPU tensor of the FULL frame, pinned for asynchronous copies: depth, velocity, and
+        normal with use_normal_plane, input for K7) to this rank's rows of the K7 output (with `input`) or of output 1 (without), written to
+        the start of out_host (CPU tensor of at least MAX_SHARE x the mean band height x W x 8 bytes).  Returns the band (row0, row1) the
+        rows belong to, after enqueueing.  Not with the TRAA tail (ERR_UNSUPPORTED): its pass reads velocity at reprojected uvs, which the
+        uploaded rows (AoShardPlan.local_input_rows) do not cover."""
+        abi = self._abi
+        if self.chain.traa is not None:
+            raise abi.RfxError(f"rfx status {abi.ERR_UNSUPPORTED}: submit_host: the sharded host path does not render the TRAA tail")
+        if host.get("depth") is None or host.get("velocity") is None:
+            raise abi.RfxError("submit_host: depth and velocity are required")
+        o = self.chain.opt
+
+        def rows(bounds):
+            return AoShardPlan(o.width, o.height, (bounds[self.rank], bounds[self.rank + 1]), o.iterations, o.radius).local_input_rows
+
+        def render(st, plane):
+            out = st["out"]
+            with_k7 = host.get("input") is not None
+            self.render(cam_u, plane("depth"), plane("velocity"), plane("normal"), plane("input"), _PlaneRef(out[1]) if with_k7 else None)
+            if not with_k7:
+                # output 1 is rendered in place (alone) or by frame parity (in a group), and the next frame's kernels may write it while
+                # this band is still going D2H: copy the band into the set's plane on the context stream first
+                torch, (b0, b1) = self._host["torch"], self.band_of_last_frame
+                p = self.chain.output(1)
+                src = torch.as_tensor(_CudaRows(p.ptr + b0 * p.pitch, b1 - b0, p.width * 8, p.pitch), device=out[0].device)
+                with torch.cuda.stream(self._host["main"]):
+                    out[0].view(self._host["H"], out[2])[b0:b1].copy_(src)
+            return out[1]
+
+        return self._submit_host_frame(host, rows, render, out_host)
 
 
 class InProcessAoGroup(InProcessGroup):
