@@ -12,7 +12,8 @@
 //   * when the projection matrix has the perspective sparsity pattern (detected on the host) the
 //     fma chain of `projectionMatrix * vec4(p, 1)` drops its exact-zero terms: x' = fma(P00,x,P20*z),
 //     y' = fma(P11,y,P21*z), w' = -z — bit-identical to the full chain;
-//   * the fast variant (ssgi_fast_kernel) projects and fetches RFX_K1_BATCH march steps together and tests them in order.
+//   * the fast variant (ssgi_fast_kernel) marches a pixel's two rays together, RFX_K1_BATCH steps of each projected and fetched
+//     together and tested in order.
 // All blue-noise driven transcendentals (sin/cos of 2*pi*k/255, the march step profile
 // 1-exp(-0.25 (i+b-0.5)^2)) come from small host-built tables indexed by the 8-bit noise value.
 // FAST = true additionally moves the remaining continuous transcendentals to the SFU pipe.
@@ -502,60 +503,90 @@ RFX_D v3 fma3(v3 d, float s, v3 p) {
   const f2 xy = f2fma(mkf2(d.x, d.y), mkf2(s), mkf2(p.x, p.y));
   return mk3(f2lo(xy), f2hi(xy), fma_(d.z, s, p.z));
 }
-// RayMarch + BinarySearch  ssgi.frag:441-503.  The ray positions do not depend on the fetched depths, so BATCH steps are projected
-// and fetched together and tested in order: the march is a chain of dependent L2-latency gathers (L1 hit ~50 %), and at ~25
-// instructions per tap the other resident warps no longer hide that latency on their own (at most BATCH - 1 wasted taps per hit).
+// RayMarch + BinarySearch  ssgi.frag:441-503 for a pixel's two rays (diffuse, specular) at once.  The ray positions do not depend on
+// the fetched depths, so BATCH steps of each live ray are projected and fetched together and then tested in order: the march is a
+// chain of dependent L2-latency gathers (L1 hit ~50 %), and at ~25 instructions per tap the other resident warps no longer hide that
+// latency on their own (at most BATCH - 1 wasted taps per hit).  Marching the two rays in one loop puts both rays' fetches in flight
+// together, where the shader marches them one after the other; each ray's operations are the shader's, step for step.
+// Ray r is live when live[r]; `dir[r]` is scaled in place like the shader's inout, `p[r]` enters as the origin and leaves as hitPos
+// (10e9 on a miss).  Returns the hit uvs in uv[r]; a miss keeps the uv of the last step tested, and with steps = 1 none is: (0, 0).
 #ifndef RFX_K1_BATCH
-#define RFX_K1_BATCH 4  // tools/sweep_k1.sh on H100 at 4K: 2 and 4 are within the run-to-run spread, 1 is slower
+#define RFX_K1_BATCH 2  // per ray, so 4 fetches per round with both rays live; H100 at 4K: 4 spills in the march loop and is slower
 #endif
 static_assert(RFX_K1_BATCH >= 1 && RFX_K1_BATCH <= 4, "the host step table (ensure_step_table) carries 3 spare rows for the speculative reads");
 template <bool SPARSE>
-RFX_D v2 march_fast(const SsgiArgs& a, v3& dir, v3& hitPos, int noiseB, bool& hit) {
+RFX_D void march_fast2(const SsgiArgs& a, v3 dir[2], v3 p[2], const bool live[2], int noiseB, bool hit[2], v2 uv[2]) {
   constexpr int BATCH = RFX_K1_BATCH;
-  dir = dir * (a.ray_distance / (float)a.steps);
-  hit = false;
+  bool run[2];
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+    dir[r] = dir[r] * (a.ray_distance / (float)a.steps);
+    hit[r] = false;
+    run[r] = live[r];
+  }
   const float* cs_row = a.step_table + noiseB;  // row i-1 holds cs(i, b); the table carries BATCH spare rows for the speculative reads
-  v3 p = hitPos;
-  for (int i = 1; i < a.steps && !hit; i += BATCH, cs_row += 256 * BATCH) {
-    v3 q[BATCH];
-    float z[BATCH];
-    v3 t = p;
+  for (int i = 1; i < a.steps && (run[0] || run[1]); i += BATCH, cs_row += 256 * BATCH) {
+    float c[BATCH];
 #pragma unroll
-    for (int k = 0; k < BATCH; k++) {  // BATCH steps are projected and fetched together ...
-      t = fma3(dir, __ldg(cs_row + 256 * k), t);
-      q[k] = t;
-      z[k] = tap_viewz<SPARSE>(a, t);
-    }
+    for (int k = 0; k < BATCH; k++) c[k] = __ldg(cs_row + 256 * k);  // both rays start from the pixel's noise value
+    float z[2][BATCH];
 #pragma unroll
-    for (int k = 0; k < BATCH; k++) {  // ... and tested in order
-      if (!hit && i + k < a.steps) {
-        p = q[k];
-        const float d = z[k] - q[k].z;
-        hit = d >= 0.0f && d < a.thickness;
+    for (int r = 0; r < 2; r++) {  // BATCH steps of each ray are projected and fetched together ...
+      v3 t = p[r];
+#pragma unroll
+      for (int k = 0; k < BATCH; k++) {
+        t = fma3(dir[r], c[k], t);
+        z[r][k] = run[r] ? tap_viewz<SPARSE>(a, t) : 0.0f;
       }
     }
-  }
-  if (!hit) {  // the shader returns the uv of the last step tested; with steps = 1 none is, and its uv keeps (0, 0)
-    hitPos = mk3(10.0e9f);
-    return a.steps > 1 ? view_to_screen<SPARSE, true>(a, p) : mk2(0.0f, 0.0f);
-  }
-  if (a.refine_steps > 0) {
-    dir = dir * 0.5f;
-    p = p - dir;
-    for (int r = 0; r < a.refine_steps; r++) {
-      const float diff = tap_viewz<SPARSE>(a, p) - p.z;
-      dir = dir * 0.5f;
-      p = diff >= 0.0f ? p - dir : p + dir;
+#pragma unroll
+    for (int r = 0; r < 2; r++) {  // ... and tested in order (the positions are recomputed, the same fma chain, to save registers)
+      if (!run[r]) continue;
+      v3 t = p[r];
+#pragma unroll
+      for (int k = 0; k < BATCH; k++) {
+        t = fma3(dir[r], c[k], t);
+        if (!hit[r] && i + k < a.steps) {
+          p[r] = t;
+          const float d = z[r][k] - t.z;
+          hit[r] = d >= 0.0f && d < a.thickness;
+        }
+      }
+      run[r] = !hit[r];
     }
   }
-  hitPos = p;
-  return view_to_screen<SPARSE, true>(a, p);
+  bool refine[2];
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+    refine[r] = live[r] && hit[r] && a.refine_steps > 0;
+    if (refine[r]) {
+      dir[r] = dir[r] * 0.5f;
+      p[r] = p[r] - dir[r];
+    }
+  }
+  for (int n = 0; n < a.refine_steps && (refine[0] || refine[1]); n++) {
+    float z[2];
+#pragma unroll
+    for (int r = 0; r < 2; r++) z[r] = refine[r] ? tap_viewz<SPARSE>(a, p[r]) : 0.0f;
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+      if (!refine[r]) continue;
+      const float diff = z[r] - p[r].z;
+      dir[r] = dir[r] * 0.5f;
+      p[r] = diff >= 0.0f ? p[r] - dir[r] : p[r] + dir[r];
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 2; r++) {
+    if (!live[r]) continue;
+    uv[r] = hit[r] || a.steps > 1 ? view_to_screen<SPARSE, true>(a, p[r]) : mk2(0.0f, 0.0f);
+    if (!hit[r]) p[r] = mk3(10.0e9f);
+  }
 }
 
-// doSample  ssgi.frag:362-439 (SFU arithmetic; `desat` = (1 - roughnessSq) * saturation(diffuse) * 0.4)
-template <bool SPARSE, bool PEER>
-RFX_D v3 sample_fast(const SsgiArgs& a, v3 viewPos, v3 viewNormal, float roughnessSq, float metalness, float desat, bool isDiffuseSample, bool isEnvSample, float NoV,
-                     float NoL, float NoH, float LoH, int noiseB, v3 l, v3& hitPos, float& brdf, float& pdf) {
+// doSample  ssgi.frag:362-439 (SFU arithmetic), before the march: the ray's brdf (cosine-weighted) and pdf
+RFX_D void sample_fast_brdf(v3 viewNormal, float roughnessSq, float metalness, bool isDiffuseSample, float NoV, float NoL, float NoH, float LoH, v3 l,
+                            float& brdf, float& pdf) {
   const float cosTheta = fmaxf(0.0f, dot(viewNormal, l));
   if (isDiffuseSample) {
     brdf = evalDisneyDiffuse<true>(NoL, NoV, LoH, roughnessSq, metalness);
@@ -566,9 +597,12 @@ RFX_D v3 sample_fast(const SsgiArgs& a, v3 viewPos, v3 viewNormal, float roughne
   }
   brdf *= cosTheta;
   pdf = fmaxf(SSGI_EPSILON, pdf);
-  hitPos = viewPos;
-  bool hit;
-  const v2 coords = march_fast<SPARSE>(a, l, hitPos, noiseB, hit);
+}
+
+// doSample after the march: `l` is the ray's direction as the march left it, `coords` and `hit` its result.
+// `desat` = (1 - roughnessSq) * saturation(diffuse) * 0.4.
+template <bool PEER>
+RFX_D v3 sample_fast_shade(const SsgiArgs& a, float roughnessSq, float desat, bool isDiffuseSample, bool isEnvSample, v3 l, v2 coords, bool hit) {
   const bool allowMissedRays = (a.flags & RFX_SSGI_MISSED_RAYS) != 0;
   if (!hit && !allowMissedRays) return getEnvColor<true, true>(a, l, roughnessSq, isDiffuseSample, isEnvSample);
   v2 vel = mk2(0.0f, 0.0f);
@@ -700,23 +734,34 @@ __global__ void __launch_bounds__(kThreads, RFX_K1_MIN_BLOCKS) ssgi_fast_kernel(
   }
   const float desat = (1.0f - roughnessSq) * getSaturation<true>(m.diffuse) * 0.4f;
   const float inv_ems = rcp_<true>(emsPdf);
-  v3 diffuseGI = mk3(0.0f), specularGI, hitPos;
-  float brdf, pdf;
-  if (MODE == RFX_MODE_SSGI && isDiffuseSample) {  // :222-242
-    const v3 dray = emsIsEnvSample ? envMisDir : cosineSampleHemisphere_cs<true>(viewNormal, random.x, sc.x, sc.y);
-    calculateAngles<true>(dray, v, n, NoL, NoH, LoH, VoH);
-    v3 gi = sample_fast<SPARSE, PEER>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, true, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, dray, hitPos, brdf, pdf);
-    gi = gi * brdf;
-    if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, pdf);
+  const bool diffuse = MODE == RFX_MODE_SSGI && isDiffuseSample;  // :222-242, then the specular ray :246-265
+  v3 dir[2] = {mk3(0.0f), l}, p[2] = {viewPos, viewPos};
+  float dBrdf = 0.0f, dPdf = 0.0f, sBrdf, sPdf;
+  if (diffuse) {
+    dir[0] = emsIsEnvSample ? envMisDir : cosineSampleHemisphere_cs<true>(viewNormal, random.x, sc.x, sc.y);
+    calculateAngles<true>(dir[0], v, n, NoL, NoH, LoH, VoH);
+    sample_fast_brdf(viewNormal, roughnessSq, m.metalness, true, NoV, NoL, NoH, LoH, dir[0], dBrdf, dPdf);
+  }
+  calculateAngles<true>(l, v, n, NoL, NoH, LoH, VoH);
+  sample_fast_brdf(viewNormal, roughnessSq, m.metalness, isDiffuseSample, NoV, NoL, NoH, LoH, l, sBrdf, sPdf);
+  const bool live[2] = {diffuse, true};
+  bool hit[2];
+  v2 coords[2];
+  march_fast2<SPARSE>(a, dir, p, live, bn.z, hit, coords);
+  v3 diffuseGI = mk3(0.0f), specularGI;
+  if (diffuse) {
+    v3 gi = sample_fast_shade<PEER>(a, roughnessSq, desat, true, emsIsEnvSample, dir[0], coords[0], hit[0]);
+    gi = gi * dBrdf;
+    if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = dPdf * dPdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, dPdf);
     diffuseGI = gi * inv_ems;
   }
-  calculateAngles<true>(l, v, n, NoL, NoH, LoH, VoH);  // the specular ray :246-265
   {
-    v3 gi = sample_fast<SPARSE, PEER>(a, viewPos, viewNormal, roughnessSq, m.metalness, desat, isDiffuseSample, emsIsEnvSample, NoV, NoL, NoH, LoH, bn.z, l, hitPos, brdf, pdf);
-    gi = gi * brdf;
-    if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = pdf * pdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, pdf);
+    v3 gi = sample_fast_shade<PEER>(a, roughnessSq, desat, isDiffuseSample, emsIsEnvSample, dir[1], coords[1], hit[1]);
+    gi = gi * sBrdf;
+    if (emsIsEnvSample) { const float aa = emsPdf * emsPdf, bb = sPdf * sPdf; gi = gi * div_<true>(aa, aa + bb); } else gi = vdiv_<true>(gi, sPdf);
     specularGI = gi * inv_ems;
   }
+  const v3 hitPos = p[1];
   float rayLength = 0.0f;
   if (!(hitPos.x > 10.0e8f)) {  // :288-296
     const v3 cameraPosWS = mk3(a.cam.camera_matrix_world.m[12], a.cam.camera_matrix_world.m[13], a.cam.camera_matrix_world.m[14]);
