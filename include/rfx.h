@@ -520,9 +520,22 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* chain, const rfx_traa_tail
  * (RFX_ERR_UNSUPPORTED); its values can change (every rank passes the same).  In a row-sharded group of n > 1 a frame with the stage has
  * two phases: rfx_ssgi_chain_render_sharded, then rfx_ssgi_chain_render_sharded_finish. */
 rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* chain, const rfx_motion_blur_params* p);
+/* Cosmetic stage of the TRAA tail: the third EffectPass of the reference demo's frame, `new EffectPass(camera, sharpnessEffect, ...)`
+ * (example/main.js:517-538), as the last pass of the chain's frame.  With the stage on, one rfx_effects_launch with p's effect list, order
+ * and values runs over the tail's image (K9's, or the merged TRAA + motion-blur pass's), with the frame's own depth (GradualBackground) and
+ * velocity (Sparkle) planes, into a chain-owned RGBA16F plane that becomes output 6; output 8 is then the stage's input.  The bytes are
+ * those of the tail followed by rfx_effects_launch with the same p.  The fused fast tail stays in use (its K9 plane is the stage's input).
+ * The host passes p before every frame, camera included (GradualBackground and Sparkle read the camera's uniforms as they stand when the
+ * EffectPass renders).  p == NULL turns the stage off and frees its plane; enable_traa(NULL) turns it off with the tail.  Tail off:
+ * RFX_ERR_NOT_READY; n_effects outside 1..4 or an unknown RFX_FX_*: RFX_ERR_INVALID_ARG; between rfx_ssgi_chain_render_sharded and
+ * rfx_ssgi_chain_render_sharded_finish: RFX_ERR_NOT_READY.  The stage keeps no plane across frames and no rank reads another rank's copy
+ * of it, so in a row-sharded group it may be turned on or off, and its values changed, between any two frames; every rank passes the same
+ * p (rfx_fx_stage_rows, below, is what each rank recomputes around its band). */
+rfx_status rfx_ssgi_chain_set_effects(rfx_ssgi_chain* chain, const rfx_effects_params* p);
 /* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the tail's output (RGBA16F: K9's, or
- * with the motion-blur stage on the merged TRAA + motion-blur pass's), 7 the TRAA accumulated plane of the latest frame (RGBA16F; next
- * frame's history).  6 / 7 with the tail off: RFX_ERR_NOT_READY. */
+ * with the motion-blur stage on the merged TRAA + motion-blur pass's; with the cosmetic stage on the stage's, the frame's final image), 7
+ * the TRAA accumulated plane of the latest frame (RGBA16F; next frame's history); with the cosmetic stage on, 8 the stage's input (the
+ * image output 6 holds with the stage off).  6 / 7 with the tail off, 8 with the stage off: RFX_ERR_NOT_READY. */
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane* out);
 /* Debug view of the TRAA tail: SSGIEffect's `outputTexture` (src/ssgi/SSGIEffect.js:228-251, picked from the "Debug" list of
  * example/SSGIDebugGUI.js:78-114).  With a view selected, the tail's K5 runs with isDebug and samples the view instead of `composed`
@@ -703,6 +716,11 @@ rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* chain, const rfx_traa_tail_opt
  * cannot be turned on or off (RFX_ERR_UNSUPPORTED).  In such a group a frame with the stage has two phases:
  * rfx_ao_chain_render_sharded_traa, then rfx_ao_chain_render_sharded_finish. */
 rfx_status rfx_ao_chain_set_motion_blur(rfx_ao_chain* chain, const rfx_motion_blur_params* p);
+/* Cosmetic stage of the AO chain's TRAA tail, as rfx_ssgi_chain_set_effects: the tail writes a chain-owned RGBA16F plane (allocated when
+ * the stage is turned on, freed when it is turned off; output 4) and the stage writes frame->output, so rfx_ao_chain_render_host /
+ * submit_host download the stage's image.  Same statuses, same rules in groups (between render_sharded_traa and render_sharded_finish:
+ * RFX_ERR_NOT_READY). */
+rfx_status rfx_ao_chain_set_effects(rfx_ao_chain* chain, const rfx_effects_params* p);
 /* What the TRAA pass needs and rfx_ao_frame lacks: near / far, the perspective flag and the position of the UN-jittered camera (jittering
  * the rasteriser, TAAUtils.js, stays the host's job), and didCameraMove (src/utils/SceneUtils.js:17-27) for fullAccumulate.  The chain
  * keeps the previous frame's camera; on the first frame and after rfx_ao_chain_reset the previous camera is the current one. */
@@ -715,7 +733,7 @@ typedef struct rfx_ao_traa_frame {
 rfx_status rfx_ao_chain_render_traa(rfx_ao_chain* chain, void* stream, const rfx_ao_frame* frame, const rfx_ao_traa_frame* traa);
 /* which: 0 the AO target (RGBA16F, the scaled size), 1 the denoised plane K7 composes (Poisson target B; the AO target with
  * iterations 0), of the latest frame; with the TRAA tail on, 2 the K7 output and 3 the TRAA accumulated plane (next frame's history).
- * 2 / 3 with the tail off: RFX_ERR_INVALID_ARG. */
+ * 2 / 3 with the tail off: RFX_ERR_INVALID_ARG.  4: the cosmetic stage's input (the tail's image); with the stage off RFX_ERR_NOT_READY. */
 rfx_status rfx_ao_chain_output(rfx_ao_chain* chain, int32_t which, rfx_plane* out);
 /* host-buffer frame: uploads the input planes from (pinned) host memory into chain-owned staging planes, renders the frame
  * (rfx_ao_chain_render, or rfx_ao_chain_render_traa with the TRAA tail on) and downloads out_color and out_ao.  Rows tightly packed. */
@@ -769,6 +787,15 @@ rfx_status rfx_ao_chain_render_sharded_finish(rfx_ao_chain* chain, void* stream)
  * RFX_TRAA_TAIL_ROWS (every earlier launch widens from K7's range as above). */
 rfx_status rfx_ao_shard_ranges(uint32_t width, uint32_t height, uint32_t own0, uint32_t own1, int32_t iterations, float radius,
                                uint32_t* ranges, uint32_t n_launches);
+/* pure host arithmetic: rows [rows[0], rows[1]) of the tail's image that the cosmetic stage (rfx_*_chain_set_effects) reads for its output
+ * band [own0, own1) of a width x height frame.  Its pixel-centre LINEAR fetch: the band +- 1 row; Sharpness's 3x3 LINEAR taps: +- 2 rows;
+ * GradualBackground and Sparkle: nothing more; LensDistortion: every row its three aberrated, distorted LINEAR taps touch, taken from a
+ * table of the lowest and highest source row per output row (fx_lens's uv arithmetic evaluated in IEEE fp32 for every pixel, clamped to
+ * the frame as the sampler clamps; a non-finite or out-of-range coordinate: every row).  The table depends on width, height, alphax,
+ * alphay and aberration only, and is kept while they stay the same.  In a row-sharded group with the stage on, the tail's last launch runs
+ * on these rows instead of the band (every earlier launch widens from there, as rfx_shard_ranges / rfx_ao_shard_ranges with own0, own1 =
+ * rows), and the stage on the band.  A bad p (NULL, n_effects outside 1..4, an unknown RFX_FX_*) or band: RFX_ERR_INVALID_ARG. */
+rfx_status rfx_fx_stage_rows(uint32_t width, uint32_t height, const rfx_effects_params* p, uint32_t own0, uint32_t own1, uint32_t rows[2]);
 
 /* Per-pass device timing (CUDA events recorded on the launching stream around every kernel of
  * the chain).  Slots: 0 K1 trace, 1 K2 temporal, 2 K3 pass 0, 3 K3 passes >= 1, 4 K4 compose.

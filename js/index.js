@@ -602,10 +602,16 @@ export class RfxEffectPass {
 		if (!this.planes || inputBuffer.width !== this.width) this.setSize(inputBuffer.width, inputBuffer.height)
 		renderer.readRenderTargetPixels(inputBuffer, 0, 0, this.width, this.height, this.hostIn)
 		rfx.planeUpload(this.ctx, this.planes.input, this.hostIn)
-		const p = { cam: cameraBlock(this.camera), count: this.effects.length, effects: this.effects.map(e => e.fxId) }
-		for (const e of this.effects) { e.update(renderer, inputBuffer, deltaTime); e.fill(p) }
+		const p = this.params(renderer, inputBuffer, deltaTime)
 		rfx.effects(this.ctx, p, this.planes.input, planes.depth ?? null, planes.velocity ?? null, this.planes.output)
 		rfx.planeDownload(this.ctx, this.planes.output, this.outputHost)
+	}
+	// the values this pass launches with (effect list in order, every effect's values after its update, the camera as it stands now): what
+	// a chain's cosmetic stage takes for the frame's last pass (rfx.chainSetEffects / rfx.aoChainSetEffects, InProcessGroup.setEffects)
+	params(renderer, inputBuffer, deltaTime) {
+		const p = { cam: cameraBlock(this.camera), count: this.effects.length, effects: this.effects.map(e => e.fxId) }
+		for (const e of this.effects) { e.update(renderer, inputBuffer, deltaTime); e.fill(p) }
+		return p
 	}
 	dispose() { if (this.planes) for (const pl of Object.values(this.planes)) rfx.planeFree(this.ctx, pl); this.planes = null }
 }
@@ -654,6 +660,8 @@ export class InProcessGroup {
 		rfx.groupAttachChainsInprocess(this.ctxs[0], this.groups, this.chains)
 	}
 	setBounds(bounds) { this.groups.forEach((g, r) => rfx.groupSetBounds(this.ctxs[r], g, bounds)) }
+	// the cosmetic stage of every member's TRAA tail (RfxEffectPass.params(...), or null to turn it off), before any frame; every member gets the same values
+	setEffects(params) { this.chains.forEach((ch, r) => rfx.chainSetEffects(this.ctxs[r], ch, params)) }
 	// planes[r]: { depth, gbuffer, velocity, directLight } device planes on device r (full frames); all members finish before the next frame starts
 	render(cam, planes, cameraPos, moved) {
 		this.chains.forEach((ch, r) => rfx.chainRenderSharded(this.ctxs[r], ch, cam, planes[r].depth, planes[r].gbuffer, planes[r].velocity, planes[r].directLight, cameraPos, moved))

@@ -500,23 +500,43 @@ napi_value ChainRenderSharded(napi_env env, napi_callback_info info) {  // chain
   return undefined(env);
 }
 
-napi_value Effects(napi_env env, napi_callback_info info) {  // effects(ctx, {cam, effects: [ids], sharpness, alphax, alphay, aberration, backgroundColor, maxDistance, spread, intensity, sparklePerspective}, input, depth|null, velocity|null, out)
-  ARGS(6); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
-  Obj b{env, argv[1]};
-  rfx_effects_params p{};
-  if (!read_camera(env, b.get("cam"), &p.cam)) { napi_throw_type_error(env, nullptr, "effects: cam"); return nullptr; }
+// {cam, effects: [ids], count, sharpness, alphax, alphay, aberration, backgroundColor, maxDistance, spread, intensity, sparklePerspective}
+static bool effects_params(napi_env env, napi_value v, rfx_effects_params* p) {
+  Obj b{env, v};
+  *p = rfx_effects_params{};
+  if (!read_camera(env, b.get("cam"), &p->cam)) return false;
   float ids[4] = {0, 0, 0, 0};
-  p.n_effects = (int32_t)b.num("count", 1);
+  p->n_effects = (int32_t)b.num("count", 1);
   b.floats("effects", ids, 4);
-  for (int i = 0; i < 4; i++) p.effects[i] = (int32_t)ids[i];
-  p.sharpness = (float)b.num("sharpness", 1); p.alphax = (float)b.num("alphax", -0.05); p.alphay = (float)b.num("alphay", -0.05); p.aberration = (float)b.num("aberration", 1);
-  b.floats("backgroundColor", p.background_color, 3);
-  p.max_distance = (float)b.num("maxDistance", 5); p.spread = (float)b.num("spread", 1); p.intensity = (float)b.num("intensity", 1);
-  p.sparkle_perspective = (int32_t)b.num("sparklePerspective", 0);
+  for (int i = 0; i < 4; i++) p->effects[i] = (int32_t)ids[i];
+  p->sharpness = (float)b.num("sharpness", 1); p->alphax = (float)b.num("alphax", -0.05); p->alphay = (float)b.num("alphay", -0.05); p->aberration = (float)b.num("aberration", 1);
+  b.floats("backgroundColor", p->background_color, 3);
+  p->max_distance = (float)b.num("maxDistance", 5); p->spread = (float)b.num("spread", 1); p->intensity = (float)b.num("intensity", 1);
+  p->sparkle_perspective = (int32_t)b.num("sparklePerspective", 0);
+  return true;
+}
+napi_value Effects(napi_env env, napi_callback_info info) {  // effects(ctx, params (effects_params), input, depth|null, velocity|null, out)
+  ARGS(6); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
+  rfx_effects_params p{};
+  if (!effects_params(env, argv[1], &p)) { napi_throw_type_error(env, nullptr, "effects: cam"); return nullptr; }
   CHECK(c, rfx_effects_launch(c, nullptr, &p, unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]), unwrap<rfx_plane>(env, argv[4]), unwrap<rfx_plane>(env, argv[5]), 0, 0),
         "rfx_effects_launch");
   return undefined(env);
 }
+// chainSetEffects(ctx, chain, params | null) / aoChainSetEffects(ctx, aoChain, params | null): the cosmetic stage of the chain's TRAA tail with
+// this frame's values (effects_params; what RfxEffectPass.params returns), or null to turn it off
+template <class Chain>
+static napi_value set_effects(napi_env env, napi_callback_info info, rfx_status (*fn)(Chain*, const rfx_effects_params*), const char* name) {
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  napi_valuetype t = napi_undefined;
+  napi_typeof(env, argv[2], &t);
+  rfx_effects_params p{};
+  if (t == napi_object && !effects_params(env, argv[2], &p)) { napi_throw_type_error(env, nullptr, "set_effects: cam"); return nullptr; }
+  CHECK(ctx, fn(unwrap<Chain>(env, argv[1]), t == napi_object ? &p : nullptr), name);
+  return undefined(env);
+}
+napi_value ChainSetEffects(napi_env env, napi_callback_info info) { return set_effects(env, info, rfx_ssgi_chain_set_effects, "rfx_ssgi_chain_set_effects"); }
+napi_value AoChainSetEffects(napi_env env, napi_callback_info info) { return set_effects(env, info, rfx_ao_chain_set_effects, "rfx_ao_chain_set_effects"); }
 napi_value Taa(napi_env env, napi_callback_info info) {  // taa(ctx, {cameraNotMovedFrames, srgbOutput}, input, history|null, out)
   ARGS(5); rfx_ctx* c = unwrap<rfx_ctx>(env, argv[0]);
   Obj b{env, argv[1]};
@@ -548,7 +568,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("aoChainCreate", AoChainCreate), FN("aoChainDestroy", AoChainDestroy), FN("aoChainRenderHost", AoChainRenderHost), FN("aoChainSubmitHost", AoChainSubmitHost), FN("aoChainWaitHost", AoChainWaitHost),
       FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
       FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur), FN("traaMotionBlur", TraaMotionBlur), FN("chainSetMotionBlur", ChainSetMotionBlur),
-      FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("taa", Taa),
+      FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("chainSetEffects", ChainSetEffects), FN("aoChainSetEffects", AoChainSetEffects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),
       FN("groupDestroy", GroupDestroy), FN("chainRenderSharded", ChainRenderSharded),
   };

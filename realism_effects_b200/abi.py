@@ -278,6 +278,7 @@ def _sig(lib):
     lib.rfx_ssgi_chain_output.argtypes = [vp, C.c_int32, PP]
     lib.rfx_ssgi_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
     lib.rfx_ssgi_chain_set_motion_blur.argtypes = [vp, _P(MotionBlurParams)]
+    lib.rfx_ssgi_chain_set_effects.argtypes = [vp, _P(EffectsParams)]
     lib.rfx_ssgi_chain_render_sharded_finish.argtypes = [vp, vp]
     lib.rfx_ao_chain_render_sharded_finish.argtypes = [vp, vp]
     lib.rfx_ssgi_chain_render_host.argtypes = [vp, _P(SsgiHostFrame)]
@@ -318,6 +319,8 @@ def _sig(lib):
     lib.rfx_ao_chain_output.argtypes = [vp, C.c_int32, PP]
     lib.rfx_ao_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
     lib.rfx_ao_chain_set_motion_blur.argtypes = [vp, _P(MotionBlurParams)]
+    lib.rfx_ao_chain_set_effects.argtypes = [vp, _P(EffectsParams)]
+    lib.rfx_fx_stage_rows.argtypes = [u32, u32, _P(EffectsParams), u32, u32, _P(u32)]
     lib.rfx_ao_chain_render_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
     lib.rfx_ao_chain_render_sharded_traa.argtypes = [vp, vp, _P(AoFrame), _P(AoTraaFrame)]
     lib.rfx_group_attach_ao_chain.argtypes = [vp, vp]
@@ -348,6 +351,7 @@ EXPORTS = [
     "rfx_ao_chain_enable_traa", "rfx_ao_chain_render_traa", "rfx_ao_chain_render_sharded_traa",
     "rfx_traa_motion_blur_launch", "rfx_ssgi_chain_set_motion_blur", "rfx_ao_chain_set_motion_blur",
     "rfx_ssgi_chain_render_sharded_finish", "rfx_ao_chain_render_sharded_finish",
+    "rfx_ssgi_chain_set_effects", "rfx_ao_chain_set_effects", "rfx_fx_stage_rows",
     "rfx_ao_chain_render_host", "rfx_ao_chain_submit_host", "rfx_ao_chain_wait_host",
 ]
 

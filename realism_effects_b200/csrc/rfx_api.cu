@@ -984,7 +984,14 @@ struct TraaTail {
   bool split = false;
   bool pending = false;
   rfx_plane p2_velocity{}, p2_out{};  // what phase 2 launches on: the frame's velocity plane and output
-  int p2_r0 = 0, p2_r1 = 0;           // ... and the band
+  int p2_r0 = 0, p2_r1 = 0;           // ... and the rows (the band, or with the cosmetic stage on its input rows)
+  // The cosmetic stage (rfx_*_chain_set_effects): one effects launch over the tail's image after the tail's last pass.  `fx_plane` is the
+  // SSGI chain's stage output (output 6) and the AO chain's stage input (the tail writes it instead of frame->output).  `fx_job` is this
+  // frame's launch, set by the chain before its tail and run by tail_end (in phase 2 of a split frame).
+  bool fx = false;
+  rfx_effects_params fx_p{};
+  rfx_plane fx_plane{};
+  struct { rfx_plane in, depth, velocity, out; int r0, r1; } fx_job{};
   uint64_t frames = 0;  // tails rendered; acc.buf[frames & 1] is written next
   float keep = 0.0f;    // keepData of the TRAA pass
   int cur() const { return (int)(frames & 1); }
@@ -1099,7 +1106,7 @@ static std::array<HistPlane*, 9> every_hist_plane(rfx_ssgi_chain* ch) {  // whet
 static int pass_latest(const GroupMember* ch);
 
 static void traa_free(rfx_ctx* ctx, TraaTail& t) {
-  for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid.buf[0], &t.mid.buf[1]}) if (p->ptr) rfx_plane_free(ctx, p);
+  for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid.buf[0], &t.mid.buf[1], &t.fx_plane}) if (p->ptr) rfx_plane_free(ctx, p);
 }
 // rfx_*_chain_enable_traa once the chain kind's own checks passed: NULL frees the tail's planes.  Otherwise the planes are allocated on
 // first use (`out` and `mid` where the chain asks for them; nothing is left allocated on failure), and the options replace the old ones.
@@ -1108,7 +1115,8 @@ static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_opt
     CU(cudaStreamSynchronize(ctx->stream));
     traa_free(ctx, t);
     t.on = false;
-    t.blur = false;  // the stage ends the tail: it goes with it
+    t.blur = false;  // the stages end the tail: they go with it
+    t.fx = false;
     return RFX_OK;
   }
   if (!t.acc.buf[0].ptr) {
@@ -1139,6 +1147,44 @@ static rfx_status traa_set_blur(rfx_ctx* ctx, TraaTail& t, const rfx_motion_blur
   t.blur = p != nullptr;
   if (p) t.blur_p = *p;
   return RFX_OK;
+}
+// The checks of an effects list shared by rfx_effects_launch's callers on the host (rfx_*_chain_set_effects, rfx_fx_stage_rows).
+static bool fx_list_ok(const rfx_effects_params* p) {
+  if (!p || p->n_effects < 1 || p->n_effects > 4) return false;
+  for (int i = 0; i < p->n_effects; i++)
+    if (p->effects[i] < RFX_FX_SHARPNESS || p->effects[i] > RFX_FX_SPARKLE) return false;
+  return true;
+}
+// rfx_*_chain_set_effects: the stage needs the tail; turning it on allocates its plane, turning it off frees it.  It keeps nothing across
+// frames and no peer reads it, so a chain in a group may change it between frames, but not between the two phases of a split frame.
+static rfx_status traa_set_fx(rfx_ctx* ctx, TraaTail& t, const rfx_effects_params* p, uint32_t W, uint32_t H) {
+  if (!t.on) return fail(ctx, RFX_ERR_NOT_READY, "set_effects: the cosmetic stage runs over the TRAA tail's image, and the tail is off");
+  if (t.pending) return fail(ctx, RFX_ERR_NOT_READY, "set_effects: the last row-sharded frame waits for its second phase (render_sharded_finish)");
+  if (p && !fx_list_ok(p)) return fail(ctx, RFX_ERR_INVALID_ARG, "set_effects: n_effects must be 1..4 and every effect an RFX_FX_* id");
+  if (!p) {
+    if (t.fx_plane.ptr) {
+      CU(cudaStreamSynchronize(ctx->stream));
+      rfx_plane_free(ctx, &t.fx_plane);
+      t.fx_plane = rfx_plane{};
+    }
+    t.fx = false;
+    return RFX_OK;
+  }
+  if (!t.fx_plane.ptr) {
+    rfx_status st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, &t.fx_plane);
+    if (st != RFX_OK) return st;
+  }
+  t.fx_p = *p;
+  t.fx = true;
+  return RFX_OK;
+}
+// The end of a frame's tail, after its last pass (K9, the fused tail or the merged TRAA + motion-blur pass): the cosmetic stage's launch
+// when it is on.  The tail advances first: its TRAA planes are complete whatever the stage returns.
+static rfx_status tail_end(rfx_ctx* ctx, void* stream, TraaTail& t) {
+  t.advance();
+  if (!t.fx) return RFX_OK;
+  const auto& j = t.fx_job;
+  return rfx_effects_launch(ctx, stream, &t.fx_p, &j.in, &j.depth, &j.velocity, &j.out, (uint32_t)j.r0, (uint32_t)j.r1);
 }
 
 static cudaEvent_t chain_event(rfx_ssgi_chain* ch) {
@@ -1272,6 +1318,11 @@ rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* ch, const rfx_motion_b
   return traa_set_blur(ch->ctx, ch->tail, p, ch->group != nullptr, ch->opt.width, ch->opt.height);
 }
 
+rfx_status rfx_ssgi_chain_set_effects(rfx_ssgi_chain* ch, const rfx_effects_params* p) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  return traa_set_fx(ch->ctx, ch->tail, p, ch->opt.width, ch->opt.height);
+}
+
 }  // extern "C"
 // fast chain: tr[]/dnB[] buffer 0 := the reference-format views of the interleaved planes, dn from fdnB.buf[parity]
 static rfx_status split_views(rfx_ssgi_chain* ch, int parity, cudaStream_t s) {
@@ -1296,10 +1347,12 @@ extern "C" {
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
-  if (which < 0 || which > 7) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..7");
+  if (which < 0 || which > 8) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..8");
   if (which >= 6) {
-    if (!ch->tail.on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
-    *out = which == 6 ? ch->tail.out : ch->tail.latest();
+    if (!ch->tail.on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 / 8 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
+    if (which == 8 && !ch->tail.fx) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: output 8 needs the cosmetic stage (rfx_ssgi_chain_set_effects)");
+    // with the cosmetic stage on, output 6 is its image and 8 the tail's image it reads
+    *out = which == 7 ? ch->tail.latest() : which == 6 && ch->tail.fx ? ch->tail.fx_plane : ch->tail.out;
     return RFX_OK;
   }
   if (ch->fastpath) {
@@ -1443,8 +1496,8 @@ static rfx_temporal_params traa_params(const TraaTail& t, const rfx_temporal_par
 // K2 in its TRAA form over the tail's `mid` on the output rows kr +- 1 (K9's LINEAR fetch) into buffer cur() of the accumulated plane,
 // reading last frame's other buffer (in a row-sharded group of n > 1, `peer`: on the rank that owns each row), then K9 from it into `out`
 // on kr, or with the motion-blur stage on the merged TRAA + motion-blur pass, whose taps read all of `mid`.  `mid` must hold rows
-// kr +- RFX_TRAA_TAIL_ROWS (with the stage alone: every row).  Then the tail advances.  With a split frame (t.split) the merged pass and
-// the advance wait for phase 2 (traa_blur_finish): this returns with t.pending set.
+// kr +- RFX_TRAA_TAIL_ROWS (with the stage alone: every row).  Then the tail ends (tail_end: the cosmetic stage, the advance).  With a
+// split frame (t.split) the merged pass and the tail's end wait for phase 2 (traa_blur_finish): this returns with t.pending set.
 static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_params& tp, TraaTail& t, const rfx_plane* velocity, bool peer,
                                 const rfx_plane* out, Rows kr) {
   const int cur = t.cur(), H = (int)t.acc.buf[cur].height;
@@ -1460,8 +1513,7 @@ static rfx_status traa_launches(rfx_ctx* ctx, void* stream, const rfx_temporal_p
   }
   if (t.blur) st = traa_motion_blur(ctx, stream, &t.blur_p, velocity, &t.acc.buf[cur], &t.mid_w(), out, (uint32_t)kr.r0, (uint32_t)kr.r1, nullptr);
   else st = rfx_traa_compose_launch(ctx, stream, &t.acc.buf[cur], out, (uint32_t)kr.r0, (uint32_t)kr.r1);
-  if (st == RFX_OK) t.advance();
-  return st;
+  return st != RFX_OK ? st : tail_end(ctx, stream, t);
 }
 // Phase 2 of a split frame, after the frame's barrier: the merged pass on the band, its taps reading this frame's `mid` through `mid_view`
 // (each row on its owner, or the local plane once the rows were replicated), then the tail advances.
@@ -1471,8 +1523,7 @@ static rfx_status traa_blur_finish(rfx_ctx* ctx, void* stream, TraaTail& t, cons
                                    mid_view.n > 1 ? &mid_view : nullptr);
   if (st != RFX_OK) return st;
   t.pending = false;
-  t.advance();
-  return RFX_OK;
+  return tail_end(ctx, stream, t);
 }
 
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
@@ -1485,6 +1536,10 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
   TraaTail& tail = ch->tail;
   const rfx_temporal_params tp = traa_params(tail, ch->traa_tp, f->camera_moved);
   const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
+  if (tail.fx) {  // the cosmetic stage: K9's plane into the stage's plane on launch k + 1's rows (the band; the tail runs on the rows it reads)
+    const Rows fr = launch_rows(ranges, k + 1, H);
+    tail.fx_job = {tail.out, *f->depth, *f->velocity, tail.fx_plane, fr.r0, fr.r1};
+  }
   // the fused kernel never writes the K5 plane, and the motion-blur stage samples all of it: with the stage on, the per-pass launches
   // (which also measured faster than the fused tail at 4K, DESIGN.md §4)
   if (ch->fastpath && !debug && !tail.blur) {
@@ -1522,10 +1577,9 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
     // the TRAA history rows live on their owners in a group of n > 1: the per-pass chain's peer forms, and the fast chain's tail when the
     // motion-blur stage takes it off its fused kernel (which reads the history through the views itself)
     if (st == RFX_OK) st = traa_launches(ctx, stream, tp, tail, f->velocity, ch->group_peer || tail.split, &tail.out, kr);
-    return st;  // the per-pass tail advances in traa_launches
+    return st;  // the per-pass tail ends in traa_launches
   }
-  tail.advance();
-  return RFX_OK;
+  return tail_end(ctx, stream, tail);
 }
 
 // 2-D TMA descriptor over a plane of 16-byte texels, addressed as rows of 4-byte elements (the box must pass cpoisson_tma_fits)
@@ -1995,13 +2049,23 @@ rfx_status rfx_ao_chain_set_motion_blur(rfx_ao_chain* ch, const rfx_motion_blur_
   return traa_set_blur(ch->ctx, ch->tail, p, ch->group && rfx_group_world(ch->group) > 1, ch->opt.width, ch->opt.height);
 }
 
+rfx_status rfx_ao_chain_set_effects(rfx_ao_chain* ch, const rfx_effects_params* p) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  return traa_set_fx(ch->ctx, ch->tail, p, ch->opt.width, ch->opt.height);
+}
+
 rfx_status rfx_ao_chain_output(rfx_ao_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
   if (ch->tail.on && (which == 2 || which == 3)) {
     *out = which == 2 ? ch->tail.mid_latest() : ch->tail.latest();
     return RFX_OK;
   }
-  if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1 (2 / 3 with the TRAA tail on)");
+  if (which == 4) {
+    if (!ch->tail.fx) return fail(ch->ctx, RFX_ERR_NOT_READY, "ao_chain_output: output 4 needs the cosmetic stage (rfx_ao_chain_set_effects)");
+    *out = ch->tail.fx_plane;
+    return RFX_OK;
+  }
+  if (which < 0 || which > 1) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "ao_chain_output: which must be 0 or 1 (2 / 3 with the TRAA tail on, 4 with the cosmetic stage)");
   const HistPlane& h = which == 1 && ch->opt.iterations > 0 ? ch->dnB : ch->target;  // AOEffect's `texture`
   *out = h.buf[h.buf[1].ptr ? pass_latest(ch) : 0];
   return RFX_OK;
@@ -2091,15 +2155,22 @@ static rfx_status ao_render_impl(rfx_ao_chain* ch, void* stream, const rfx_ao_fr
     if (st != RFX_OK) return st;
   }
   k++;
-  // ---- the TRAA tail: TRAAEffect's temporal pass over the K7 plane, then K9 into frame->output
+  // ---- the TRAA tail: TRAAEffect's temporal pass over the K7 plane, then K9 into frame->output (with the cosmetic stage on: K9 into the
+  // stage's plane, then the stage into frame->output on launch k + 1's rows, the band)
   if (t) {
+    const rfx_plane* tail_out = f->output;
+    if (ch->tail.fx) {
+      const Rows fr = launch_rows(ranges, k + 1, (int)o.height);
+      ch->tail.fx_job = {ch->tail.fx_plane, *f->depth, *f->velocity, *f->output, fr.r0, fr.r1};
+      tail_out = &ch->tail.fx_plane;
+    }
     rfx_temporal_params cam{};
     const rfx_ao_traa_frame& prev = ch->traa_have_prev ? ch->traa_prev : *t;  // TemporalReprojectPass.js:94-97 on the first frame
     cam.cam = t->cam;
     memcpy(cam.prev_view_matrix, prev.cam.view_matrix, 64); memcpy(cam.prev_camera_matrix_world, prev.cam.camera_matrix_world, 64);
     memcpy(cam.prev_projection, prev.cam.projection, 64); memcpy(cam.prev_projection_inverse, prev.cam.projection_inverse, 64);
     memcpy(cam.camera_pos, t->camera_pos, 12); memcpy(cam.prev_camera_pos, prev.camera_pos, 12);
-    st = traa_launches(ctx, stream, traa_params(ch->tail, cam, t->camera_moved), ch->tail, f->velocity, ch->group_peer, f->output,
+    st = traa_launches(ctx, stream, traa_params(ch->tail, cam, t->camera_moved), ch->tail, f->velocity, ch->group_peer, tail_out,
                        launch_rows(ranges, k, (int)o.height));
     if (st != RFX_OK) return st;
     ch->traa_prev = *t;

@@ -835,16 +835,24 @@ class EffectPass:
             p = mb.params(inputBuffer, 1 / 60 if deltaTime is None else deltaTime, window)
             ctx.traa_motion_blur(p, mb.velocityPass.texture, traa.temporalReprojectPass.accumulated, inputBuffer, outputBuffer)
             return
-        p = abi.make_effects_params(self._camera.uniforms(), [e.fx_id for e in self.effects])
+        p = self.params(renderer, inputBuffer, deltaTime)
         depth = velocity = None
         for e in self.effects:
-            e.update(renderer, inputBuffer, deltaTime)
-            e._fill(p)
             if isinstance(e, GradualBackgroundEffect):
                 depth = e.depthTexture
             if isinstance(e, SparkleEffect):
                 velocity = e.velocityDepthNormalPass.texture
         ctx.effects(p, inputBuffer, depth, velocity, outputBuffer)
+
+    def params(self, renderer=None, inputBuffer=None, deltaTime=None) -> abi.EffectsParams:
+        """The rfx_effects_params this pass launches with for the cosmetic effects: the effect list in order, every effect's values after its
+        update, and the camera's uniforms as they stand now.  A chain's cosmetic stage takes the same values for the frame's last pass
+        (engine.SsgiChain.set_effects / AoChain.set_effects); it reads the frame's own depth and velocity planes."""
+        p = abi.make_effects_params(self._camera.uniforms(), [e.fx_id for e in self.effects])
+        for e in self.effects:
+            e.update(renderer, inputBuffer, deltaTime)
+            e._fill(p)
+        return p
 
 
 class TAAPass:

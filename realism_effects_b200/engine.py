@@ -281,6 +281,12 @@ class _Chain:
         (frame, delta_time change); None turns the stage off."""
         self.ctx._chk(self._fn("set_motion_blur")(self.h, C.byref(params) if params is not None else None))
 
+    def set_effects(self, params: "abi.EffectsParams | None"):
+        """Cosmetic stage of the TRAA tail (include/rfx.h: rfx_<kind>_chain_set_effects): `EffectPass(camera, ...cosmetic effects)` over the
+        tail's image as the frame's last pass, one launch of the merged effects.  params: what that EffectPass launches with
+        (effects.EffectPass.params()), camera included, passed before every frame; None turns the stage off."""
+        self.ctx._chk(self._fn("set_effects")(self.h, C.byref(params) if params is not None else None))
+
     def output(self, which: int | None = None) -> Plane:
         """chain output `which` (the class docstring lists them; default: _DEFAULT_OUTPUT)"""
         p = Plane()
@@ -300,7 +306,7 @@ class _Chain:
 class SsgiChain(_Chain):
     """Native SSGI chain (rfx_ssgi_chain): K1 -> K2 -> K3 x 2*iterations -> K4 with history, and optionally the TRAA frame tail (K5 ->
     TRAA -> K9 after K4).  Outputs: 0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA
-    accumulated plane."""
+    accumulated plane; with the cosmetic stage on (set_effects), 6 is the stage's image and 8 the K9 output it reads."""
 
     _PREFIX = "rfx_ssgi_chain"
 
@@ -378,7 +384,8 @@ class AoChain(_Chain):
     """Native AO chain (rfx_ao_chain): K6 or K6h -> K3 x 2*iterations -> K7 in one call, the launches of HBAOEffect.update /
     HorizonAOEffect.update, and optionally the TRAA frame tail (K7 -> TRAA -> K9): render() then takes the TRAA camera and writes the K9
     frame to `out`.  Options: ao_chain_options(...).  Outputs: 0 the AO target, 1 the denoised plane K7 composes (the AO target with
-    iterations 0); with the TRAA tail on, 2 the K7 plane and 3 the TRAA accumulated plane."""
+    iterations 0); with the TRAA tail on, 2 the K7 plane and 3 the TRAA accumulated plane; with the cosmetic stage on (set_effects), 4 the
+    tail's image the stage reads (the stage writes `out`)."""
 
     _PREFIX = "rfx_ao_chain"
     _DEFAULT_OUTPUT = 1

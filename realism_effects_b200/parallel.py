@@ -29,8 +29,11 @@ between frames and the result stays bit-identical to the single-GPU chain (tests
 """
 from __future__ import annotations
 
+import functools
 import math
 from dataclasses import dataclass
+
+import numpy as np
 
 
 def _poisson_halo(radius: float, height: int, width: int | None) -> int:
@@ -52,6 +55,62 @@ def _widen_back(own, height: int, reaches) -> list:
     return out[::-1]
 
 
+def _with_stage(own, stage_rows, height: int, reaches) -> list:
+    """_widen_back for the band `own`; with the cosmetic stage (stage_rows not None) the launches are planned for stage_rows as if they were
+    the band, and the stage runs on the band as one more launch (mirror of shard_ranges in csrc/rfx_group.inl)"""
+    if stage_rows is None:
+        return _widen_back(own, height, reaches)
+    return _widen_back(tuple(stage_rows), height, reaches) + [tuple(own)]
+
+
+@functools.lru_cache(maxsize=4)
+def _lens_rows(width: int, height: int, alphax, alphay, aberration):
+    f = np.float32
+    one, two, half = f(1.0), f(2.0), f(0.5)
+    W, H = f(width), f(height)
+    ax, ay, ab = f(alphax), f(alphay), f(aberration)
+    with np.errstate(all="ignore"):
+        Y = (two * ((np.arange(height, dtype=f) + half) / H) - one)[:, None]
+        X = (two * ((np.arange(width, dtype=f) + half) / W) - one)[None, :]
+        r = X * X + Y * Y
+        x3, y3 = X / (one - ax * r), Y / (one - ay * r)
+        q = x3 * x3 + y3 * y3
+        y2 = Y / (one - ay * q)
+        dv = (y2 + one) * one / two
+        lo = np.full(height, height, dtype=np.int64)
+        hi = np.full(height, -1, dtype=np.int64)
+        for d in (ab * f(0.0), ab * (one / H)):  # the v offsets of the taps: aberration * (ox, 0), aberration * (0, oy) and (ox, oy)
+            fy = (dv - d) * H - half
+            every = ~(np.abs(fy) < f(1.0e9))  # not finite, or beyond the kernel's saturating integer conversion: every row
+            iy = np.floor(np.where(every, f(0.0), fy)).astype(np.int64)
+            lo = np.minimum(lo, np.where(every, 0, np.clip(iy, 0, height - 1)).min(axis=1))
+            hi = np.maximum(hi, np.where(every, height - 1, np.clip(iy + 1, 0, height - 1)).max(axis=1))
+    return lo, hi
+
+
+def lens_rows(width: int, height: int, alphax: float, alphay: float, aberration: float):
+    """LensDistortion's rows (mirror of lens_rows in csrc/rfx_group.inl): numpy arrays lo, hi with the lowest and highest input rows the
+    three taps of output row y touch.  fx_lens's uv arithmetic (csrc/k_fx.cu) in numpy float32 (IEEE, no contraction), then the bilinear
+    footprint rows floor(v * H - 0.5) and the one after, clamped to the frame; a coordinate that is not finite or beyond |1e9| rows: every
+    row.  Kept for the last few (size, alphax, alphay, aberration)."""
+    return _lens_rows(int(width), int(height), float(np.float32(alphax)), float(np.float32(alphay)), float(np.float32(aberration)))
+
+
+def fx_stage_rows(width: int, height: int, own, effects, alphax: float = -0.05, alphay: float = -0.05, aberration: float = 1.0) -> tuple:
+    """Rows [a, b) of the tail's image the cosmetic stage reads for its output band `own` (mirror of rfx_fx_stage_rows): the band +- 1 row
+    for every pixel's LINEAR fetch at its centre, +- 2 with Sharpness (its 3x3 LINEAR taps), and with LensDistortion every row lens_rows
+    gives for the band's rows.  effects: RFX_FX_* ids (abi.FX_*); GradualBackground and Sparkle read nothing more."""
+    from . import abi
+
+    own0, own1 = int(own[0]), int(own[1])
+    reach = 2 if abi.FX_SHARPNESS in effects else 1
+    a, b = max(0, own0 - reach), min(height, own1 + reach)
+    if abi.FX_LENS_DISTORTION in effects:
+        lo, hi = lens_rows(width, height, alphax, alphay, aberration)
+        a, b = min(a, int(lo[own0:own1].min())), max(b, int(hi[own0:own1].max()) + 1)
+    return a, b
+
+
 @dataclass
 class ShardPlan:
     """Row ranges [a, b) per launch of one SSGI chain frame for the contiguous band this rank owns, in chain order: K1, K2, K3 pass 0..n-1,
@@ -67,6 +126,8 @@ class ShardPlan:
     width: int | None = None     # frame width: portrait frames (H > W) stretch the Poisson taps' row reach by H / W
     traa: bool = False           # the TRAA tail runs as one more launch after K4 (rfx_ssgi_chain_enable_traa)
     denoise_mode: int = 0        # 0 "full"; 1 "full_temporal" / 2 "temporal" run no Poisson pass, so their ranges are those of 0 passes
+    stage_rows: tuple | None = None  # the cosmetic stage (rfx_ssgi_chain_set_effects) runs on the band as one more launch after the tail,
+                                     # and the chain is planned for the rows it reads (fx_stage_rows) as if they were the band
 
     K2_NEIGHBOURHOOD_ROWS = 2  # 5x5 clamp window (reproject.frag:57-59)
     K4_INPUT_ROWS = 1          # literal bilinear fetch of the LINEAR Poisson targets at the pixel centre
@@ -95,7 +156,7 @@ class ShardPlan:
 
     @property
     def n_launches(self) -> int:
-        return 3 + self.passes + (1 if self.traa else 0)
+        return 3 + self.passes + (1 if self.traa else 0) + (1 if self.stage_rows is not None else 0)
 
     @property
     def ranges(self) -> list:
@@ -103,7 +164,7 @@ class ShardPlan:
         # K2 reads K1's output in its 5x5 window, every Poisson pass the previous target through its taps, K4 the last Poisson target at
         # the pixel centre (nothing without a pass) and the tail `composed`.  K4 runs in both modes (SSR composes with inputType specular)
         reaches = [self.K2_NEIGHBOURHOOD_ROWS] + [self.poisson_halo] * n + [self.K4_INPUT_ROWS if n else 0]
-        return _widen_back((self.r0, self.r1), self.height, reaches + ([self.TRAA_TAIL_ROWS] if self.traa else []))
+        return _with_stage((self.r0, self.r1), self.stage_rows, self.height, reaches + ([self.TRAA_TAIL_ROWS] if self.traa else []))
 
     @property
     def local_input_rows(self) -> tuple:
@@ -128,6 +189,7 @@ class AoShardPlan:
     iterations: int
     radius: float
     traa: bool = False  # the TRAA tail runs as one more launch after K7 (rfx_ao_chain_enable_traa)
+    stage_rows: tuple | None = None  # the cosmetic stage's input rows (fx_stage_rows), as ShardPlan.stage_rows
 
     K7_INPUT_ROWS = 1
 
@@ -137,12 +199,12 @@ class AoShardPlan:
 
     @property
     def n_launches(self) -> int:
-        return 2 + 2 * self.iterations + (1 if self.traa else 0)
+        return 2 + 2 * self.iterations + (1 if self.traa else 0) + (1 if self.stage_rows is not None else 0)
 
     @property
     def ranges(self) -> list:
         reaches = [self.poisson_halo] * (2 * self.iterations) + [self.K7_INPUT_ROWS] + ([ShardPlan.TRAA_TAIL_ROWS] if self.traa else [])
-        return _widen_back(tuple(self.own), self.height, reaches)
+        return _with_stage(tuple(self.own), self.stage_rows, self.height, reaches)
 
     @property
     def local_input_rows(self) -> tuple:
@@ -302,6 +364,11 @@ class ShardedSsgiChain:
     def set_motion_blur(self, params):
         """this frame's MotionBlurEffect uniforms (the same on every rank; the stage was turned on at construction)"""
         self.chain.set_motion_blur(params)
+
+    def set_effects(self, params):
+        """the cosmetic stage (engine.SsgiChain.set_effects) with this frame's values, or None to turn it off; the same on every rank, any
+        frame (the stage keeps no plane the group maps)"""
+        self.chain.set_effects(params)
 
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None):
         """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collectives.  Both
@@ -500,6 +567,11 @@ class InProcessGroup:
         """this frame's MotionBlurEffect uniforms for every member (the stage was turned on at construction)"""
         for ch in self.chains:
             ch.set_motion_blur(params)
+
+    def set_effects(self, params):
+        """the cosmetic stage with this frame's values for every member, or None to turn it off (any frame)"""
+        for ch in self.chains:
+            ch.set_effects(params)
 
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, wait: bool = True):
         """one frame: every member renders its band; all of them finish before the next frame starts (the host is the barrier).
