@@ -532,10 +532,25 @@ rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* chain, const rfx_motio
  * of it, so in a row-sharded group it may be turned on or off, and its values changed, between any two frames; every rank passes the same
  * p (rfx_fx_stage_rows, below, is what each rank recomputes around its band). */
 rfx_status rfx_ssgi_chain_set_effects(rfx_ssgi_chain* chain, const rfx_effects_params* p);
+/* Compose stage: the image SSGIEffect writes into the composer buffer, K5 ssgi_compose (ssgi_compose.frag:20-44) over output 0 (the
+ * denoiser's texture: `composed`, or tr[0] in denoiseMode "temporal"), frame->depth and frame->direct_light, as the frame's last launch.
+ * With p set, every frame ends with the stage, which writes a chain-owned RGBA16F plane: output 9.  p is used as rfx_traa_tail_options.compose
+ * is by the tail (fog; camera near / far / perspective for the fog depth).  The bytes are those of rfx_ssgi_compose_launch(p, depth,
+ * output 0, direct_light) after the frame.  The fast chain computes K5 in K4's epilogue (the last Poisson pass, or the stand-alone K4 with
+ * denoise_iterations 0) from the texel it composed, so the stage costs no launch; every other chain runs rfx_ssgi_compose_launch after
+ * the launch that writes output 0.  With a debug view selected (rfx_ssgi_chain_set_debug_view), the stage's K5 samples the view with
+ * isDebug, as the tail's K5 does, and the fast chain runs it as that per-pass launch.  p == NULL turns the stage off and frees its plane.
+ * p->is_debug != 0: RFX_ERR_INVALID_ARG (views are selected with rfx_ssgi_chain_set_debug_view).  The tail runs K5 itself, so the stage and
+ * the TRAA tail exclude each other: the stage with the tail on, and rfx_ssgi_chain_enable_traa(opt) with the stage on, are
+ * RFX_ERR_INVALID_ARG.  With the stage on, a frame without direct_light is RFX_ERR_INVALID_ARG.  K5 reads only its own pixel and the stage
+ * keeps no plane across frames, so in a row-sharded group it runs on the band (no wider rows, no peer reads) and may be turned on or off,
+ * and its values changed, between any two frames; every rank passes the same p. */
+rfx_status rfx_ssgi_chain_set_compose(rfx_ssgi_chain* chain, const rfx_ssgi_compose_params* p);
 /* which: 0 composed (RGBA32F), 1 ssgiOut, 2/3 trOut[0/1], 4/5 dnB[0/1]; with the TRAA tail on: 6 the tail's output (RGBA16F: K9's, or
  * with the motion-blur stage on the merged TRAA + motion-blur pass's; with the cosmetic stage on the stage's, the frame's final image), 7
  * the TRAA accumulated plane of the latest frame (RGBA16F; next frame's history); with the cosmetic stage on, 8 the stage's input (the
- * image output 6 holds with the stage off).  6 / 7 with the tail off, 8 with the stage off: RFX_ERR_NOT_READY. */
+ * image output 6 holds with the stage off); with the compose stage on, 9 its image (RGBA16F).  6 / 7 with the tail off, 8 with the
+ * cosmetic stage off: RFX_ERR_NOT_READY; 9 with the compose stage off: RFX_ERR_INVALID_ARG. */
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane* out);
 /* Debug view of the TRAA tail: SSGIEffect's `outputTexture` (src/ssgi/SSGIEffect.js:228-251, picked from the "Debug" list of
  * example/SSGIDebugGUI.js:78-114).  With a view selected, the tail's K5 runs with isDebug and samples the view instead of `composed`
@@ -556,8 +571,8 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane
 #define RFX_DEBUG_VIEW_GBUFFER 10
 #define RFX_DEBUG_VIEW_GBUFFER_CHANNEL 16
 rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* chain, int32_t view);
-/* host-buffer frame: uploads the four input planes from (pinned) host memory, renders,
- * downloads `composed` into out_host.  This is the call `bench.py`'s e2e leg times. */
+/* host-buffer frame: uploads the four input planes from (pinned) host memory, renders, downloads `composed` into out_composed and
+ * the frame's image into out_color.  This is the call `bench.py`'s e2e leg times (with out_composed). */
 typedef struct rfx_ssgi_host_frame {
   rfx_camera cam;
   const float* depth;             /* W*H      fp32 */
@@ -566,7 +581,9 @@ typedef struct rfx_ssgi_host_frame {
   const uint16_t* direct_light;   /* W*H*4    fp16, may be NULL */
   float camera_pos[3];
   int32_t camera_moved;
-  float* out_composed;            /* W*H*4    fp32 */
+  float* out_composed;            /* W*H*4    fp32; may be NULL when out_color is given (both NULL: RFX_ERR_INVALID_ARG) */
+  uint16_t* out_color;            /* W*H*4    fp16, the frame's image: output 9 with the compose stage on, output 6 with the TRAA tail on;
+                                     NULL: not downloaded; set with neither on: RFX_ERR_NOT_READY */
 } rfx_ssgi_host_frame;
 rfx_status rfx_ssgi_chain_render_host(rfx_ssgi_chain* chain, const rfx_ssgi_host_frame* frame);
 /* Pipelined form of the same path (what a per-frame caller such as EffectComposer.render would drive): submit enqueues the
@@ -575,7 +592,9 @@ rfx_status rfx_ssgi_chain_render_host(rfx_ssgi_chain* chain, const rfx_ssgi_host
  * wait_host blocks until at most max_in_flight (0 or 1) submitted frames are incomplete.  A frame's host input buffers and
  * out_composed must stay untouched until it is complete, so a caller alternates two host buffer sets:
  *     submit(frame i, set i&1);  wait_host(chain, 1);   // frame i-1 is complete, its set is free for frame i+1
- * render_host(f) == submit_host(f) + wait_host(chain, 0).  Results are bit-identical to rfx_ssgi_chain_render. */
+ * render_host(f) == submit_host(f) + wait_host(chain, 0).  Results are bit-identical to rfx_ssgi_chain_render.  Each downloaded
+ * plane is safe with two frames in flight: the fast chain double-buffers `composed` and output 9 by frame parity, and every other
+ * downloaded plane's writer (K4, the compose stage or the tail) waits for the previous frame's download. */
 rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* chain, const rfx_ssgi_host_frame* frame);
 rfx_status rfx_ssgi_chain_wait_host(rfx_ssgi_chain* chain, int32_t max_in_flight);
 

@@ -121,6 +121,13 @@ export const defaultSSGIOptions = {
 	importanceSampling: true, steps: 20, refineSteps: 5, resolutionScale: 1, missedRays: false, outputTexture: null
 }
 
+// K5's values (ssgi_compose.frag): the camera's near / far / projection and the scene's fog (SSGIEffect.js:404-412)
+function composeParams(camera, scene) {
+	const fog = scene?.fog
+	return { near: camera.near, far: camera.far, perspective: camera.isPerspectiveCamera !== false,
+		...(fog ? { fog: { color: fog.color.toArray(), near: fog.near, far: fog.far, density: fog.density, isFogExp2: !!fog.isFogExp2 } } : {}) }
+}
+
 export class SSGIEffect {
 	// new SSGIEffect(composer, scene, camera, options) — src/ssgi/SSGIEffect.js:31 (the code's signature, SURVEY.md D6)
 	constructor(composer, scene, camera, options = {}) {
@@ -215,11 +222,8 @@ export class SSGIEffect {
 			new Float32Array(this._camera.position.toArray()), moved)
 		if (this.gBufferDebugTarget) rfx.gbufferDebug(this.ctx, this._gBufferDebugMode, planes.gbuffer, this.gBufferDebugTarget)   // SSGIEffect.js:398-399
 		// K5: ssgi_compose.frag (mainImage of the effect); with isDebug the view itself, with its own sampler (:21-24)
-		const fog = this._scene.fog   // SSGIEffect.js:404-412
-		rfx.ssgiCompose(this.ctx, planes.depth, this._resolve(this.outputTexture, planes), planes.directLight, this.outputPlane, {
-			near: this._camera.near, far: this._camera.far, perspective: this._camera.isPerspectiveCamera !== false, isDebug: this.isDebug,
-			...(fog ? { fog: { color: fog.color.toArray(), near: fog.near, far: fog.far, density: fog.density, isFogExp2: !!fog.isFogExp2 } } : {})
-		})
+		rfx.ssgiCompose(this.ctx, planes.depth, this._resolve(this.outputTexture, planes), planes.directLight, this.outputPlane,
+			{ ...composeParams(this._camera, this._scene), isDebug: this.isDebug })
 		rfx.planeDownload(this.ctx, this.outputPlane, this.outputHost)
 	}
 	dispose() {
@@ -688,4 +692,35 @@ export class AOHostChain {
 	submitHost(camera, host) { rfx.aoChainSubmitHost(this.ctx, this.chain, this.frame(camera, host)) }
 	waitHost(maxInFlight = 0) { rfx.aoChainWaitHost(this.ctx, this.chain, maxInFlight) }
 	dispose() { rfx.aoChainDestroy(this.chain) }
+}
+
+// ---- the native SSGI chain from host buffers (rfx_ssgi_chain_render_host / _submit_host / _wait_host) -------------------------------------------
+// For hosts whose G-buffer, depth, velocity and colour live in host memory (no GL interop): the SSGI chain and its compose stage (K5 in the
+// chain's last launch, chain output 9: the image SSGIEffect writes into the composer buffer) on the GPU, with the uploads of frame i+1 and the
+// download of frame i-1 running under frame i's kernels.  options: SSGIEffect's keys plus width / height; scene: the three.js scene whose fog
+// K5 applies (or null).  host: { depth: Float32Array, gbuffer: Float32Array, velocity: Float32Array (VelocityDepthNormalPass layout),
+// directLight: Uint16Array RGBA16F (the composer input buffer), outColor: Uint16Array RGBA16F (the frame's image) | null,
+// outComposed: Float32Array (the denoiser's texture) | null }.
+export class SSGIHostChain {
+	constructor(options, scene = null, device = 0) {
+		this.ctx = context(device)
+		this.scene = scene
+		const o = { denoiseMode: "full", ...defaultSSGIOptions, ...options }
+		const denoiseModeId = ["full", "full_temporal", "temporal"].indexOf(o.denoiseMode)   // Denoiser.js:7
+		if (denoiseModeId < 0) throw new Error(`denoiseMode "${o.denoiseMode}" cannot run (in the reference "denoised" binds an array of textures to a sampler)`)
+		this.chain = rfx.chainCreate(this.ctx, { ...o, flags: FLAG.useDirectLight, mode: o.mode === "ssr" ? 1 : 0, denoiseModeId })
+		this.lastPos = null; this.lastQuat = null
+	}
+	_frame(camera, host, sync) {
+		const moved = didCameraMove(camera, this.lastPos, this.lastQuat)
+		this.lastPos = camera.position.clone(); this.lastQuat = camera.quaternion.clone()
+		rfx.chainSetCompose(this.ctx, this.chain, composeParams(camera, this.scene))   // the camera's and the fog's values as they stand now
+		rfx.chainRenderHost(this.ctx, this.chain, cameraBlock(camera), host.depth, host.gbuffer, host.velocity, host.directLight,
+			new Float32Array(camera.position.toArray()), moved, host.outComposed ?? null, sync, host.outColor ?? null)
+	}
+	renderHost(camera, host) { this._frame(camera, host, true) }
+	// pipelined: alternate two host sets; after submitHost(frame i) waitHost(1) returns once frame i-1 is complete and its set is free
+	submitHost(camera, host) { this._frame(camera, host, false) }
+	waitHost(maxInFlight = 0) { rfx.chainWaitHost(this.ctx, this.chain, maxInFlight) }
+	dispose() { rfx.chainDestroy(this.chain) }
 }

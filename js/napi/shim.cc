@@ -204,9 +204,10 @@ napi_value ChainOutput(napi_env env, napi_callback_info info) {  // chainOutput(
   return v;
 }
 // chainRenderHost(ctx, chain, camera, depth:Float32Array, gbuffer:Float32Array, velocity:Float32Array, direct:Uint16Array|null,
-//                 cameraPos:Float32Array(3), cameraMoved:boolean, out:Float32Array[, sync:boolean = true])
+//                 cameraPos:Float32Array(3), cameraMoved:boolean, out:Float32Array|null[, sync:boolean = true[, outColor:Uint16Array|null]])
+// out receives `composed`, outColor the frame's image (the compose stage's output 9, or the TRAA tail's output 6)
 napi_value ChainRenderHost(napi_env env, napi_callback_info info) {
-  ARGS(11); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  ARGS(12); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
   rfx_ssgi_chain* ch = unwrap<rfx_ssgi_chain>(env, argv[1]);
   rfx_ssgi_host_frame f{};
   if (!read_camera(env, argv[2], &f.cam)) { napi_throw_type_error(env, nullptr, "camera: expected Float32Array(16) matrices"); return nullptr; }
@@ -215,6 +216,7 @@ napi_value ChainRenderHost(napi_env env, napi_callback_info info) {
   read_f32(env, argv[7], f.camera_pos, 3);
   bool moved = true; napi_get_value_bool(env, argv[8], &moved); f.camera_moved = moved;
   f.out_composed = (float*)typed_ptr(env, argv[9]);
+  if (argc > 11) f.out_color = (uint16_t*)typed_ptr(env, argv[11]);
   // `sync` selects the synchronous call; otherwise the frame is only enqueued (pipelined H2D / kernels / D2H) and the caller
   // pairs it with chainWaitHost(ctx, chain, 1) - the typed arrays of a frame must stay alive and untouched until it completed.
   bool sync = true;
@@ -286,6 +288,15 @@ napi_value AoChainWaitHost(napi_env env, napi_callback_info info) {  // aoChainW
 }
 napi_value ChainReset(napi_env env, napi_callback_info info) { ARGS(1); rfx_ssgi_chain_reset(unwrap<rfx_ssgi_chain>(env, argv[0])); return undefined(env); }
 napi_value ChainDestroy(napi_env env, napi_callback_info info) { ARGS(1); rfx_ssgi_chain_destroy(unwrap<rfx_ssgi_chain>(env, argv[0])); return undefined(env); }
+// K5's uniforms from {fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug} (three's scene.fog and camera)
+void read_compose(napi_env env, Obj& b, rfx_ssgi_compose_params* p) {
+  p->camera_near = (float)b.num("near", 0.1); p->camera_far = (float)b.num("far", 1000); p->perspective = (int32_t)b.num("perspective", 1); p->is_debug = (int32_t)b.num("isDebug", 0);
+  if (b.has("fog")) {
+    Obj f{env, b.get("fog")};
+    p->use_fog = 1; p->fog_exp2 = (int32_t)f.num("isFogExp2", 0); f.floats("color", p->fog_color, 3);
+    p->fog_near = (float)f.num("near", 1); p->fog_far = (float)f.num("far", 1000); p->fog_density = (float)f.num("density", 0.00025);
+  }
+}
 // chainEnableTraa(ctx, chain, {maxBlend, neighborhoodClampIntensity, confidencePower, logTransform, fullAccumulate,
 //                              fog: {color, near, far, density, isFogExp2}, near, far, perspective, isDebug} | null)
 // null turns the TRAA tail off; the defaults are the values TRAAEffect forces
@@ -298,14 +309,22 @@ napi_value ChainEnableTraa(napi_env env, napi_callback_info info) {
   rfx_traa_tail_options o{};
   o.max_blend = (float)b.num("maxBlend", 0.9); o.neighborhood_clamp_intensity = (float)b.num("neighborhoodClampIntensity", 1);
   o.confidence_power = (float)b.num("confidencePower", 4); o.log_transform = (int32_t)b.num("logTransform", 1); o.full_accumulate = (int32_t)b.num("fullAccumulate", 0);
-  rfx_ssgi_compose_params& p = o.compose;
-  p.camera_near = (float)b.num("near", 0.1); p.camera_far = (float)b.num("far", 1000); p.perspective = (int32_t)b.num("perspective", 1); p.is_debug = (int32_t)b.num("isDebug", 0);
-  if (b.has("fog")) {
-    Obj f{env, b.get("fog")};
-    p.use_fog = 1; p.fog_exp2 = (int32_t)f.num("isFogExp2", 0); f.floats("color", p.fog_color, 3);
-    p.fog_near = (float)f.num("near", 1); p.fog_far = (float)f.num("far", 1000); p.fog_density = (float)f.num("density", 0.00025);
-  }
+  read_compose(env, b, &o.compose);
   CHECK(ctx, rfx_ssgi_chain_enable_traa(unwrap<rfx_ssgi_chain>(env, argv[1]), &o), "rfx_ssgi_chain_enable_traa");
+  return undefined(env);
+}
+// chainSetCompose(ctx, chain, {fog: {color, near, far, density, isFogExp2}, near, far, perspective} | null): the compose stage (output 9,
+// SSGIEffect's image); null turns it off
+napi_value ChainSetCompose(napi_env env, napi_callback_info info) {
+  ARGS(3); rfx_ctx* ctx = unwrap<rfx_ctx>(env, argv[0]);
+  napi_valuetype t = napi_undefined;
+  napi_typeof(env, argv[2], &t);
+  rfx_ssgi_compose_params p{};
+  if (t == napi_object) {
+    Obj b{env, argv[2]};
+    read_compose(env, b, &p);
+  }
+  CHECK(ctx, rfx_ssgi_chain_set_compose(unwrap<rfx_ssgi_chain>(env, argv[1]), t == napi_object ? &p : nullptr), "rfx_ssgi_chain_set_compose");
   return undefined(env);
 }
 
@@ -319,12 +338,7 @@ napi_value SsgiCompose(napi_env env, napi_callback_info info) {
   if (argc > 5) napi_typeof(env, argv[5], &t);
   if (t == napi_object) {
     Obj b{env, argv[5]};
-    p.camera_near = (float)b.num("near", 0.1); p.camera_far = (float)b.num("far", 1000); p.perspective = (int32_t)b.num("perspective", 1); p.is_debug = (int32_t)b.num("isDebug", 0);
-    if (b.has("fog")) {
-      Obj f{env, b.get("fog")};
-      p.use_fog = 1; p.fog_exp2 = (int32_t)f.num("isFogExp2", 0); f.floats("color", p.fog_color, 3);
-      p.fog_near = (float)f.num("near", 1); p.fog_far = (float)f.num("far", 1000); p.fog_density = (float)f.num("density", 0.00025);
-    }
+    read_compose(env, b, &p);
   }
   CHECK(c, rfx_ssgi_compose_launch(c, nullptr, t == napi_object ? &p : nullptr, unwrap<rfx_plane>(env, argv[1]), unwrap<rfx_plane>(env, argv[2]), unwrap<rfx_plane>(env, argv[3]),
                                    unwrap<rfx_plane>(env, argv[4]), 0, 0), "rfx_ssgi_compose_launch");
@@ -566,7 +580,7 @@ napi_value Init(napi_env env, napi_value exports) {
       FN("planeUpload", PlaneUpload), FN("planeDownload", PlaneDownload), FN("chainCreate", ChainCreate), FN("chainSetOptions", ChainSetOptions),
       FN("chainRender", ChainRender), FN("chainOutput", ChainOutput), FN("chainRenderHost", ChainRenderHost), FN("chainWaitHost", ChainWaitHost),
       FN("aoChainCreate", AoChainCreate), FN("aoChainDestroy", AoChainDestroy), FN("aoChainRenderHost", AoChainRenderHost), FN("aoChainSubmitHost", AoChainSubmitHost), FN("aoChainWaitHost", AoChainWaitHost),
-      FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
+      FN("chainReset", ChainReset), FN("chainDestroy", ChainDestroy), FN("chainEnableTraa", ChainEnableTraa), FN("chainSetCompose", ChainSetCompose), FN("ssgiCompose", SsgiCompose), FN("temporalReproject", TemporalReproject),
       FN("poissonDenoise", PoissonDenoise), FN("giCompose", GiCompose), FN("hbao", Hbao), FN("hbaoHorizon", HbaoHorizon), FN("aoCompose", AoCompose), FN("motionBlur", MotionBlur), FN("traaMotionBlur", TraaMotionBlur), FN("chainSetMotionBlur", ChainSetMotionBlur),
       FN("traaCompose", TraaCompose), FN("gbufferDebug", GbufferDebug), FN("chainSetDebugView", ChainSetDebugView), FN("gbufferIngest", GbufferIngest), FN("effects", Effects), FN("chainSetEffects", ChainSetEffects), FN("aoChainSetEffects", AoChainSetEffects), FN("taa", Taa),
       FN("groupCreateInprocess", GroupCreateInprocess), FN("groupAttachChainsInprocess", GroupAttachChainsInprocess), FN("groupSetBounds", GroupSetBounds),

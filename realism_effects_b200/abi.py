@@ -19,6 +19,8 @@ FMT_BYTES = {FMT_R32F: 4, FMT_RGBA32F: 16, FMT_RGBA16F: 8, FMT_RGBA8: 4}
 SSGI_IMPORTANCE_SAMPLING, SSGI_MISSED_RAYS, SSGI_USE_DIRECT_LIGHT, SSGI_USE_ENVMAP = 1, 2, 4, 8
 MODE_SSGI, MODE_SSR = 0, 1
 GROUP_ID_BYTES = 128
+ERR_INVALID_ARG = 1
+ERR_NOT_READY = 5
 ERR_UNSUPPORTED = 6
 ERR_NCCL = 7
 INPUT_DIFFUSE_SPECULAR, INPUT_DIFFUSE, INPUT_SPECULAR = 0, 1, 2
@@ -165,7 +167,7 @@ class SsgiFrame(C.Structure):
 
 class SsgiHostFrame(C.Structure):
     _fields_ = [("cam", CameraS), ("depth", C.c_void_p), ("gbuffer", C.c_void_p), ("velocity", C.c_void_p), ("direct_light", C.c_void_p),
-                ("camera_pos", F3), ("camera_moved", C.c_int32), ("out_composed", C.c_void_p)]
+                ("camera_pos", F3), ("camera_moved", C.c_int32), ("out_composed", C.c_void_p), ("out_color", C.c_void_p)]
 
 
 AO_HBAO, AO_HORIZON = 0, 1  # rfx_ao_chain_options.algorithm: K6 (HBAOEffect) or K6h (HorizonAOEffect)
@@ -279,6 +281,7 @@ def _sig(lib):
     lib.rfx_ssgi_chain_enable_traa.argtypes = [vp, _P(TraaTailOptions)]
     lib.rfx_ssgi_chain_set_motion_blur.argtypes = [vp, _P(MotionBlurParams)]
     lib.rfx_ssgi_chain_set_effects.argtypes = [vp, _P(EffectsParams)]
+    lib.rfx_ssgi_chain_set_compose.argtypes = [vp, _P(SsgiComposeParams)]
     lib.rfx_ssgi_chain_render_sharded_finish.argtypes = [vp, vp]
     lib.rfx_ao_chain_render_sharded_finish.argtypes = [vp, vp]
     lib.rfx_ssgi_chain_render_host.argtypes = [vp, _P(SsgiHostFrame)]
@@ -352,7 +355,7 @@ EXPORTS = [
     "rfx_traa_motion_blur_launch", "rfx_ssgi_chain_set_motion_blur", "rfx_ao_chain_set_motion_blur",
     "rfx_ssgi_chain_render_sharded_finish", "rfx_ao_chain_render_sharded_finish",
     "rfx_ssgi_chain_set_effects", "rfx_ao_chain_set_effects", "rfx_fx_stage_rows",
-    "rfx_ao_chain_render_host", "rfx_ao_chain_submit_host", "rfx_ao_chain_wait_host",
+    "rfx_ao_chain_render_host", "rfx_ao_chain_submit_host", "rfx_ao_chain_wait_host", "rfx_ssgi_chain_set_compose",
 ]
 
 

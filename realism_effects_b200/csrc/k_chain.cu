@@ -387,7 +387,7 @@ RFX_D f2 cp_lum2(f2 r, f2 g, f2 b) {  // luminance(): pow(dot(w, c), 0.125) on l
   return f2ex2(f2fma(f2lg2(d), mkf2(0.125f), mkf2(CP_LUM_C)));
 }
 
-template <bool FIRST, bool COMPOSE, bool INTERIOR, bool SMEM = false>
+template <bool FIRST, bool COMPOSE, bool IMAGE, bool INTERIOR, bool SMEM = false>
 RFX_D void cpoisson_body(const CPoissonArgs& a, int x, int y, float4 nc, float fwn, const SmemTile& st = SmemTile{}) {
   const v2 vUv = pixel_uv(x, y, a.W, a.H);
   const float depth = nc.w;
@@ -447,13 +447,20 @@ RFX_D void cpoisson_body(const CPoissonArgs& a, int x, int y, float4 nc, float f
   if (COMPOSE) {
     if (y >= a.crow0 && y < a.crow1) {  // K4 reads the fp16 texel just stored (DenoiserComposePass.js:66-67)
       const float4 g = ld_f4(a.gb, x, y);
-      st_f4(a.composed.p, a.composed.pitch, x, y,
-            c_compose(a.cam, x, y, a.W, a.H, g, roughness, depth, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
+      const float4 c = c_compose(a.cam, x, y, a.W, a.H, g, roughness, depth, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w)));
+      st_f4(a.composed.p, a.composed.pitch, x, y, c);
+      if (IMAGE) st_h4(a.k5.out.p, a.k5.out.pitch, x, y, ssgi_compose_lit(a.k5, x, y, depth, [&] { return c; }));  // K5 of the texel just stored
     }
   }
 }
 
-template <bool FIRST, bool COMPOSE>
+// K5 of a discarded (background: depth 1) pixel, which reads the scene texel only
+RFX_D v4 k5_background(const SsgiComposeArgs& k5, int x, int y) {
+  return ssgi_compose_lit(k5, x, y, 1.0f, [] { return make_float4(0.0f, 0.0f, 0.0f, 0.0f); });
+}
+
+// IMAGE (with COMPOSE): the composing pixels also store K5 of their composed texel into a.k5.out (the chain's compose stage)
+template <bool FIRST, bool COMPOSE, bool IMAGE = false>
 __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_constant__ CPoissonArgs a) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
@@ -473,6 +480,7 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_cons
       const unsigned off = (unsigned)y * (unsigned)a.composed_carry.local.pitch + (unsigned)x * 16u;
       st_f4(a.composed.p, a.composed.pitch, x, y, *((const float4*)(peer_row_base(a.composed_carry, y) + off)));
     }
+    if (IMAGE && y >= a.crow0 && y < a.crow1) st_h4(a.k5.out.p, a.k5.out.pitch, x, y, k5_background(a.k5, x, y));
     return;
   }
   // block-uniform: can any tap of this 16x16 tile leave the image?
@@ -480,14 +488,20 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_kernel(const __grid_cons
   lane_to_pixel(threadIdx.x & 31, lx, ly);
   const int bx0 = blockIdx.x * kTileW, by0 = y - ((int)((threadIdx.x >> 6) << 2) + ly);
   const bool interior = bx0 - a.reach_x >= 0 && bx0 + kTileW - 1 + a.reach_x <= a.W - 1 && by0 - a.reach_y >= 0 && by0 + kTileH - 1 + a.reach_y <= a.H - 1;
-  if (interior) cpoisson_body<FIRST, COMPOSE, true>(a, x, y, nc, fwn);
-  else cpoisson_body<FIRST, COMPOSE, false>(a, x, y, nc, fwn);
+  if (interior) cpoisson_body<FIRST, COMPOSE, IMAGE, true>(a, x, y, nc, fwn);
+  else cpoisson_body<FIRST, COMPOSE, IMAGE, false>(a, x, y, nc, fwn);
 }
 
+template <bool FIRST>
+static void cpoisson_go(const CPoissonArgs& a, dim3 grid, cudaStream_t s) {
+  if (!a.compose) cpoisson_kernel<FIRST, false><<<grid, kThreads, 0, s>>>(a);
+  else if (a.k5.out.p) cpoisson_kernel<FIRST, true, true><<<grid, kThreads, 0, s>>>(a);
+  else cpoisson_kernel<FIRST, true><<<grid, kThreads, 0, s>>>(a);
+}
 cudaError_t launch_cpoisson(const CPoissonArgs& a, cudaStream_t s) {
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
-  if (a.first) { if (a.compose) cpoisson_kernel<true, true><<<grid, kThreads, 0, s>>>(a); else cpoisson_kernel<true, false><<<grid, kThreads, 0, s>>>(a); }
-  else { if (a.compose) cpoisson_kernel<false, true><<<grid, kThreads, 0, s>>>(a); else cpoisson_kernel<false, false><<<grid, kThreads, 0, s>>>(a); }
+  if (a.first) cpoisson_go<true>(a, grid, s);
+  else cpoisson_go<false>(a, grid, s);
   return cudaGetLastError();
 }
 
@@ -513,7 +527,7 @@ RFX_D void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, unsign
                : "memory");
 }
 
-template <bool COMPOSE>
+template <bool COMPOSE, bool IMAGE = false>
 __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_constant__ CPoissonTmaArgs t) {
   extern __shared__ __align__(1024) unsigned char tile[];
   __shared__ unsigned long long bar;
@@ -559,10 +573,11 @@ __global__ void __launch_bounds__(kThreads, 4) cpoisson_tma_kernel(const __grid_
       const unsigned off = (unsigned)y * (unsigned)a.composed_carry.local.pitch + (unsigned)x * 16u;
       st_f4(a.composed.p, a.composed.pitch, x, y, *((const float4*)(peer_row_base(a.composed_carry, y) + off)));
     }
+    if (IMAGE && y >= a.crow0 && y < a.crow1) st_h4(a.k5.out.p, a.k5.out.pitch, x, y, k5_background(a.k5, x, y));
     return;
   }
-  if (interior) cpoisson_body<false, COMPOSE, true, true>(a, x, y, nc, fwn, st);
-  else cpoisson_body<false, COMPOSE, false, false>(a, x, y, nc, fwn);
+  if (interior) cpoisson_body<false, COMPOSE, IMAGE, true, true>(a, x, y, nc, fwn, st);
+  else cpoisson_body<false, COMPOSE, IMAGE, false, false>(a, x, y, nc, fwn);
 }
 
 static constexpr size_t kTmaSmemCap = 100 * 1024;  // dynamic shared memory cpoisson_tma_kernel may take
@@ -587,13 +602,17 @@ cudaError_t launch_cpoisson_tma(const CPoissonTmaArgs& t, cudaStream_t s) {
   if (dev >= 64 || !attr_set[dev]) {
     cudaFuncSetAttribute(cpoisson_tma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemCap);
     cudaFuncSetAttribute(cpoisson_tma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemCap);
+    cudaFuncSetAttribute(cpoisson_tma_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTmaSmemCap);
     if (dev < 64) attr_set[dev] = true;
   }
-  if (t.a.compose) cpoisson_tma_kernel<true><<<grid, kThreads, smem, s>>>(t); else cpoisson_tma_kernel<false><<<grid, kThreads, smem, s>>>(t);
+  if (!t.a.compose) cpoisson_tma_kernel<false><<<grid, kThreads, smem, s>>>(t);
+  else if (t.a.k5.out.p) cpoisson_tma_kernel<true, true><<<grid, kThreads, smem, s>>>(t);
+  else cpoisson_tma_kernel<true><<<grid, kThreads, smem, s>>>(t);
   return cudaGetLastError();
 }
 
-// stand-alone K4 (denoiseIterations == 0: no Poisson pass to ride on)
+// stand-alone K4 (denoiseIterations == 0: no Poisson pass to ride on); IMAGE as cpoisson_kernel's
+template <bool IMAGE>
 __global__ void __launch_bounds__(kThreads) ccompose_kernel(const __grid_constant__ CComposeArgs a) {
   int x, y;
   const bool in_rows = range_pixel(a.row0, a.row1, x, y);
@@ -607,16 +626,19 @@ __global__ void __launch_bounds__(kThreads) ccompose_kernel(const __grid_constan
       const unsigned off = (unsigned)y * (unsigned)a.composed_carry.local.pitch + (unsigned)x * 16u;
       st_f4(a.composed.p, a.composed.pitch, x, y, *((const float4*)(peer_row_base(a.composed_carry, y) + off)));
     }
+    if (IMAGE) st_h4(a.k5.out.p, a.k5.out.pitch, x, y, k5_background(a.k5, x, y));
     return;
   }
   const uint4 q = __ldg((const uint4*)(a.dn.p + ((unsigned)y * (unsigned)a.dn.pitch + (unsigned)x * 16u)));
   const float4 g = ld_f4(a.gb, x, y);
-  st_f4(a.composed.p, a.composed.pitch, x, y,
-        c_compose(a.cam, x, y, a.W, a.H, g, nrdz_roughness(nc), nc.w, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w))));
+  const float4 c = c_compose(a.cam, x, y, a.W, a.H, g, nrdz_roughness(nc), nc.w, mk3(h_lo(q.x), h_hi(q.x), h_lo(q.y)), mk3(h_lo(q.z), h_hi(q.z), h_lo(q.w)));
+  st_f4(a.composed.p, a.composed.pitch, x, y, c);
+  if (IMAGE) st_h4(a.k5.out.p, a.k5.out.pitch, x, y, ssgi_compose_lit(a.k5, x, y, nc.w, [&] { return c; }));
 }
 cudaError_t launch_ccompose(const CComposeArgs& a, cudaStream_t s) {
   dim3 grid((a.W + kTileW - 1) / kTileW, row_tiles(a.row0, a.row1));
-  ccompose_kernel<<<grid, kThreads, 0, s>>>(a);
+  if (a.k5.out.p) ccompose_kernel<true><<<grid, kThreads, 0, s>>>(a);
+  else ccompose_kernel<false><<<grid, kThreads, 0, s>>>(a);
   return cudaGetLastError();
 }
 

@@ -634,6 +634,12 @@ rfx_status rfx_gi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_compose_p
   return gi_compose(ctx, stream, p, depth, gb, dgi, sgi, scene, out, r0, r1);
 }
 
+// K5's uniforms from the C ABI's parameters (fog, camera, isDebug)
+static void compose_uniforms(const rfx_ssgi_compose_params& p, SsgiComposeArgs& a) {
+  a.use_fog = p.use_fog; a.fog_exp2 = p.fog_exp2; a.perspective = p.perspective; a.is_debug = p.is_debug;
+  memcpy(a.fog_color, p.fog_color, 12);
+  a.fog_near = p.fog_near; a.fog_far = p.fog_far; a.fog_density = p.fog_density; a.camera_near = p.camera_near; a.camera_far = p.camera_far;
+}
 // K5 with isDebug for a view ssgi_compose_kernel does not fetch (another format or size): depth and scene are not read
 static rfx_status ssgi_compose_debug(rfx_ctx* ctx, void* stream, const rfx_plane* gi, const rfx_plane* out, uint32_t row0, uint32_t row1) {
   SsgiComposeDebugArgs a{};
@@ -656,11 +662,7 @@ rfx_status rfx_ssgi_compose_launch(rfx_ctx* ctx, void* stream, const rfx_ssgi_co
   a.W = (int)out->width; a.H = (int)out->height;
   if (a.depth.w != a.W || a.depth.h != a.H || a.gi.w != a.W || a.scene.w != a.W) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "ssgi_compose: plane sizes differ");
   rows(row0, row1, out->height, a.row0, a.row1);
-  if (p) {
-    a.use_fog = p->use_fog; a.fog_exp2 = p->fog_exp2; a.perspective = p->perspective; a.is_debug = p->is_debug;
-    memcpy(a.fog_color, p->fog_color, 12);
-    a.fog_near = p->fog_near; a.fog_far = p->fog_far; a.fog_density = p->fog_density; a.camera_near = p->camera_near; a.camera_far = p->camera_far;
-  }
+  if (p) compose_uniforms(*p, a);
   LAUNCHED(launch_ssgi_compose(a, pick(ctx, stream)));
   return RFX_OK;
 }
@@ -1078,6 +1080,11 @@ struct rfx_ssgi_chain : GroupMember {
   // debug view of the tail's K5 (rfx_ssgi_chain_set_debug_view); RFX_DEBUG_VIEW_NONE: composed, isDebug off
   int32_t debug_view = RFX_DEBUG_VIEW_NONE;
   rfx_plane debug_gb{};                 // GBufferDebugPass target of the G-buffer channel views
+  // the compose stage (rfx_ssgi_chain_set_compose): K5 of output 0 into `image` (output 9).  The fast chain writes image[frame parity]
+  // (as `composed`, so that a host-path download of frame i-1 never races frame i); the per-pass chain writes image[0].
+  bool compose_on = false;
+  rfx_ssgi_compose_params compose_p{};
+  rfx_plane image[2]{};
   // optional per-pass event timing
   bool profiling = false;
   struct Span { cudaEvent_t a, b; int slot; };
@@ -1256,7 +1263,7 @@ void rfx_ssgi_chain_destroy(rfx_ssgi_chain* ch) {
   for (HistPlane* h : every_hist_plane(ch))
     for (rfx_plane& p : h->buf) if (p.ptr) rfx_plane_free(ctx, &p);
   traa_free(ctx, ch->tail);
-  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->debug_gb,
+  rfx_plane* all[] = {&ch->fb, &ch->ssgi_out, &ch->debug_gb, &ch->image[0], &ch->image[1],
                       &ch->in_depth[0], &ch->in_gb[0], &ch->in_vel[0], &ch->in_direct[0], &ch->in_depth[1], &ch->in_gb[1], &ch->in_vel[1], &ch->in_direct[1]};
   for (rfx_plane* p : all) if (p->ptr) rfx_plane_free(ctx, p);
   for (IPlane* p : {&ch->nrdz, &ch->tr32}) if (p->p) cudaFree(p->p);
@@ -1309,8 +1316,35 @@ rfx_status rfx_ssgi_chain_reset(rfx_ssgi_chain* ch) {
 rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_options* opt) {
   if (!ch) return RFX_ERR_INVALID_ARG;
   if (ch->group) return fail(ch->ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
+  if (opt && ch->compose_on) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain_enable_traa: the compose stage is on, and the tail runs K5 itself (turn the stage off first)");
   const bool k5 = !ch->fastpath || ch->debug_view != RFX_DEBUG_VIEW_NONE;  // the fast chain's fused tail needs no K5 plane
   return traa_enable(ch->ctx, ch->tail, opt, ch->opt.width, ch->opt.height, true, k5);
+}
+
+rfx_status rfx_ssgi_chain_set_compose(rfx_ssgi_chain* ch, const rfx_ssgi_compose_params* p) {
+  if (!ch) return RFX_ERR_INVALID_ARG;
+  rfx_ctx* ctx = ch->ctx;
+  if (!p) {
+    if (ch->image[0].ptr) {  // no launch or download may still use the planes
+      CU(cudaStreamSynchronize(ctx->stream));
+      rfx_status st = host_pipe_wait(ctx, ch->host, 0);
+      if (st != RFX_OK) return st;
+      for (rfx_plane& b : ch->image)
+        if (b.ptr) { rfx_plane_free(ctx, &b); b = rfx_plane{}; }
+    }
+    ch->compose_on = false;
+    return RFX_OK;
+  }
+  if (p->is_debug) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_set_compose: is_debug is not a stage option (select a view with rfx_ssgi_chain_set_debug_view)");
+  if (ch->tail.on) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_set_compose: the TRAA tail is on, and it runs K5 itself");
+  for (int b = 0; b < (ch->fastpath ? 2 : 1); b++)
+    if (!ch->image[b].ptr) {
+      rfx_status st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->image[b]);
+      if (st != RFX_OK) return st;
+    }
+  ch->compose_p = *p;
+  ch->compose_on = true;
+  return RFX_OK;
 }
 
 rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* ch, const rfx_motion_blur_params* p) {
@@ -1347,7 +1381,12 @@ extern "C" {
 rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* ch, int32_t which, rfx_plane* out) {
   if (!ch || !out) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
-  if (which < 0 || which > 8) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..8");
+  if (which < 0 || which > 9) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: which must be 0..9");
+  if (which == 9) {
+    if (!ch->compose_on) return fail(ctx, RFX_ERR_INVALID_ARG, "chain_output: output 9 needs the compose stage (rfx_ssgi_chain_set_compose)");
+    *out = ch->image[ch->fastpath ? (int)((ch->frame_idx + 1) & 1) : 0];  // the fast chain's by the parity of the latest frame
+    return RFX_OK;
+  }
   if (which >= 6) {
     if (!ch->tail.on) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: outputs 6 / 7 / 8 need the TRAA tail (rfx_ssgi_chain_enable_traa)");
     if (which == 8 && !ch->tail.fx) return fail(ctx, RFX_ERR_NOT_READY, "chain_output: output 8 needs the cosmetic stage (rfx_ssgi_chain_set_effects)");
@@ -1526,6 +1565,30 @@ static rfx_status traa_blur_finish(rfx_ctx* ctx, void* stream, TraaTail& t, cons
   return tail_end(ctx, stream, t);
 }
 
+// The compose stage as a per-pass launch on rows kr: K5 of output 0 (`out0`), or with a debug view selected K5 with isDebug of the view,
+// into `out` (the per-pass chain, and the fast chain while a view is selected)
+static rfx_status chain_render_stage(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane* out0, const rfx_plane* out, Rows kr) {
+  rfx_ssgi_compose_params q = ch->compose_p;
+  const rfx_plane* view = out0;
+  if (ch->debug_view != RFX_DEBUG_VIEW_NONE) {
+    q.is_debug = 1;
+    rfx_status st = debug_view_plane(ch, stream, f, &view);
+    if (st != RFX_OK) return st;
+  }
+  return rfx_ssgi_compose_launch(ch->ctx, stream, &q, f->depth, view, f->direct_light, out, (uint32_t)kr.r0, (uint32_t)kr.r1);
+}
+// The compose stage fused into the fast chain's K4 (cpoisson / ccompose with k5.out set): K5's planes and uniforms, `out` its image
+static rfx_status stage_args(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f, const rfx_plane& out, SsgiComposeArgs& c) {
+  rfx_ctx* ctx = ch->ctx;
+  const int W = (int)ch->opt.width, H = (int)ch->opt.height;
+  if (!pv(f->depth, RFX_FMT_R32F, c.depth) || !pv(f->direct_light, RFX_FMT_RGBA16F, c.scene) || !ov(&out, RFX_FMT_RGBA16F, c.out))
+    return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: the compose stage needs an RGBA16F direct light plane");
+  if (c.scene.w != W || c.scene.h != H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "chain: the direct light plane must match the chain size");
+  c.W = W; c.H = H; c.row0 = 0; c.row1 = H;
+  compose_uniforms(ch->compose_p, c);
+  return RFX_OK;
+}
+
 // The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
 // rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
 // K2 on them +- 1).
@@ -1554,10 +1617,7 @@ static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_
       return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: the TRAA tail needs an RGBA16F direct light plane");
     if (c.scene.w != W || c.scene.h != H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "chain: the direct light plane must match the chain size");
     c.W = W; c.H = H; c.row0 = 0; c.row1 = H;
-    const rfx_ssgi_compose_params& q = tail.opt.compose;
-    c.use_fog = q.use_fog; c.fog_exp2 = q.fog_exp2; c.perspective = q.perspective; c.is_debug = q.is_debug;
-    memcpy(c.fog_color, q.fog_color, 12);
-    c.fog_near = q.fog_near; c.fog_far = q.fog_far; c.fog_density = q.fog_density; c.camera_near = q.camera_near; c.camera_far = q.camera_far;
+    compose_uniforms(tail.opt.compose, c);
     a.hist = tail.acc.view[tail.cur() ^ 1];
     a.acc = rov(tail.acc.buf[tail.cur()]);
     a.out = rov(tail.out);
@@ -1665,6 +1725,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     return RFX_OK;
   };
   const uint32_t k_compose = 2u + (uint32_t)n_pass;
+  // the compose stage rides on K4 unless a debug view is selected (then it is a launch of its own after K4)
+  const bool fused_stage = ch->compose_on && ch->debug_view == RFX_DEBUG_VIEW_NONE;
   for (int i = 0; i < n_pass; i++, k++) {
     if (!on(k)) continue;
     const bool horizontal = (i % 2) == 0, last = i == n_pass - 1;
@@ -1704,6 +1766,7 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
       a.composed = rov(ch->composed.buf[cur]);
       a.composed_carry = ch->composed.view[prev];
       a.cam = cam;
+      if (fused_stage && (st = stage_args(ch, f, ch->image[cur], a.k5)) != RFX_OK) return st;
     }
     SpanGuard g(ch, cs, i == 0 ? 2 : 3);
     const int box_w = (kTileW + 2 * a.reach_x) | 1, box_h = kTileH + 2 * a.reach_y;  // odd row pitch in texels: consecutive tile rows start 4 banks apart
@@ -1730,9 +1793,12 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
     a.composed = rov(ch->composed.buf[cur]);
     a.composed_carry = ch->composed.view[prev];
     a.W = W; a.H = H; a.cam = cam;
+    if (fused_stage && (st = stage_args(ch, f, ch->image[cur], a.k5)) != RFX_OK) return st;
     SpanGuard g(ch, cs, 4);
     LAUNCHED(launch_ccompose(a, cs));
   }
+  if (ch->compose_on && !fused_stage && on(k) && (st = chain_render_stage(ch, stream, f, &ch->composed.buf[cur], &ch->image[cur], launch_rows(ranges, k, H))) != RFX_OK)
+    return st;
   // ---- TRAA tail (reads this frame's `composed`, so it runs before the planes change parity)
   if (ch->tail.on && on(k_compose + 1) && (st = chain_render_tail(ch, stream, f, &ch->composed.buf[cur], ranges, k_compose + 1)) != RFX_OK) return st;
   if (on(ch->tail.on ? k_compose + 1 : k_compose)) ch->frame_idx++;  // the frame is complete: its planes become `prev`
@@ -1744,7 +1810,8 @@ static rfx_status chain_render_fast(rfx_ssgi_chain* ch, void* stream, const rfx_
 // recompute locally (rfx_shard_ranges).  Only launches k in [k_begin, k_end) are issued, so a caller can wait between two
 // launches of a frame (rfx_ssgi_chain_submit_host waits before K4); per-frame state advances with the launch that consumes it.
 static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const uint32_t* ranges, uint32_t k_begin, uint32_t k_end) {
-  if (ch->tail.on && !f->direct_light) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail composes over the direct light plane (the composer input buffer): it may not be NULL");
+  if ((ch->tail.on || ch->compose_on) && !f->direct_light)
+    return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain: the TRAA tail and the compose stage compose over the direct light plane (the composer input buffer): it may not be NULL");
   if (ch->fastpath) return chain_render_fast(ch, stream, f, ranges, k_begin, k_end);
   rfx_ctx* ctx = ch->ctx;
   const rfx_ssgi_chain_options& o = ch->opt;
@@ -1857,6 +1924,8 @@ static rfx_status chain_render_impl(rfx_ssgi_chain* ch, void* stream, const rfx_
     }
     if (st != RFX_OK) return st;
   }
+  // ---- the compose stage over output 0 (`composed`, or the temporal texture in denoiseMode "temporal", which K2 wrote)
+  if (ch->compose_on && on(k) && (st = chain_render_stage(ch, stream, f, &accumulated.buf[wr], &ch->image[0], launch_rows(ranges, k, H))) != RFX_OK) return st;
   k++;
   // ---- TRAA tail over the effect's output (`composed`, or the temporal texture in denoiseMode "temporal")
   if (ch->tail.on && on(k)) return chain_render_tail(ch, stream, f, &accumulated.buf[wr], ranges, k);
@@ -1869,14 +1938,21 @@ rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* ch, void* stream, const rfx_ssg
 }
 
 // Host-buffer path.  submit enqueues one frame and returns: the four input planes go H2D on a copy stream into staging set
-// (frame & 1), the chain runs on the context stream once that upload's event fires, and `composed` goes D2H on a third stream once
-// the frame's last kernel is done.  Frame i+1 therefore uploads (and frame i-1 downloads) while frame i renders; PCIe is full
-// duplex, so steady-state time per frame is max(H2D, kernels, D2H) instead of their sum.  Hazards, all resolved on the device:
+// (frame & 1), the chain runs on the context stream once that upload's event fires, and `composed` and / or the frame's image go D2H
+// on a third stream once the frame's last kernel is done.  Frame i+1 therefore uploads (and frame i-1 downloads) while frame i renders;
+// PCIe is full duplex, so steady-state time per frame is max(H2D, kernels, D2H) instead of their sum.  Hazards, all resolved on the
+// device:
 //   staging set reuse   - the upload of frame i+2 waits for frame i's kernels (ev_rendered);
-//   `composed` reuse    - K4 of frame i+1 (the only writer) waits for frame i's D2H (ev_dn); K1 of frame i+1 only reads it.
+//   downloaded planes   - fast chain: `composed` and the compose stage's image (output 9) are double-buffered by frame parity, and
+//                         frame i+2's kernels wait for frame i's D2H (ev_dn); the TRAA tail's image (output 6: K9's, the merged
+//                         TRAA + motion-blur pass's or the cosmetic stage's plane) is single-buffered, so frame i+1's tail waits for
+//                         frame i's D2H.  Per-pass chain: every downloaded plane is written by K4, the compose stage or the tail, which
+//                         all wait for frame i's D2H (ev_dn); K1 of frame i+1 only reads `composed`.
 rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_frame* hf) {
-  if (!ch || !hf || !hf->depth || !hf->gbuffer || !hf->velocity || !hf->out_composed) return RFX_ERR_INVALID_ARG;
+  if (!ch || !hf || !hf->depth || !hf->gbuffer || !hf->velocity || (!hf->out_composed && !hf->out_color)) return RFX_ERR_INVALID_ARG;
   rfx_ctx* ctx = ch->ctx;
+  if (hf->out_color && !ch->compose_on && !ch->tail.on)
+    return fail(ctx, RFX_ERR_NOT_READY, "chain_submit_host: out_color is the compose stage's or the TRAA tail's image, and both are off");
   rfx_status st = RFX_OK;
   HostPipe& hp = ch->host;
   if (!hp.ready) {
@@ -1906,7 +1982,13 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     const int cur = (int)(ch->frame_idx & 1);
     for (int q = 0; q < 2; q++)
       if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[q], 0));
-    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, 0xffffffffu)) != RFX_OK) return st;
+    // the tail (the launch after K4) writes its single-buffered image: it waits for the previous frame's D2H
+    const uint32_t split = ch->tail.on ? 3u + 2u * (uint32_t)ch->opt.denoise_iterations : 0xffffffffu;
+    if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, split)) != RFX_OK) return st;
+    if (ch->tail.on) {
+      if (hp.submitted >= 1) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[set ^ 1], 0));
+      if ((st = chain_render_impl(ch, nullptr, &f, nullptr, split, 0xffffffffu)) != RFX_OK) return st;
+    }
     result = &ch->composed.buf[cur];
     ch->dn_buf[set] = cur;
   } else {
@@ -1916,9 +1998,12 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     if (hp.submitted >= 1) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[set ^ 1], 0));
     if ((st = chain_render_impl(ch, nullptr, &f, nullptr, split, 0xffffffffu)) != RFX_OK) return st;
   }
+  rfx_plane image{};  // the frame's image: output 9 with the compose stage, else output 6 (the tail's)
+  if (hf->out_color && (st = rfx_ssgi_chain_output(ch, ch->compose_on ? 9 : 6, &image)) != RFX_OK) return st;
   CU(cudaEventRecord(hp.ev_rendered[set], ctx->stream));
   CU(cudaStreamWaitEvent(hp.s_dn, hp.ev_rendered[set], 0));
-  if ((st = rfx_plane_download(ctx, hp.s_dn, result, hf->out_composed, 0)) != RFX_OK) return st;
+  if (hf->out_composed && (st = rfx_plane_download(ctx, hp.s_dn, result, hf->out_composed, 0)) != RFX_OK) return st;
+  if (hf->out_color && (st = rfx_plane_download(ctx, hp.s_dn, &image, hf->out_color, 0)) != RFX_OK) return st;
   CU(cudaEventRecord(hp.ev_dn[set], hp.s_dn));
   hp.submitted++;
   return RFX_OK;

@@ -121,18 +121,15 @@ struct SsgiComposeArgs {
   float fog_color[3], fog_near, fog_far, fog_density, camera_near, camera_far;
 };
 cudaError_t launch_ssgi_compose(const SsgiComposeArgs& a, cudaStream_t s);
-// K5 for pixel (x, y): the texel ssgi_compose_kernel stores (RGBA16F).  Shared with the fused TRAA tail (k_temporal.cu).
-RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
-  if (a.is_debug) {  // ssgi_compose.frag:21-24
-    const float4 t = ld_f4(a.gi, x, y);
-    return mk4(t.x, t.y, t.z, t.w);
-  }
-  const float depth = ld_r32f(a.depth, x, y);
+// K5 without isDebug for pixel (x, y) of depth `depth`; gi() returns the pixel's GI texel and is called for a foreground pixel only.
+// Shared with the compose stage fused into the fast chain's K4 (k_chain.cu), which passes the texel it just composed.
+template <class GI>
+RFX_D v4 ssgi_compose_lit(const SsgiComposeArgs& a, int x, int y, float depth, const GI& gi) {
   v3 c;
   if (depth == 1.0f) {
     c = xyz(tex_h4_linear(a.scene, pixel_uv(x, y, a.W, a.H)));
   } else {
-    c = xyz(f4v(ld_f4(a.gi, x, y)));
+    c = xyz(f4v(gi()));
     if (a.use_fog) {  // :34-41 + three.js <fog_fragment>
       const float gz = a.perspective ? perspectiveDepthToViewZ(depth, a.camera_near, a.camera_far) : orthographicDepthToViewZ(depth, a.camera_near, a.camera_far);
       const float vFogDepth = -(gz * 0.4f);
@@ -141,6 +138,14 @@ RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
     }
   }
   return mk4(c, 1.0f);
+}
+// K5 for pixel (x, y): the texel ssgi_compose_kernel stores (RGBA16F).  Shared with the fused TRAA tail (k_temporal.cu).
+RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
+  if (a.is_debug) {  // ssgi_compose.frag:21-24
+    const float4 t = ld_f4(a.gi, x, y);
+    return mk4(t.x, t.y, t.z, t.w);
+  }
+  return ssgi_compose_lit(a, x, y, ld_r32f(a.depth, x, y), [&] { return ld_f4(a.gi, x, y); });
 }
 // K5 with isDebug for the views ssgi_compose_kernel does not fetch (its debug branch reads an RGBA32F plane of the output's size):
 // `gi` of any size and format, sampled at the pixel centre with its own sampler.
@@ -394,6 +399,9 @@ struct CPoissonArgs {
   OutV composed;
   PeerPV composed_carry;
   CamD cam;
+  // the chain's compose stage fused into K4 (rfx_ssgi_chain_set_compose): k5.out.p != nullptr selects the instantiations whose composing
+  // pixels also store K5 of the texel they composed (k5.gi is not read; a discarded pixel is background, whose K5 is the scene texel)
+  SsgiComposeArgs k5;
 };
 cudaError_t launch_cpoisson(const CPoissonArgs& a, cudaStream_t s);
 struct CPoissonTmaArgs {  // passes >= 1 with TMA-staged tiles (experiment, RFX_K3_TMA=1)
@@ -412,6 +420,7 @@ struct CComposeArgs {   // stand-alone K4 over dn (denoiseIterations == 0)
   PeerPV composed_carry;
   int W, H, row0, row1;
   CamD cam;
+  SsgiComposeArgs k5;  // as CPoissonArgs::k5
 };
 cudaError_t launch_ccompose(const CComposeArgs& a, cudaStream_t s);
 

@@ -306,9 +306,18 @@ class _Chain:
 class SsgiChain(_Chain):
     """Native SSGI chain (rfx_ssgi_chain): K1 -> K2 -> K3 x 2*iterations -> K4 with history, and optionally the TRAA frame tail (K5 ->
     TRAA -> K9 after K4).  Outputs: 0 composed, 1 ssgiOut, 2/3 trOut, 4/5 dnB; with the TRAA tail on, 6 the K9 output and 7 the TRAA
-    accumulated plane; with the cosmetic stage on (set_effects), 6 is the stage's image and 8 the K9 output it reads."""
+    accumulated plane; with the cosmetic stage on (set_effects), 6 is the stage's image and 8 the K9 output it reads; with the compose
+    stage on (set_compose), 9 the stage's image."""
 
     _PREFIX = "rfx_ssgi_chain"
+    compose = None  # the compose stage's parameters while it is on
+
+    def set_compose(self, params: "abi.SsgiComposeParams | None"):
+        """Compose stage (include/rfx.h: rfx_ssgi_chain_set_compose): every frame ends with K5 ssgi_compose over output 0, depth and the
+        direct light, SSGIEffect's image, into output 9.  params: the fog and camera values (is_debug 0); None turns the stage off.  Not
+        with the TRAA tail, which runs K5 itself."""
+        self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_set_compose(self.h, C.byref(params) if params is not None else None))
+        self.compose = params
 
     def set_debug_view(self, view: int):
         """the TRAA tail's K5 shows `view` (abi.DEBUG_VIEW_*; include/rfx.h: rfx_ssgi_chain_set_debug_view) instead of composed"""
@@ -341,6 +350,26 @@ class SsgiChain(_Chain):
         n = (C.c_uint64 * 5)()
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_get_profile(self.h, ms, n))
         return {k: (float(ms[i]), int(n[i])) for i, k in enumerate(self.PROFILE_SLOTS)}
+
+    @staticmethod
+    def host_frame(cam: abi.CameraS, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, out_composed=None,
+                   out_color=None) -> abi.SsgiHostFrame:
+        """rfx_ssgi_host_frame over host arrays (numpy, or CPU torch tensors, pinned for asynchronous copies; rows tightly packed):
+        depth float32 H x W, gbuffer / velocity float32 H x W x 4, direct_light float16 H x W x 4 (or None); out_composed float32
+        H x W x 4 receives `composed`, out_color float16 H x W x 4 the frame's image (output 9 with the compose stage, output 6 with the
+        TRAA tail); either may be None.  The arrays must outlive the frame: the returned struct holds their addresses only."""
+        def addr(a):
+            if a is None:
+                return None
+            return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
+
+        hf = abi.SsgiHostFrame()
+        hf.cam = cam
+        hf.depth, hf.gbuffer, hf.velocity, hf.direct_light = addr(depth), addr(gbuffer), addr(velocity), addr(direct_light)
+        hf.camera_pos[:] = [float(x) for x in camera_pos]
+        hf.camera_moved = int(bool(camera_moved))
+        hf.out_composed, hf.out_color = addr(out_composed), addr(out_color)
+        return hf
 
     def render_host(self, hf: abi.SsgiHostFrame):
         self.ctx._chk(self.ctx.lib.rfx_ssgi_chain_render_host(self.h, C.byref(hf)))

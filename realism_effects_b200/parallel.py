@@ -271,6 +271,22 @@ def _raw_plane(abi, ptr: int, width: int, height: int, pitch: int, fmt: int):
     return p
 
 
+def download_band(ctx, stream, downloads, b0: int, b1: int) -> int:
+    """rows [b0, b1) of every (rfx_plane, host tensor) pair of `downloads` D2H on `stream`, tightly packed at the start of the host
+    tensor (a pair whose tensor is None is skipped); returns the bytes moved"""
+    import ctypes as C
+
+    from . import abi
+
+    n = 0
+    for plane, out in downloads:
+        if out is None:
+            continue
+        ctx._chk(ctx.lib.rfx_plane_download_rows(ctx.h, stream, C.byref(plane), out.data_ptr(), b0, b1))
+        n += (b1 - b0) * plane.width * abi.FMT_BYTES[plane.format]
+    return n
+
+
 def _group_unique_id(ctx, rank, world, unique_id, dist_group):
     """(rank, world, 128-byte NCCL unique id): as given, or from torch.distributed (rank 0 makes the id and broadcasts it)"""
     import ctypes as C
@@ -370,6 +386,11 @@ class ShardedSsgiChain:
         frame (the stage keeps no plane the group maps)"""
         self.chain.set_effects(params)
 
+    def set_compose(self, params):
+        """the compose stage (engine.SsgiChain.set_compose: output 9, K5 over output 0), or None to turn it off; the same on every rank,
+        any frame (it runs on the band and keeps no plane the group maps)"""
+        self.chain.set_compose(params)
+
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, stream=None):
         """Collective: one frame from full-frame device planes; this rank renders its band and joins the frame's collectives.  Both
         phases of a frame with the motion-blur stage (render_sharded, then render_sharded_finish; the latter is a no-op otherwise)."""
@@ -424,33 +445,39 @@ class ShardedSsgiChain:
         h["bytes"] = (0, 0)
         self._host = h
 
-    def submit_host(self, cam, host: dict, camera_pos, camera_moved: bool, out_host):
+    def submit_host(self, cam, host: dict, camera_pos, camera_moved: bool, out_host, out_color=None):
         """One frame from host planes (dict name -> CPU tensor of the FULL frame, pinned for asynchronous copies) to this rank's
-        rows of `composed`, written to the start of out_host (CPU float32 tensor of at least MAX_SHARE x the mean band height).
-        Returns the band (row0, row1) the rows belong to, after enqueueing.  Not with the TRAA tail: the rows uploaded here
-        (local_input_rows) are sized for the chain without it."""
+        rows of `composed`, written to the start of out_host (CPU float32 tensor of at least MAX_SHARE x the mean band height x W x 4),
+        and of the compose stage's image (output 9, set_compose first), written to the start of out_color (CPU float16 tensor of the
+        same number of texels).  Either may be None, not both.  Returns the band (row0, row1) the rows belong to, after enqueueing.  Not
+        with the TRAA tail: the rows uploaded here (local_input_rows) are sized for the chain without it."""
+        abi = self._abi
         if self.chain.traa is not None:
-            raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path does not render the TRAA tail")
+            raise abi.RfxError(f"rfx status {abi.ERR_UNSUPPORTED}: submit_host: the sharded host path does not render the TRAA tail")
         o = self.chain.opt
-        if o.mode != self._abi.MODE_SSGI or o.denoise_mode != 0:
-            raise self._abi.RfxError(f"rfx status {self._abi.ERR_UNSUPPORTED}: submit_host: the sharded host path renders the fast SSGI chain only "
-                                     "(mode SSGI, denoiseMode \"full\"): its upload rows are planned for that chain")
+        if o.mode != abi.MODE_SSGI or o.denoise_mode != 0:
+            raise abi.RfxError(f"rfx status {abi.ERR_UNSUPPORTED}: submit_host: the sharded host path renders the fast SSGI chain only "
+                               "(mode SSGI, denoiseMode \"full\"): its upload rows are planned for that chain")
+        if out_host is None and out_color is None:
+            raise abi.RfxError(f"rfx status {abi.ERR_INVALID_ARG}: submit_host: out_host and out_color are both None")
+        if out_color is not None and self.chain.compose is None:
+            raise abi.RfxError(f"rfx status {abi.ERR_NOT_READY}: submit_host: out_color is the compose stage's image, and the stage is off")
 
         def rows(bounds):
             return ShardPlan(o.height, self.world, self.rank, 2 * o.denoise_iterations, o.radius, True, bounds=bounds, width=o.width).local_input_rows
 
         def render(st, plane):
             self.render(cam, plane("depth"), plane("gbuffer"), plane("velocity"), plane("direct"), camera_pos, camera_moved)
-            # `composed` is double-buffered by frame parity: the plane of frame i is next written by frame i+2, which waits for this
-            # frame's D2H through ev_dn, so the rows go D2H straight from the plane
-            return self.chain.output(0)
+            # `composed` and the compose stage's image are double-buffered by frame parity: the planes of frame i are next written by
+            # frame i+2, which waits for this frame's D2H through ev_dn, so the rows go D2H straight from the planes
+            return [(self.chain.output(0), out_host), (self.chain.output(9) if out_color is not None else None, out_color)]
 
-        return self._submit_host_frame(host, rows, render, out_host)
+        return self._submit_host_frame(host, rows, render)
 
-    def _submit_host_frame(self, host: dict, local_rows, render, out_host):
+    def _submit_host_frame(self, host: dict, local_rows, render):
         """submit_host's pipeline: this rank's uploads into staging set (frame & 1) on the copy stream, the all-gather of the planes sampled
-        anywhere, render(staging set, plane of name) -> the plane whose band goes D2H, then that band on the third stream.
-        local_rows(bounds): the rows of the per-pixel input planes this rank reads."""
+        anywhere, render(staging set, plane of name) -> the (plane, host tensor) pairs whose band goes D2H, then those bands on the third
+        stream (download_band).  local_rows(bounds): the rows of the per-pixel input planes this rank reads."""
         if self._host is None:
             self._host_init()
         h = self._host
@@ -481,13 +508,12 @@ class ShardedSsgiChain:
             for name, _bpp, anywhere, _fmt in self.INPUTS:
                 if anywhere and host.get(name) is not None:
                     self.ctx._chk(self.lib.rfx_group_allgather_rows(self.g, None, self._C.byref(st[name][1]), bnd))
-        p = render(st, lambda n: _PlaneRef(st[n][1]) if host.get(n) is not None else None)
-        nbytes = (b1 - b0) * W * self._abi.FMT_BYTES[p.format]
+        downloads = render(st, lambda n: _PlaneRef(st[n][1]) if host.get(n) is not None else None)
         with torch.cuda.stream(h["main"]):
             h["ev_rendered"][k].record(h["main"])
         with torch.cuda.stream(h["dn"]):
             h["dn"].wait_event(h["ev_rendered"][k])
-            self.ctx._chk(self.lib.rfx_plane_download_rows(self.ctx.h, h["dn"].cuda_stream, self._C.byref(p), out_host.data_ptr(), b0, b1))
+            nbytes = download_band(self.ctx, h["dn"].cuda_stream, downloads, b0, b1)
             h["ev_dn"][k].record(h["dn"])
         h["frames"] += 1
         h["bytes"] = (h2d, nbytes)
@@ -572,6 +598,11 @@ class InProcessGroup:
         """the cosmetic stage with this frame's values for every member, or None to turn it off (any frame)"""
         for ch in self.chains:
             ch.set_effects(params)
+
+    def set_compose(self, params):
+        """the compose stage (output 9) for every member, or None to turn it off (any frame)"""
+        for ch in self.chains:
+            ch.set_compose(params)
 
     def render(self, cam, depth, gbuffer, velocity, direct_light, camera_pos, camera_moved: bool, wait: bool = True):
         """one frame: every member renders its band; all of them finish before the next frame starts (the host is the barrier).
@@ -685,9 +716,9 @@ class ShardedAoChain(ShardedSsgiChain):
                 src = torch.as_tensor(_CudaRows(p.ptr + b0 * p.pitch, b1 - b0, p.width * 8, p.pitch), device=out[0].device)
                 with torch.cuda.stream(self._host["main"]):
                     out[0].view(self._host["H"], out[2])[b0:b1].copy_(src)
-            return out[1]
+            return [(out[1], out_host)]
 
-        return self._submit_host_frame(host, rows, render, out_host)
+        return self._submit_host_frame(host, rows, render)
 
 
 class InProcessAoGroup(InProcessGroup):
