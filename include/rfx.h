@@ -493,9 +493,8 @@ rfx_status rfx_ssgi_chain_render(rfx_ssgi_chain* chain, void* stream, const rfx_
  * after K4 on every frame:  K5 ssgi_compose (of `composed`, depth and frame->direct_light, the composer input buffer SSGIEffect.update
  * binds) rounded to RGBA16F -> K2 in its TRAA form (temporal_reproject.frag with textureCount 1, inputType "diffuse", RGBA16F history
  * sampled LINEAR; src/traa/TRAAEffect.js:21-31) -> K9 traa_compose.  The TRAA pass uses the frame's un-jittered camera and the chain's
- * previous-frame matrices; jittering the rasteriser (TAAUtils.js) stays the host's job.  The fast chain runs the three passes as ONE
- * kernel (the K5 plane never reaches memory); every other chain runs rfx_ssgi_compose_launch -> rfx_temporal_reproject_launch ->
- * rfx_traa_compose_launch.  Both write the same bytes. */
+ * previous-frame matrices; jittering the rasteriser (TAAUtils.js) stays the host's job.  Every chain runs the three passes as
+ * rfx_ssgi_compose_launch -> rfx_temporal_reproject_launch -> rfx_traa_compose_launch would, and writes their bytes. */
 typedef struct rfx_traa_tail_options {
   rfx_ssgi_compose_params compose;    /* K5: fog / isDebug (ssgi_compose.frag:20-44)                                           */
   float max_blend;                    /* TRAAEffect forces 0.9                                                                   */
@@ -505,18 +504,17 @@ typedef struct rfx_traa_tail_options {
   int32_t full_accumulate;            /* option fullAccumulate (0); AND-ed with !frame->camera_moved                          */
   int32_t _pad;
 } rfx_traa_tail_options;
-/* Allocates the tail's planes (TRAA accumulated RGBA16F x 2 by frame parity, K9 output RGBA16F) and renders the tail from the next
- * frame on.  On a chain whose tail is on it replaces the options and resets the TRAA history (keepData 0 on the next frame:
+/* Allocates the tail's planes (TRAA accumulated RGBA16F x 2 by frame parity, K5 and K9 outputs RGBA16F) and renders the tail from the
+ * next frame on.  On a chain whose tail is on it replaces the options and resets the TRAA history (keepData 0 on the next frame:
  * TemporalReprojectPass.reset()).  opt == NULL turns the tail off and frees its planes.  With the tail on, a frame without
  * direct_light is RFX_ERR_INVALID_ARG; rfx_ssgi_chain_reset resets the TRAA history too.  A chain attached to a group
  * (rfx_group_attach_chain*) cannot change its tail: RFX_ERR_UNSUPPORTED. */
 rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* chain, const rfx_traa_tail_options* opt);
 /* Motion-blur stage of the TRAA tail: `new EffectPass(camera, traaEffect, motionBlurEffect)` as the reference README wires the SSGI frame
  * (readme.md:141-151).  With the stage on, rfx_traa_motion_blur_launch replaces K9 and writes output 6; its taps read the tail's K5 plane
- * (the TRAA pass's input buffer), so the fast chain runs its tail as the per-pass launches K5 -> K2 -> the merged pass (same TRAA bytes
- * as its fused tail).  p == NULL turns the stage off.  The host passes every frame's values before the frame, as MotionBlurEffect.update
- * sets them (frame, delta_time; resolution = the window size).  Tail off: RFX_ERR_NOT_READY (enable_traa(NULL) turns the stage off
- * with the tail).  samples < 1: RFX_ERR_INVALID_ARG.  On a chain attached to a group the stage cannot be turned on or off
+ * (the TRAA pass's input buffer).  p == NULL turns the stage off.  The host passes every frame's values before the frame, as
+ * MotionBlurEffect.update sets them (frame, delta_time; resolution = the window size).  Tail off: RFX_ERR_NOT_READY (enable_traa(NULL)
+ * turns the stage off with the tail).  samples < 1: RFX_ERR_INVALID_ARG.  On a chain attached to a group the stage cannot be turned on or off
  * (RFX_ERR_UNSUPPORTED); its values can change (every rank passes the same).  In a row-sharded group of n > 1 a frame with the stage has
  * two phases: rfx_ssgi_chain_render_sharded, then rfx_ssgi_chain_render_sharded_finish. */
 rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* chain, const rfx_motion_blur_params* p);
@@ -524,7 +522,7 @@ rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* chain, const rfx_motio
  * (example/main.js:517-538), as the last pass of the chain's frame.  With the stage on, one rfx_effects_launch with p's effect list, order
  * and values runs over the tail's image (K9's, or the merged TRAA + motion-blur pass's), with the frame's own depth (GradualBackground) and
  * velocity (Sparkle) planes, into a chain-owned RGBA16F plane that becomes output 6; output 8 is then the stage's input.  The bytes are
- * those of the tail followed by rfx_effects_launch with the same p.  The fused fast tail stays in use (its K9 plane is the stage's input).
+ * those of the tail followed by rfx_effects_launch with the same p.
  * The host passes p before every frame, camera included (GradualBackground and Sparkle read the camera's uniforms as they stand when the
  * EffectPass renders).  p == NULL turns the stage off and frees its plane; enable_traa(NULL) turns it off with the tail.  Tail off:
  * RFX_ERR_NOT_READY; n_effects outside 1..4 or an unknown RFX_FX_*: RFX_ERR_INVALID_ARG; between rfx_ssgi_chain_render_sharded and
@@ -562,8 +560,8 @@ rfx_status rfx_ssgi_chain_output(rfx_ssgi_chain* chain, int32_t which, rfx_plane
  *   RFX_DEBUG_VIEW_DEPTH / _VELOCITY / _GBUFFER   the frame's depth, velocity or packed G-buffer plane
  *   RFX_DEBUG_VIEW_GBUFFER_CHANNEL + m     GBufferDebugPass mode m (0..5, see rfx_gbuffer_debug_launch) of the frame's G-buffer,
  *                                          rendered into a chain-owned RGBA32F target every frame before the tail
- * While a view is selected the fast chain runs its tail as the three per-pass launches.  Selecting a view does not reset any
- * history (the reference's outputTexture setter calls no reset()).  A chain in a group of n > 1 takes no view: RFX_ERR_UNSUPPORTED. */
+ * Selecting a view does not reset any history (the reference's outputTexture setter calls no reset()).  A chain in a group of n > 1
+ * takes no view: RFX_ERR_UNSUPPORTED. */
 #define RFX_DEBUG_VIEW_NONE (-1)
 #define RFX_DEBUG_VIEW_OUTPUT 0
 #define RFX_DEBUG_VIEW_DEPTH 8

@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(256) traa_motion_blur_kernel(const __grid_cons
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = m.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= m.W || y >= m.row1) return;
   const v2 vUv = pixel_uv(x, y, m.W, m.H);
-  const v4 inputColor = traa_compose_px(PlaneH4{a.acc}, x, y, m.W, m.H);
+  const v4 inputColor = traa_compose_px(a.acc, x, y, m.W, m.H);
   v4 c;
   if constexpr (PEER) c = motion_blur_px(m, PeerH4{in}, inputColor, vUv, x, y);
   else c = motion_blur_px(m, PlaneH4{m.input}, inputColor, vUv, x, y);
@@ -261,7 +261,7 @@ cudaError_t launch_traa_motion_blur(const TraaMotionBlurArgs& a, cudaStream_t s,
 __global__ void __launch_bounds__(256) traa_compose_kernel(const __grid_constant__ TraaComposeArgs a) {
   const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = a.row0 + blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.W || y >= a.row1) return;
-  st_h4(a.out.p, a.out.pitch, x, y, traa_compose_px(PlaneH4{a.acc}, x, y, a.W, a.H));
+  st_h4(a.out.p, a.out.pitch, x, y, traa_compose_px(a.acc, x, y, a.W, a.H));
 }
 cudaError_t launch_traa_compose(const TraaComposeArgs& a, cudaStream_t s) {
   dim3 grid((a.W + 31) / 32, (a.row1 - a.row0 + 7) / 8);

@@ -392,7 +392,7 @@ static rfx_status ensure_step_table(rfx_ctx* ctx, int steps) {
   ctx->step_table_steps = steps;
   return RFX_OK;
 }
-// K2's uniforms for an a.W x a.H target (rfx_temporal_reproject_launch and the fused TRAA tail of the chain)
+// K2's uniforms for an a.W x a.H target
 static void temporal_uniforms(const rfx_ctx* ctx, const rfx_temporal_params* p, TemporalArgs& a) {
   cam_to_dev(p->cam, a.cam);
   memcpy(a.prev_view.m, p->prev_view_matrix, 64);
@@ -969,9 +969,8 @@ struct HistPlane {
   PeerPV view[2]{};
 };
 // The TRAA frame tail a chain can end with (rfx_*_chain_enable_traa): TRAAEffect's temporal pass over `mid` into the accumulated plane,
-// then K9.  `mid` is the composer buffer before the TRAA EffectPass: the SSGI chain's K5 output (per-pass tail only; the fused fast tail
-// has none), the AO chain's K7 output.  With the motion-blur stage on (rfx_*_chain_set_motion_blur), the merged TRAA + motion-blur pass
-// replaces K9; its taps read all of `mid`.  `mid` is single-buffered (buffer 0) unless a row-sharded group with the stage gave it buffer 1:
+// then K9.  `mid` is the composer buffer before the TRAA EffectPass: the SSGI chain's K5 output, the AO chain's K7 output.  With the
+// motion-blur stage on (rfx_*_chain_set_motion_blur), the merged TRAA + motion-blur pass replaces K9; its taps read all of `mid`.  `mid` is single-buffered (buffer 0) unless a row-sharded group with the stage gave it buffer 1:
 // then it goes by tail parity like `acc`, so that a rank's next frame never writes rows a slower peer's merged pass still reads.
 struct TraaTail {
   bool on = false;
@@ -1075,7 +1074,7 @@ struct rfx_ssgi_chain : GroupMember {
   float keep_data = 0.0f;  // SSGIEffect's constructor resets the denoiser (makeOptionsReactive -> reset())
   // blue-noise counters: one closure per material (BlueNoiseUtils.js:17-33)
   int32_t bn_trace = 0, bn_poisson = 0;
-  // the TRAA tail (`tail`, one more launch after K4) reads the frame's camera and the previous-frame matrices its K2 used
+  // the TRAA tail (`tail`, after K4) reads the frame's camera and the previous-frame matrices its K2 used
   rfx_temporal_params traa_tp{};
   // debug view of the tail's K5 (rfx_ssgi_chain_set_debug_view); RFX_DEBUG_VIEW_NONE: composed, isDebug off
   int32_t debug_view = RFX_DEBUG_VIEW_NONE;
@@ -1116,8 +1115,8 @@ static void traa_free(rfx_ctx* ctx, TraaTail& t) {
   for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], &t.out, &t.mid.buf[0], &t.mid.buf[1], &t.fx_plane}) if (p->ptr) rfx_plane_free(ctx, p);
 }
 // rfx_*_chain_enable_traa once the chain kind's own checks passed: NULL frees the tail's planes.  Otherwise the planes are allocated on
-// first use (`out` and `mid` where the chain asks for them; nothing is left allocated on failure), and the options replace the old ones.
-static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_options* opt, uint32_t W, uint32_t H, bool with_out, bool with_mid) {
+// first use (`out` where the chain asks for it; nothing is left allocated on failure), and the options replace the old ones.
+static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_options* opt, uint32_t W, uint32_t H, bool with_out) {
   if (!opt) {
     CU(cudaStreamSynchronize(ctx->stream));
     traa_free(ctx, t);
@@ -1128,7 +1127,7 @@ static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_opt
   }
   if (!t.acc.buf[0].ptr) {
     rfx_status st = RFX_OK;
-    for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], with_out ? &t.out : nullptr, with_mid ? &t.mid.buf[0] : nullptr})
+    for (rfx_plane* p : {&t.acc.buf[0], &t.acc.buf[1], with_out ? &t.out : nullptr, &t.mid.buf[0]})
       if (p && st == RFX_OK) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, p);
     if (st != RFX_OK) { traa_free(ctx, t); return st; }
     local_views(t.acc);
@@ -1140,17 +1139,11 @@ static rfx_status traa_enable(rfx_ctx* ctx, TraaTail& t, const rfx_traa_tail_opt
   return RFX_OK;
 }
 // rfx_*_chain_set_motion_blur: `fixed` = the chain's tail cannot change (it is attached to a group), so neither can the stage; its values can.
-// Turning the stage on allocates `mid` where the chain has none (the fused fast tail): the merged pass needs the whole input buffer.
-static rfx_status traa_set_blur(rfx_ctx* ctx, TraaTail& t, const rfx_motion_blur_params* p, bool fixed, uint32_t W, uint32_t H) {
+static rfx_status traa_set_blur(rfx_ctx* ctx, TraaTail& t, const rfx_motion_blur_params* p, bool fixed) {
   if (!t.on) return fail(ctx, RFX_ERR_NOT_READY, "set_motion_blur: the motion-blur stage shares the TRAA tail's pass, and the tail is off");
   if (fixed && (p != nullptr) != t.blur)
     return fail(ctx, RFX_ERR_UNSUPPORTED, "set_motion_blur: the chain is attached to a group, whose planes are fixed at attach time: the stage cannot be turned on or off");
   if (p && p->samples < 1) return fail(ctx, RFX_ERR_INVALID_ARG, "set_motion_blur: samples < 1");
-  if (p && !t.mid.buf[0].ptr) {
-    rfx_status st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, W, H, &t.mid.buf[0]);
-    if (st != RFX_OK) return st;
-    local_views(t.mid);
-  }
   t.blur = p != nullptr;
   if (p) t.blur_p = *p;
   return RFX_OK;
@@ -1185,7 +1178,7 @@ static rfx_status traa_set_fx(rfx_ctx* ctx, TraaTail& t, const rfx_effects_param
   t.fx = true;
   return RFX_OK;
 }
-// The end of a frame's tail, after its last pass (K9, the fused tail or the merged TRAA + motion-blur pass): the cosmetic stage's launch
+// The end of a frame's tail, after its last pass (K9 or the merged TRAA + motion-blur pass): the cosmetic stage's launch
 // when it is on.  The tail advances first: its TRAA planes are complete whatever the stage returns.
 static rfx_status tail_end(rfx_ctx* ctx, void* stream, TraaTail& t) {
   t.advance();
@@ -1317,8 +1310,7 @@ rfx_status rfx_ssgi_chain_enable_traa(rfx_ssgi_chain* ch, const rfx_traa_tail_op
   if (!ch) return RFX_ERR_INVALID_ARG;
   if (ch->group) return fail(ch->ctx, RFX_ERR_UNSUPPORTED, "chain_enable_traa: the chain is attached to a group, whose peer mappings are fixed at attach time");
   if (opt && ch->compose_on) return fail(ch->ctx, RFX_ERR_INVALID_ARG, "chain_enable_traa: the compose stage is on, and the tail runs K5 itself (turn the stage off first)");
-  const bool k5 = !ch->fastpath || ch->debug_view != RFX_DEBUG_VIEW_NONE;  // the fast chain's fused tail needs no K5 plane
-  return traa_enable(ch->ctx, ch->tail, opt, ch->opt.width, ch->opt.height, true, k5);
+  return traa_enable(ch->ctx, ch->tail, opt, ch->opt.width, ch->opt.height, true);
 }
 
 rfx_status rfx_ssgi_chain_set_compose(rfx_ssgi_chain* ch, const rfx_ssgi_compose_params* p) {
@@ -1349,7 +1341,7 @@ rfx_status rfx_ssgi_chain_set_compose(rfx_ssgi_chain* ch, const rfx_ssgi_compose
 
 rfx_status rfx_ssgi_chain_set_motion_blur(rfx_ssgi_chain* ch, const rfx_motion_blur_params* p) {
   if (!ch) return RFX_ERR_INVALID_ARG;
-  return traa_set_blur(ch->ctx, ch->tail, p, ch->group != nullptr, ch->opt.width, ch->opt.height);
+  return traa_set_blur(ch->ctx, ch->tail, p, ch->group != nullptr);
 }
 
 rfx_status rfx_ssgi_chain_set_effects(rfx_ssgi_chain* ch, const rfx_effects_params* p) {
@@ -1440,8 +1432,6 @@ rfx_status rfx_ssgi_chain_set_debug_view(rfx_ssgi_chain* ch, int32_t view) {
   rfx_status st = RFX_OK;
   if (ch->fastpath && plane && view >= RFX_DEBUG_VIEW_OUTPUT + 2) st = alloc_split_views(ch);
   if (st == RFX_OK && channel && !ch->debug_gb.ptr) st = rfx_plane_alloc(ctx, RFX_FMT_RGBA32F, ch->opt.width, ch->opt.height, &ch->debug_gb);
-  if (st == RFX_OK && view != RFX_DEBUG_VIEW_NONE && ch->tail.on && !ch->tail.mid.buf[0].ptr)  // the tail's K5 plane (the fused fast tail has none)
-    st = rfx_plane_alloc(ctx, RFX_FMT_RGBA16F, ch->opt.width, ch->opt.height, &ch->tail.mid.buf[0]);
   if (st != RFX_OK) return st;
   ch->debug_view = view;
   return RFX_OK;
@@ -1589,57 +1579,31 @@ static rfx_status stage_args(rfx_ssgi_chain* ch, const rfx_ssgi_frame* f, const 
   return RFX_OK;
 }
 
-// The TRAA tail (launch k of the frame): K5 of `composed` -> K2 in its TRAA form -> K9.  The fast chain runs the fused kernel over the
-// rows of launch k; every other chain runs the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS,
-// K2 on them +- 1).
+// The TRAA tail (launch k of the frame): K5 of `composed` (or with a debug view selected, K5 with isDebug of the view) -> K2 in its TRAA
+// form -> K9, as the three per-pass entry points on the rows each needs (K5 on the K9 rows +- RFX_TRAA_TAIL_ROWS, K2 on them +- 1).
 static rfx_status chain_render_tail(rfx_ssgi_chain* ch, void* stream, const rfx_ssgi_frame* f, const rfx_plane* composed, const uint32_t* ranges, uint32_t k) {
   rfx_ctx* ctx = ch->ctx;
-  const int W = (int)ch->opt.width, H = (int)ch->opt.height;
+  const int H = (int)ch->opt.height, halo = RFX_TRAA_TAIL_ROWS;
   const Rows kr = launch_rows(ranges, k, H);
   TraaTail& tail = ch->tail;
-  const rfx_temporal_params tp = traa_params(tail, ch->traa_tp, f->camera_moved);
-  const bool debug = ch->debug_view != RFX_DEBUG_VIEW_NONE;
   if (tail.fx) {  // the cosmetic stage: K9's plane into the stage's plane on launch k + 1's rows (the band; the tail runs on the rows it reads)
     const Rows fr = launch_rows(ranges, k + 1, H);
     tail.fx_job = {tail.out, *f->depth, *f->velocity, tail.fx_plane, fr.r0, fr.r1};
   }
-  // the fused kernel never writes the K5 plane, and the motion-blur stage samples all of it: with the stage on, the per-pass launches
-  // (which also measured faster than the fused tail at 4K, DESIGN.md §4)
-  if (ch->fastpath && !debug && !tail.blur) {
-    CTraaArgs a{};
-    TemporalArgs& t = a.t;
-    if (!pv(f->velocity, RFX_FMT_RGBA32F, t.velocity)) return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: velocity must be RGBA32F");
-    t.W = W; t.H = H; t.row0 = kr.r0; t.row1 = kr.r1;
-    temporal_uniforms(ctx, &tp, t);
-    t.input_half = 1; t.out_half = 1;
-    SsgiComposeArgs& c = a.k5;
-    if (!pv(f->depth, RFX_FMT_R32F, c.depth) || !pv(composed, RFX_FMT_RGBA32F, c.gi) || !pv(f->direct_light, RFX_FMT_RGBA16F, c.scene))
-      return fail(ctx, RFX_ERR_BAD_FORMAT, "chain: the TRAA tail needs an RGBA16F direct light plane");
-    if (c.scene.w != W || c.scene.h != H) return fail(ctx, RFX_ERR_SIZE_MISMATCH, "chain: the direct light plane must match the chain size");
-    c.W = W; c.H = H; c.row0 = 0; c.row1 = H;
-    compose_uniforms(tail.opt.compose, c);
-    a.hist = tail.acc.view[tail.cur() ^ 1];
-    a.acc = rov(tail.acc.buf[tail.cur()]);
-    a.out = rov(tail.out);
-    LAUNCHED(launch_ctraa(a, stream ? (cudaStream_t)stream : ctx->stream));
-  } else {
-    const int halo = RFX_TRAA_TAIL_ROWS;
-    rfx_status st = RFX_OK;
-    rfx_ssgi_compose_params q = tail.opt.compose;
-    const rfx_plane* view = composed;
-    if (debug && st == RFX_OK) {
-      q.is_debug = 1;
-      st = debug_view_plane(ch, stream, f, &view);
-    }
-    if (st == RFX_OK)
-      st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &tail.mid_w(), (uint32_t)std::max(0, kr.r0 - halo),
-                                   (uint32_t)std::min(H, kr.r1 + halo));
-    // the TRAA history rows live on their owners in a group of n > 1: the per-pass chain's peer forms, and the fast chain's tail when the
-    // motion-blur stage takes it off its fused kernel (which reads the history through the views itself)
-    if (st == RFX_OK) st = traa_launches(ctx, stream, tp, tail, f->velocity, ch->group_peer || tail.split, &tail.out, kr);
-    return st;  // the per-pass tail ends in traa_launches
+  rfx_status st = RFX_OK;
+  rfx_ssgi_compose_params q = tail.opt.compose;
+  const rfx_plane* view = composed;
+  if (ch->debug_view != RFX_DEBUG_VIEW_NONE) {
+    q.is_debug = 1;
+    st = debug_view_plane(ch, stream, f, &view);
   }
-  return tail_end(ctx, stream, tail);
+  if (st == RFX_OK)
+    st = rfx_ssgi_compose_launch(ctx, stream, &q, f->depth, view, f->direct_light, &tail.mid_w(), (uint32_t)std::max(0, kr.r0 - halo),
+                                 (uint32_t)std::min(H, kr.r1 + halo));
+  // in a group of n > 1 the TRAA history rows live on their owners, whichever chain kind renders the rest of the frame
+  const bool peer = ch->group && rfx_group_world(ch->group) > 1;
+  if (st == RFX_OK) st = traa_launches(ctx, stream, traa_params(tail, ch->traa_tp, f->camera_moved), tail, f->velocity, peer, &tail.out, kr);
+  return st;  // the tail ends in traa_launches
 }
 
 // 2-D TMA descriptor over a plane of 16-byte texels, addressed as rows of 4-byte elements (the box must pass cpoisson_tma_fits)
@@ -1982,7 +1946,7 @@ rfx_status rfx_ssgi_chain_submit_host(rfx_ssgi_chain* ch, const rfx_ssgi_host_fr
     const int cur = (int)(ch->frame_idx & 1);
     for (int q = 0; q < 2; q++)
       if (ch->dn_buf[q] == cur) CU(cudaStreamWaitEvent(ctx->stream, hp.ev_dn[q], 0));
-    // the tail (the launch after K4) writes its single-buffered image: it waits for the previous frame's D2H
+    // the tail (its launches after K4) writes the single-buffered image: it waits for the previous frame's D2H
     const uint32_t split = ch->tail.on ? 3u + 2u * (uint32_t)ch->opt.denoise_iterations : 0xffffffffu;
     if ((st = chain_render_impl(ch, nullptr, &f, nullptr, 0, split)) != RFX_OK) return st;
     if (ch->tail.on) {
@@ -2126,12 +2090,12 @@ rfx_status rfx_ao_chain_enable_traa(rfx_ao_chain* ch, const rfx_traa_tail_option
   static const rfx_ssgi_compose_params no_compose{};
   if (opt && memcmp(&opt->compose, &no_compose, sizeof no_compose) != 0)
     return fail(ctx, RFX_ERR_INVALID_ARG, "ao_chain_enable_traa: the AO tail has no K5: `compose` must be all zero");
-  return traa_enable(ctx, ch->tail, opt, ch->opt.width, ch->opt.height, false, true);
+  return traa_enable(ctx, ch->tail, opt, ch->opt.width, ch->opt.height, false);
 }
 
 rfx_status rfx_ao_chain_set_motion_blur(rfx_ao_chain* ch, const rfx_motion_blur_params* p) {
   if (!ch) return RFX_ERR_INVALID_ARG;
-  return traa_set_blur(ch->ctx, ch->tail, p, ch->group && rfx_group_world(ch->group) > 1, ch->opt.width, ch->opt.height);
+  return traa_set_blur(ch->ctx, ch->tail, p, ch->group && rfx_group_world(ch->group) > 1);
 }
 
 rfx_status rfx_ao_chain_set_effects(rfx_ao_chain* ch, const rfx_effects_params* p) {

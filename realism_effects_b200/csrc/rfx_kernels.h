@@ -139,7 +139,7 @@ RFX_D v4 ssgi_compose_lit(const SsgiComposeArgs& a, int x, int y, float depth, c
   }
   return mk4(c, 1.0f);
 }
-// K5 for pixel (x, y): the texel ssgi_compose_kernel stores (RGBA16F).  Shared with the fused TRAA tail (k_temporal.cu).
+// K5 for pixel (x, y): the texel ssgi_compose_kernel stores (RGBA16F)
 RFX_D v4 ssgi_compose_px(const SsgiComposeArgs& a, int x, int y) {
   if (a.is_debug) {  // ssgi_compose.frag:21-24
     const float4 t = ld_f4(a.gi, x, y);
@@ -193,18 +193,6 @@ struct TemporalPeer {
   PeerCarry carry;
 };
 cudaError_t launch_temporal_peer(const TemporalArgs& a, const TemporalPeer& p, cudaStream_t s);
-
-// TRAA frame tail of the fast chain (k_temporal.cu: ctraa_kernel): K5 -> K2 (TRAA form) -> K9 in one launch over rows [t.row0, t.row1).
-// `t` carries the TRAA K2 uniforms exactly as rfx_temporal_reproject_launch fills them (input_half = out_half = history_linear = 1,
-// texture_count 1, input_type DIFFUSE); `k5.gi` is `composed`, `k5.scene` the direct light; history rows live on their owners.
-struct CTraaArgs {
-  TemporalArgs t;
-  SsgiComposeArgs k5;
-  PeerPV hist;  // TRAA accumulated plane of the previous frame
-  OutV acc;     // TRAA accumulated plane of this frame
-  OutV out;     // K9 output
-};
-cudaError_t launch_ctraa(const CTraaArgs& a, cudaStream_t s);
 
 // ---- K1 ----------------------------------------------------------------------------------
 struct SsgiArgs {
@@ -290,7 +278,7 @@ struct TraaComposeArgs {
   int W, H, row0, row1;
 };
 cudaError_t launch_traa_compose(const TraaComposeArgs& a, cudaStream_t s);
-// LINEAR sampler of an RGBA16F plane in device memory; the fused TRAA tail has one with the same interface over shared memory
+// LINEAR sampler of an RGBA16F plane in device memory (motion_blur_px's taps)
 struct PlaneH4 {
   const PV& t;
   RFX_D v4 linear(v2 uv) const { return tex_h4_linear(t, uv); }
@@ -310,9 +298,8 @@ struct TraaMotionBlurArgs {
 };
 cudaError_t launch_traa_motion_blur(const TraaMotionBlurArgs& a, cudaStream_t s, const PeerPV* peer = nullptr);
 // K9 for pixel (x, y) of the W x H target (traa_compose.frag:3-6): the accumulated plane fetched LINEAR at the pixel centre, a = 1
-template <class S>
-RFX_D v4 traa_compose_px(const S& acc, int x, int y, int W, int H) {
-  const v4 t = acc.linear(pixel_uv(x, y, W, H));
+RFX_D v4 traa_compose_px(const PV& acc, int x, int y, int W, int H) {
+  const v4 t = tex_h4_linear(acc, pixel_uv(x, y, W, H));
   return mk4(t.x, t.y, t.z, 1.0f);
 }
 

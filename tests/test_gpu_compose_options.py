@@ -7,8 +7,7 @@ tests/test_compose_options_cpu.py, which also holds the oracle to the reference'
 * The fast chain's own K4 (c_compose in ccompose_kernel, cpoisson_kernel and cpoisson_tma_kernel) over 3 frames on the material-edge
   G-buffer, at 200x120 and on 3840x16 strips: each frame's output 0 against the oracle's compose of the chain's own outputs 4 and 5
   (dn0, dn1) over its last output 0, so no Poisson drift is carried in.
-The fused TRAA tail (ctraa_kernel, which shares ssgi_compose_px with ssgi_compose_kernel) runs with each K5 grid point as its
-compose options in tests/test_gpu_traa_tail.py."""
+The chain's TRAA tail runs with each K5 grid point as its compose options in tests/test_gpu_traa_tail.py."""
 from __future__ import annotations
 
 import os

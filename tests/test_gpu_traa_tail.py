@@ -1,7 +1,7 @@
 """GPU tests of the chain's TRAA frame tail (rfx_ssgi_chain_enable_traa): K5 ssgi_compose -> TRAA (K2 with textureCount 1, inputType
-"diffuse") -> K9 traa_compose rendered by the chain after K4.  The fast chain's fused kernel must write the bytes of the three per-pass
-launches, turning the tail on must not change outputs 0..5, the tail must follow the oracle (the passes pinned to the reference shaders),
-and a row-sharded group with the tail must equal one chain byte for byte."""
+"diffuse") -> K9 traa_compose rendered by the chain after K4.  The chain's tail must write the bytes of the three stand-alone launches on
+the chain's own `composed`, turning the tail on must not change outputs 0..5 and costs exactly those three launches, the tail must follow
+the oracle (the passes pinned to the reference shaders), and a row-sharded group with the tail must equal one chain byte for byte."""
 import os
 import socket
 
@@ -28,11 +28,11 @@ def _options(fog, cam_u):
     return abi.make_traa_tail_options(compose=ch.fog_params(cam_u, exp2=False) if fog else None)
 
 
-def _tail_equals_per_pass_sequence(ctx, inp, o, topt, name, reset_at=None, with_plain=False):
-    """Renders inp.frames with the fast chain's fused tail; every frame, outputs 6 / 7 == ssgi_compose -> temporal_reproject (TRAA form,
+def _tail_equals_stand_alone_launches(ctx, inp, o, topt, name, reset_at=None, with_plain=False):
+    """Renders inp.frames with the fast chain's tail; every frame, outputs 6 / 7 == ssgi_compose -> temporal_reproject (TRAA form,
     RGBA16F history, LINEAR) -> traa_compose launched one by one on the chain's own `composed`, byte for byte.  reset_at: the frame
-    before which the chain is reset.  with_plain: a chain without the tail runs alongside, and outputs 0..5 must be byte-identical.
-    Returns the last frame's output 6."""
+    before which the chain is reset.  with_plain: a chain without the tail runs alongside, outputs 0..5 must be byte-identical, and
+    a frame with the tail must launch exactly the three kernels of the tail more than one without it.  Returns the last frame's output 6."""
     from realism_effects_b200 import engine
 
     W, H = inp.width, inp.height
@@ -52,8 +52,10 @@ def _tail_equals_per_pass_sequence(ctx, inp, o, topt, name, reset_at=None, with_
                 keep = 0.0
             planes = [ctx.upload(fr[k]) for k in ("depth", "gbuffer", "velocity", "direct")]
             cam = abi.make_camera(fr["cam"])
+            n0 = ctx.launch_count
             chain.render(cam, *planes, fr["cam"]["position"], fr["moved"])
-            # the per-pass sequence on the chain's own `composed`
+            tail_launches = ctx.launch_count - n0
+            # the stand-alone launches on the chain's own `composed`
             ctx.ssgi_compose(planes[0], chain.output(0), planes[3], k5, params=topt.compose)
             tp = _traa_params(topt, fr["cam"], prev or fr["cam"], keep, fr["moved"])
             ctx.temporal_reproject(tp, k5, planes[2], acc[(t + 1) & 1], None, acc[t & 1], None)
@@ -64,7 +66,9 @@ def _tail_equals_per_pass_sequence(ctx, inp, o, topt, name, reset_at=None, with_
             assert got6.tobytes() == out.download().tobytes(), (name, t, "K9 output")
             assert np.isfinite(got6).all() and (got6[..., 3] == 1).all()
             if plain is not None:
+                n0 = ctx.launch_count
                 plain.render(cam, *planes, fr["cam"]["position"], fr["moved"])
+                assert tail_launches - (ctx.launch_count - n0) == 3, (name, t, "launches of the tail")
                 for which in range(6):
                     assert chain.download(which).tobytes() == plain.download(which).tobytes(), (name, t, which)
             for p in planes:
@@ -80,9 +84,10 @@ def _tail_equals_per_pass_sequence(ctx, inp, o, topt, name, reset_at=None, with_
 
 @pytest.mark.parametrize("size", [(320, 192), (3840, 2160)])
 @pytest.mark.parametrize("fog", [False, True])
-def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
-    """4 frames with history and a reset before frame 2: the fused tail writes the bytes of the per-pass sequence every frame.  At the
-    small size a chain without the tail runs alongside: outputs 0..5 are byte-identical with and without it."""
+def test_tail_writes_the_bytes_of_the_stand_alone_launches(built, size, fog):
+    """4 frames with history and a reset before frame 2: the chain's tail writes the bytes of the stand-alone launches every frame.  At
+    the small size a chain without the tail runs alongside: outputs 0..5 are byte-identical with and without it, and the tail adds
+    exactly its three launches."""
     from realism_effects_b200 import engine
 
     W, H = size
@@ -90,7 +95,7 @@ def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
     ctx = engine.Context(0, inp.blue)
     try:
         ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
-        got6 = _tail_equals_per_pass_sequence(ctx, inp, ch.Opts(denoise_iterations=1 if W > 1000 else 2), _options(fog, inp.frames[0]["cam"]),
+        got6 = _tail_equals_stand_alone_launches(ctx, inp, ch.Opts(denoise_iterations=1 if W > 1000 else 2), _options(fog, inp.frames[0]["cam"]),
                                               f"{size} fog={fog}", reset_at=2, with_plain=W < 1000)
         assert np.abs(got6[..., :3].astype(np.float32)).max() > 0.05
     finally:
@@ -98,17 +103,17 @@ def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence(built, size, fog):
 
 
 @pytest.mark.parametrize("case", K5_CASES, ids=str)
-def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence_across_k5_options(built, case):
+def test_tail_writes_the_bytes_of_the_stand_alone_launches_across_k5_options(built, case):
     """3 frames at each point of the SSGI compose grid (tests/test_compose_options_cpu.py: no fog, linear fog and FogExp2 with
-    perspective and orthographic cameras, isDebug, odd sizes and a 3840x16 strip) as the tail's compose options: the fused tail
-    (ctraa_kernel, which shares ssgi_compose_px with ssgi_compose_kernel) writes the bytes of the per-pass sequence every frame"""
+    perspective and orthographic cameras, isDebug, odd sizes and a 3840x16 strip) as the tail's compose options: the chain's tail
+    writes the bytes of the stand-alone launches every frame"""
     from realism_effects_b200 import engine
 
     inp = make_inputs(case.W, case.H, case.camera, frames=3)
     ctx = engine.Context(0, inp.blue)
     try:
         ctx.set_env(inp.env_map, inp.env_marginal, inp.env_conditional, inp.env_total)
-        _tail_equals_per_pass_sequence(ctx, inp, ch.Opts(), abi.make_traa_tail_options(compose=case.params(inp.frames[0]["cam"])), str(case))
+        _tail_equals_stand_alone_launches(ctx, inp, ch.Opts(), abi.make_traa_tail_options(compose=case.params(inp.frames[0]["cam"])), str(case))
     finally:
         ctx.close()
 
@@ -116,9 +121,9 @@ def test_fused_tail_writes_the_bytes_of_the_per_pass_sequence_across_k5_options(
 @pytest.mark.parametrize("kw", [dict(), dict(mode=abi.MODE_SSR), dict(fast_math=False)], ids=["fast", "ssr", "exact"])
 def test_tail_follows_the_oracle(built, kw):
     """The tail over 3 frames vs orc.ssgi_compose -> orc.temporal_reproject(out_half=True) -> orc.traa_compose on the ORACLE chain's
-    `composed`: within the bar tests/test_gpu_effects.py uses for TRAA (<= 2e-3 of the pixels outside 1e-3).  The fast chain runs the fused
-    kernel; SSR mode and fast_math off run the three per-pass launches.  With fast_math off every kernel of the chain and of the tail
-    (K5 -> K2 in TRAA form -> K9) is bit-equal to the oracle, so outputs 6 and 7 must equal it byte for byte."""
+    `composed`: within the bar tests/test_gpu_effects.py uses for TRAA (<= 2e-3 of the pixels outside 1e-3), for the fast chain, SSR mode
+    and fast_math off.  With fast_math off every kernel of the chain and of the tail (K5 -> K2 in TRAA form -> K9) is bit-equal to the
+    oracle, so outputs 6 and 7 must equal it byte for byte."""
     import orc
 
     from realism_effects_b200 import engine

@@ -4,7 +4,7 @@
     python tools/bench_fx_stage.py [--frames 100] [--warmup 10] [--width 3840 --height 2160]
 
 Two workloads, each as three chains timed with CUDA events on the context's stream in alternating blocks:
-  ssgi_c3   the SSGI + TRAA frame of tools/bench_traa.py (fast chain, denoiseIterations 2, fused tail);
+  ssgi_c3   the SSGI + TRAA frame of tools/bench_traa.py (fast chain, denoiseIterations 2, TRAA tail);
   ao_c4     the AO frame of tools/bench_ao_traa.py (K6 spp 8, iterations 1, K7, TRAA tail), and in-process groups of N = 2, 4, 8 bands with
             the stage (the members render one after the other on one card, so a group's frame is the sum of its members' kernel times and its
             ratio to the chain with the stage is the cost of sharding);

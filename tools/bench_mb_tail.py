@@ -4,8 +4,8 @@ one GPU.  Prints one JSON line with the card's name and power limit.
     python tools/bench_mb_tail.py [--frames 100] [--warmup 10] [--width 3840 --height 2160]
 
 Two workloads, each as two chains timed with CUDA events on the context's stream in alternating blocks:
-  ssgi_c3   the SSGI + TRAA frame of tools/bench_traa.py (fast chain, denoiseIterations 2): the tail (fused K5 -> K2 -> K9) against the tail
-            with the stage (per-pass K5 -> K2 -> the merged TRAA + motion-blur launch);
+  ssgi_c3   the SSGI + TRAA frame of tools/bench_traa.py (fast chain, denoiseIterations 2): the tail (K5 -> K2 -> K9) against the tail
+            with the stage (K5 -> K2 -> the merged TRAA + motion-blur launch);
   ao_c4     the AO frame of tools/bench_ao_traa.py (K6 spp 8, iterations 1, K7): the tail (K2 -> K9) against the tail with the stage, and
             in-process groups of N = 2, 4, 8 bands with the stage (two phases per frame; the members render one after the other on one card,
             so a group's frame is the sum of its members' kernel times and its ratio to the chain with the stage is the cost of sharding).

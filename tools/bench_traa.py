@@ -4,12 +4,11 @@ bench.py workload (synthetic scene, demo HDR environment, denoiseIterations 2). 
     python tools/bench_traa.py [--frames 100] [--warmup 10] [--width 3840 --height 2160]
     python -m torch.distributed.run --nproc_per_node N tools/bench_traa.py     # + C5: 7680 x 4320 row-sharded over N GPUs with the tail
 
-Three setups, each on its own chain, timed in alternating blocks in one process (CUDA events on the context's stream):
-  (a) the chain alone;  (b) the chain with the fused TRAA tail;  (c) the chain followed by the three per-pass tail launches
-  (ssgi_compose -> temporal_reproject in its TRAA form -> traa_compose).
-Reported: ms per frame of each, the tail's cost (b - a) and (c - a), Mpx/s of (b) with the 540 B/px algorithmic traffic of the frame
-(BASELINE.md: 432 for the chain, then K5, the 1-plane TRAA form of K2 and K9) and its share of the H100 SXM data-sheet 3.35 TB/s, the
-card's name and power limit, and whether (b) and (c) wrote identical bytes (K9 output and TRAA history) on the last frame."""
+Two setups, each on its own chain, timed in alternating blocks in one process (CUDA events on the context's stream):
+  (a) the chain alone;  (b) the chain with its TRAA tail (ssgi_compose -> temporal_reproject in its TRAA form -> traa_compose).
+Reported: ms per frame of each, the tail's cost (b - a), Mpx/s of (b) with the 540 B/px algorithmic traffic of the frame (BASELINE.md:
+432 for the chain, then K5, the 1-plane TRAA form of K2 and K9) and its share of the H100 SXM data-sheet 3.35 TB/s, and the card's name
+and power limit.  tests/test_gpu_traa_tail.py holds the tail's bytes to the stand-alone launches."""
 import argparse
 import json
 import os
@@ -37,36 +36,24 @@ def single_gpu(a) -> dict:
     stream = torch.cuda.ExternalStream(ctx.stream, device=torch.device("cuda", 0))
     copt = ch.chain_options(inp, o)
     topt = abi.make_traa_tail_options()
-    chains = {s: engine.SsgiChain(ctx, copt) for s in "abc"}
+    chains = {s: engine.SsgiChain(ctx, copt) for s in "ab"}
     chains["b"].enable_traa(topt)
     frames = [([ctx.upload(fr[k]) for k in ("depth", "gbuffer", "velocity", "direct")], abi.make_camera(fr["cam"]), fr) for fr in inp.frames]
-    k5, out = ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)
-    acc = [ctx.alloc(abi.FMT_RGBA16F, W, H), ctx.alloc(abi.FMT_RGBA16F, W, H)]
-    n = {s: 0 for s in "abc"}
-    state = {"keep": 0.0, "prev": None}
+    n = {s: 0 for s in "ab"}
 
     def step(s):
         planes, cam, fr = frames[n[s] % len(frames)]
-        moved = n[s] > 0
-        chains[s].render(cam, *planes, fr["cam"]["position"], moved)
-        if s == "c":
-            t = n[s]
-            ctx.ssgi_compose(planes[0], chains[s].output(0), planes[3], k5, params=topt.compose)
-            tp = ch.traa_temporal_params(cam, fr["cam"]["position"], state["prev"] or fr["cam"], state["keep"])
-            tp.full_accumulate = int(bool(topt.full_accumulate) and not moved)
-            ctx.temporal_reproject(tp, k5, planes[2], acc[(t + 1) & 1], None, acc[t & 1], None)
-            ctx.traa_compose(acc[t & 1], out)
-            state["keep"], state["prev"] = 1.0, fr["cam"]
+        chains[s].render(cam, *planes, fr["cam"]["position"], n[s] > 0)
         n[s] += 1
 
-    for s in "abc":
+    for s in "ab":
         for _ in range(a.warmup):
             step(s)
     ctx.sync()
     blocks = 4
-    ms = {s: 0.0 for s in "abc"}
-    for _ in range(blocks):  # alternate the setups so that clock and neighbour load drift hit all three alike
-        for s in "abc":
+    ms = {s: 0.0 for s in "ab"}
+    for _ in range(blocks):  # alternate the setups so that clock and neighbour load drift hit both alike
+        for s in "ab":
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record(stream)
             for _ in range(a.frames // blocks):
@@ -74,16 +61,12 @@ def single_gpu(a) -> dict:
             e1.record(stream)
             e1.synchronize()
             ms[s] += e0.elapsed_time(e1)
-    per = {s: ms[s] / (blocks * (a.frames // blocks)) for s in "abc"}
-    identical = (chains["b"].download(6).tobytes() == out.download().tobytes() and chains["b"].download(7).tobytes() == acc[(n["c"] - 1) & 1].download().tobytes()
-                 and n["b"] == n["c"])
+    per = {s: ms[s] / (blocks * (a.frames // blocks)) for s in "ab"}
     mpx = W * H / (per["b"] * 1e-3) / 1e6
     res = {"c3": {"workload": f"C3 as BASELINE.json defines it: SSGI (denoiseIterations 2) + TRAA at {W}x{H}, demo HDR env", "frames": blocks * (a.frames // blocks),
-                  "warmup": a.warmup, "ms_chain": round(per["a"], 4), "ms_chain_fused_tail": round(per["b"], 4), "ms_chain_per_pass_tail": round(per["c"], 4),
-                  "tail_ms_fused": round(per["b"] - per["a"], 4), "tail_ms_per_pass": round(per["c"] - per["a"], 4),
-                  "mpx_per_s_fused": round(mpx, 1), "algorithmic_bytes_per_px": BYTES_PER_PX,
-                  "algorithmic_share_of_3.35TBps": round(BYTES_PER_PX * W * H / (per["b"] * 1e-3) / HBM_PEAK, 4),
-                  "fused_equals_per_pass_last_frame": identical}}
+                  "warmup": a.warmup, "ms_chain": round(per["a"], 4), "ms_chain_with_tail": round(per["b"], 4), "tail_ms": round(per["b"] - per["a"], 4),
+                  "mpx_per_s": round(mpx, 1), "algorithmic_bytes_per_px": BYTES_PER_PX,
+                  "algorithmic_share_of_3.35TBps": round(BYTES_PER_PX * W * H / (per["b"] * 1e-3) / HBM_PEAK, 4)}}
     for c in chains.values():
         c.close()
     ctx.close()
@@ -91,7 +74,7 @@ def single_gpu(a) -> dict:
 
 
 def c5(a, rank, world) -> dict:
-    """7680 x 4320 row-sharded over `world` GPUs (one process each) with the fused tail: ms per frame of the slowest rank"""
+    """7680 x 4320 row-sharded over `world` GPUs (one process each) with the tail: ms per frame of the slowest rank"""
     import torch
     import torch.distributed as dist
 
